@@ -2,6 +2,7 @@
 """bench.py -- headline benchmark of the hot path (BASELINE.json metric: CTR forward+backward samples/sec).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--workload NAME] [--ids uniform|zipf]
+                    [--dump-outputs DIR]
 
 One "step" = one pass of the hot path over one batch.  Workloads (BASELINE.json `configs`):
   deepfm_cfg5          configs[4] on ONE GPU (default at N=1): DeepFM, 40 fields, embed_dim 32, batch 65536, 100 M-row
@@ -13,11 +14,15 @@ Prints ONE JSON line (rank 0).  Keys beyond the base contract:
   value        device-resident throughput (inputs already in HBM), CUDA-event timed, max over ranks
   e2e          same metric through the public autograd API with HOST (pinned) ids/labels: H2D copies, loss, D2H of the loss
                inside the timed region
-  roofline     achieved algorithmic GB/s (or TFLOP/s) of the dominant kernel vs MEASURED_PEAKS.json
+  roofline     achieved algorithmic GB/s (or TFLOP/s) of the dominant kernel vs the H100 SXM data-sheet peak (or
+               MEASURED_PEAKS.json when present)
   sustained    the same step looped for >= 2 s with the clock sampler running
   configs      (default line only) samples/s + roofline fraction of configs 2, 3, 4 from short runs in the same process
   cpu_baseline the restated reference (oracle port, torch CPU op-for-op) timed on this box's host cores
 --impl reference times that CPU restatement as the reference arm (TF 1.14 itself cannot be installed).
+--dump-outputs DIR   after the timed steps, writes what the last timed step computed (the arrays a caller of the hot path
+                     receives) as DIR/<name>.npy in float32; batch-sized arrays are cut to a fixed, seeded sample of samples.
+                     Inputs are seeded, so two builds run with the same arguments can be compared output for output.
 """
 from __future__ import annotations
 
@@ -62,11 +67,12 @@ def deepfm_config(workload, model, B, world, F, D, rows, ids_desc, NB):
                             else "single device, no exchange"),
             "l2": f"inputs larger than the last-level cache: {NB} rotating id batches over a {rows * F * D * 4 / 1e9:.1f} GB table; "
                   f"tile/d_tile/row_grads are {B * F * D * 4 / 1e6:.0f} MB each"}
-NVLINK_PEAK_GBS = 770.0       # B200_PROFILING.md: measured peer copy, per direction per GPU
+NVLINK_PEAK_GBS = 450.0       # H100 SXM data sheet: NVLink 4, 900 GB/s per GPU = 450 GB/s per direction (not measured)
 
 
 def measured_peaks():
-    d = {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "source": "fallback (B200_PROFILING.md)"}
+    d = {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0,
+         "source": "H100 SXM data sheet (700 W), dense; not measured"}
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         try:
@@ -91,21 +97,6 @@ def kernel_source_hash():
     for f in ("embed_fm2.cu", "ctr_common.cuh"):
         h.update(open(os.path.join(ROOT, "recalgorithm_b200", "csrc", f), "rb").read())
     return h.hexdigest()[:16]
-
-
-def measured_traffic(workload, ids_kind):
-    """DRAM bytes per launch of the gather from the committed ncu capture -- only while the kernel source still hashes to
-    what was profiled (ncu cannot run inside the bench); otherwise null + the reason."""
-    tp = os.path.join(ROOT, "profiles", "traffic.json")
-    try:
-        t = json.load(open(tp)).get(workload, {})
-    except Exception:
-        return None, "profiles/traffic.json missing"
-    if ids_kind != "uniform":
-        return None, "ncu capture was taken with uniform ids"
-    if t.get("kernel_source_sha256_16") != kernel_source_hash():
-        return None, f"stale: kernel source changed since {t.get('source', 'the capture')} (hash {t.get('kernel_source_sha256_16')} != {kernel_source_hash()})"
-    return t.get("embed_fm2_fwd_dram_bytes_per_launch"), t.get("source")
 
 
 class ClockSampler:
@@ -528,11 +519,11 @@ def run_deepfm(args, cfg, dd: Dist):
             ops.embed_fm2_bwd(tile, d_tile, d_fm2, row_grads=row_grads)
             if ev:
                 ev[2].record()
-        return tables, rows, id_sets, ids_desc, step
+        return tables, rows, id_sets, ids_desc, step, row_grads
 
     if not sharded_mode:
         # ------------------------------------------------------------------ one GPU (or N replicas, no exchange step)
-        tables, rows, id_sets, ids_desc, step = replica_setup()
+        tables, rows, id_sets, ids_desc, step, row_grads = replica_setup()
         for i in range(args.warmup):
             step(i)
         dd.barrier()
@@ -541,6 +532,8 @@ def run_deepfm(args, cfg, dd: Dist):
         ms_total, (fwd_ms, bwd_ms) = timed_steps(dd, step, args.steps, n_marks=2)
         clocks = sampler.stop()
         launches = _lib.kernel_launches() - launches0
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, {"tile": tile, "fm2": fm2, "row_grads": row_grads})
         value = world * B * args.steps / (ms_total * 1e-3)
         sustained = sustained_run(dd, step, ms_total / args.steps, B)
 
@@ -583,7 +576,7 @@ def run_deepfm(args, cfg, dd: Dist):
         ach_fwd = fwd_b * B / (fwd_ms * 1e-3) / 1e9
         ach_bwd = bwd_b * B / (bwd_ms * 1e-3) / 1e9
         ach_step = (fwd_b + bwd_b) * B * args.steps / (ms_total * 1e-3) / 1e9
-        traffic, traffic_src = measured_traffic(args.workload, args.ids)
+        traffic, traffic_src = None, "not measured: DRAM traffic needs an Nsight Compute capture, which the bench does not take"
         hbm = peaks["hbm_gbs"]
         line = {
             "metric": "ctr_fwd_bwd_samples_per_sec", "value": value, "unit": "samples/s", "n_gpus": world,
@@ -612,7 +605,7 @@ def run_deepfm(args, cfg, dd: Dist):
             "gpu_launches": int(launches), "clocks": clocks,
         }
         if world == 1 and not args.no_extra and args.ids == "uniform":
-            # the same step on Zipf(1.05) ids (SURVEY 8d's second case): hot rows are served by the 126 MB L2, so the
+            # the same step on Zipf(1.05) ids (SURVEY 8d's second case): hot rows are served by the 50 MB L2, so the
             # algorithmic rate may exceed the HBM peak -- reported beside the uniform (L2-miss) headline, never instead of it
             zargs = argparse.Namespace(**{**vars(args), "ids": "zipf"})
             zsets, zdesc = make_ids(zargs, rows, B, F, NB, dev, gen)
@@ -699,6 +692,8 @@ def run_deepfm(args, cfg, dd: Dist):
     ms_total, (plan_ms, fwd_ms, push_ms) = timed_steps(dd, step, args.steps, n_marks=3)
     clocks = sampler.stop()
     launches = _lib.kernel_launches() - launches0
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"tile": tile, "fm2": fm2})          # the pushed gradient rows live in the owners' queues
     tables.finish_push()                                                # raises if a receive queue overflowed
     value = world * B * args.steps / (ms_total * 1e-3)
     per_rank = {"plan_ms": dd.gather(plan_ms), "pull_ms": dd.gather(fwd_ms), "bwd_push_ms": dd.gather(push_ms)}
@@ -764,7 +759,7 @@ def run_deepfm(args, cfg, dd: Dist):
     # the zero-traffic split of the same batch (replicated 12.8 GB table) for comparison -- NOT the headline at N > 1
     rep = None
     if not args.no_extra:
-        _t, _rows, _ids, _desc, rstep = replica_setup()
+        _t, _rows, _ids, _desc, rstep, _rg = replica_setup()
         for i in range(3):
             rstep(i)
         rms, _ = timed_steps(dd, rstep, min(args.steps, 50))
@@ -799,15 +794,14 @@ def run_deepfm(args, cfg, dd: Dist):
         "roofline": {"bound": "nvlink", "kernel": "embed_fm2_fwd_kernel<8,sharded> (peer-pull gather + FM2)",
                      "achieved": nv_bytes / (fwd_ms * 1e-3) / 1e9, "peak": NVLINK_PEAK_GBS, "unit": "GB/s",
                      "frac": nv_bytes / (fwd_ms * 1e-3) / 1e9 / NVLINK_PEAK_GBS, "traffic": None,
-                     "peak_source": "B200_PROFILING.md: measured peer copy 770 GB/s per direction per GPU",
+                     "peak_source": "H100 SXM data sheet: NVLink 4, 450 GB/s per direction per GPU (not measured)",
                      "nvlink_bytes_per_direction_per_rank": nv_bytes, "avg_launch_ms": fwd_ms,
                      "push": {"kernel": "embed_fm2_bwd_push_kernel<8,12> (backward fused with the gradient exchange)",
                               "achieved": nv_bytes / (push_ms * 1e-3) / 1e9, "frac": nv_bytes / (push_ms * 1e-3) / 1e9 / NVLINK_PEAK_GBS,
                               "avg_launch_ms": push_ms},
                      "plan_ms": plan_ms, "per_rank_pull_GBps": pull_gbs, "per_rank_push_GBps": push_gbs,
                      "step_bound_ms": bound_ms, "step_frac_of_bound": bound_ms / (ms_total / args.steps),
-                     "bound_terms_ms": {"pull_nvlink": pull_nv_ms, "pull_hbm": pull_hbm_ms, "push_nvlink": pull_nv_ms, "push_hbm": push_hbm_ms},
-                     "link_ceiling_note": "tools/peerbench.cu (all ranks active, 128 B rows): pull tops out at ~650 GB/s, push at ~690 GB/s"},
+                     "bound_terms_ms": {"pull_nvlink": pull_nv_ms, "pull_hbm": pull_hbm_ms, "push_nvlink": pull_nv_ms, "push_hbm": push_hbm_ms}},
         "sustained": sustained,
         "e2e": {"value": e2e_value, "unit": "samples/s", "h2d_bytes_per_step": B * F * 4 + B * 4, "d2h_bytes_per_step": 4,
                 "steps": e2e_steps, "ms_per_step": e2e_ms / e2e_steps, "loss_last": losses[-1], "launch": e2e_mode, "eager": e2e_eager,
@@ -823,11 +817,11 @@ def run_deepfm(args, cfg, dd: Dist):
 # ----------------------------------------------------------------------------------------------------
 # configs 2, 3, 4: lookup + interaction layer chains
 # ----------------------------------------------------------------------------------------------------
-def layer_workload_measure(dd: Dist, name, steps, warmup, brief=False):
+def layer_workload_measure(dd: Dist, name, steps, warmup, brief=False, dump_dir=None):
     from tools import workloads as W
     peaks = measured_peaks()
     wl = W.BUILDERS[name]()
-    flush = torch.empty(64 * 1024 * 1024, device=dd.dev)      # 256 MB: these working sets fit the 126 MB L2, flush it every step
+    flush = torch.empty(64 * 1024 * 1024, device=dd.dev)      # 256 MB written before every step: flushes the 50 MB L2
     marks = wl["marks"]
 
     def step(i, ev=None):
@@ -842,6 +836,8 @@ def layer_workload_measure(dd: Dist, name, steps, warmup, brief=False):
     for i in range(steps):
         step(i, evs[i])
     dd.barrier()
+    if dump_dir and dd.rank == 0:
+        dump_outputs(dump_dir, wl["outputs"])             # the last timed eager step, before any graph replay below
     per = {m: statistics.mean(e[j].elapsed_time(e[j + 1]) for e in evs) for j, m in enumerate(marks)}
     ms_step = dd.max(statistics.mean(e[0].elapsed_time(e[-1]) for e in evs))
     out = {"value": dd.world * wl["B"] / (ms_step * 1e-3), "unit": "samples/s", "ms_per_step": ms_step, "stage_ms": per,
@@ -866,11 +862,25 @@ def layer_workload_measure(dd: Dist, name, steps, warmup, brief=False):
     return out, wl
 
 
+def dump_outputs(out_dir, arrays, max_rows=2048):
+    """--dump-outputs: each tensor as <out_dir>/<name>.npy in float32.  Tensors with more than `max_rows` rows keep a fixed,
+    seeded sample of rows (the same rows in every run), so that the files stay small (2048 x 40 x 32 floats = 10.5 MB)."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    torch.cuda.synchronize()
+    for name, t in arrays.items():
+        t = t.detach()
+        if t.shape[0] > max_rows:
+            rows = torch.randperm(t.shape[0], generator=torch.Generator().manual_seed(0))[:max_rows].sort().values
+            t = t[rows.to(t.device)]
+        np.save(os.path.join(out_dir, name + ".npy"), t.float().cpu().numpy())
+
+
 def run_layer_workload(args, dd: Dist):
     from recalgorithm_b200 import _lib
     sampler = ClockSampler(dd.local if dd.world > 1 else 0).start()
     n0 = _lib.kernel_launches()
-    res, wl = layer_workload_measure(dd, args.workload, args.steps, args.warmup)
+    res, wl = layer_workload_measure(dd, args.workload, args.steps, args.warmup, dump_dir=args.dump_outputs)
     launches = _lib.kernel_launches() - n0
     clocks = sampler.stop()
     sustained = sustained_run(dd, lambda i, ev=None: wl["step"](None), res["ms_per_step"], wl["B"])
@@ -910,6 +920,8 @@ def main():
                     help="sharded workloads: 1 = also time the e2e step as a CUDA-graph replay and report the faster form")
     ap.add_argument("--ids", default="uniform", choices=["uniform", "zipf"],
                     help="id distribution of the synthetic batches (default: uniform = every row an HBM miss)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="write what the last timed step computed as DIR/<name>.npy (float32, a seeded sample of large arrays)")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     world = int(os.environ.get("WORLD_SIZE", "1"))

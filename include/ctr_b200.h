@@ -1,7 +1,7 @@
-/* ctr_b200.h -- C ABI of the Blackwell-native CTR feature-interaction engine (libctr_b200.so).
+/* ctr_b200.h -- C ABI of the Hopper-native (sm_90a) CTR feature-interaction engine (libctr_b200.so).
  *
  * Drop-in boundary for the hot path of tangxyw/RecAlgorithm (reference paths below are relative to
- * /root/reference/algorithm).  The reference has no FFI of its own -- its boundary is Python
+ * the reference's algorithm/ directory).  The reference has no FFI of its own -- its boundary is Python
  * callables invoked while a TF1 graph is built (SURVEY.md section 8b) -- so each entry point here
  * names the reference callable whose forward / autodiff-backward it replaces.  The Python side
  * (recalgorithm_b200/layers.py) re-exposes them under the reference's own signatures.
@@ -13,7 +13,7 @@
  *   - the CALLER owns every buffer; kernels never allocate, never synchronise, and are re-entrant
  *     across streams.  Where a workspace is needed there is a *_workspace_bytes() query;
  *   - all tensors are dense row-major fp32 unless stated; ids / offsets / lengths are int64;
- *   - there is no CPU fallback: on a machine without an sm_100 GPU every compute entry point fails
+ *   - there is no CPU fallback: on a machine without an sm_90 GPU every compute entry point fails
  *     with CTR_ERR_CUDA.
  */
 #ifndef CTR_B200_H_
@@ -272,10 +272,6 @@ int ctr_cin_bwd(const float* x0, const float* xk, const float* filter, const flo
                 float* dx0, float* dxk, float* dfilter,
                 void* workspace, int64_t workspace_bytes, void* stream);
 int64_t ctr_cin_bwd_workspace_bytes(int64_t B, int64_t m, int64_t hk, int64_t D, int64_t H);
-/* Tuning hook (process-wide, returns the previous setting): 1 (default) = the dX kernel runs as CTA pairs (tcgen05
- * cta_group::2, M = 256, each SM feeds half of every filter stage); 0 = the single-CTA form with TMA multicast.  Same results;
- * used by tools/bench_layers.py for A/B timings. */
-int ctr_cin_bwd_set_dx_pair(int on);
 
 /* ---- Row DIN-ATT: DIN attention unit -----------------------------------------------------------------
  * Replaces din_attention(query, keys, keys_length, is_softmax) (DIN/din_attention.py:17-43).

@@ -1,7 +1,7 @@
 """NumPy restatement of the reference hot path (TEST INFRASTRUCTURE -- see oracle/__init__.py).
 
 Every function follows the reference file:line it cites (paths relative to
-/root/reference/algorithm).  Arithmetic runs in the dtype of the inputs: float32 mirrors
+the reference's algorithm/ directory).  Arithmetic runs in the dtype of the inputs: float32 mirrors
 the reference's TF1 CPU graph, float64 is the high-precision anchor the fp32 results are
 themselves checked against.  Forward functions mirror the reference op-for-op (including
 its quirks); backward functions are the analytic gradients of those forwards and are

@@ -1,10 +1,10 @@
 """Generate tests/golden/*.npz by EXECUTING THE REFERENCE'S OWN LAYER FILES (TEST INFRASTRUCTURE).
 
-Run in the build container only (needs /root/reference):
+Needs a checkout of the reference project (its ``algorithm`` directory):
 
-    python oracle/make_golden.py
+    python oracle/make_golden.py /path/to/RecAlgorithm/algorithm
 
-The five interaction-layer files are imported verbatim from /root/reference/algorithm with
+The five interaction-layer files are imported verbatim from that directory with
 ``oracle/tf1_shim`` standing in for TensorFlow 1.14 (see that package's docstring for what
 this does and does not pin).  Each fixture stores the seeded inputs, the injected weights
 (under the TF variable names the reference created), and the reference outputs computed in
@@ -12,7 +12,8 @@ float32 (like the reference) and float64 (anchor).  FM2 and the lookup have no i
 reference function (inline code / TF-internal); their fixtures come from
 ``oracle/layers_np.py`` and are marked ``source='restated'``.
 
-The GPU box has no /root/reference: tests read only the committed .npz files.
+Tests read only the committed .npz files; tests/golden/reference_digests.json holds the SHA-256 of every array of a
+run of this script over the reference, so that the fixtures stay pinned to it without the checkout.
 """
 from __future__ import annotations
 
@@ -24,7 +25,7 @@ import numpy as np
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-REF = "/root/reference/algorithm"
+REF = os.environ.get("RECALG_REFERENCE", "")          # the reference's algorithm/ directory (argv[1] wins)
 OUT = os.path.join(ROOT, "tests", "golden")
 
 sys.path.insert(0, os.path.join(HERE, "tf1_shim"))
@@ -77,7 +78,7 @@ def run_both(fn, variables):
 def save(name, **arrays):
     os.makedirs(OUT, exist_ok=True)
     path = os.path.join(OUT, name + ".npz")
-    np.savez(path, **arrays)
+    np.savez_compressed(path, **arrays)
     print(f"{name}: {os.path.getsize(path) / 1024:.0f} KiB")
 
 
@@ -108,7 +109,7 @@ def gen_cross():
 
 def gen_cin():
     rng = np.random.default_rng(2345)
-    for m, D, maps, B in ((8, 8, ("50", "50", "50"), 4), (30, 16, ("128", "128"), 3), (8, 16, ("17",), 5)):
+    for m, D, maps, B in ((8, 8, ("50", "50", "50"), 4), (10, 16, ("128", "128"), 3), (8, 16, ("17",), 5)):
         x0 = trunc_normal(rng, (B, m, D), 1.0 / np.sqrt(D))
         variables, hk = {}, m
         for i, h in enumerate(maps):
@@ -173,7 +174,7 @@ def gen_din():
 
 def gen_fibinet():
     rng = np.random.default_rng(4567)
-    for F, K, ratio, B in ((8, 8, 2, 5), (30, 16, 2, 3)):
+    for F, K, ratio, B in ((8, 8, 2, 5), (30, 16, 2, 2)):
         x = trunc_normal(rng, (B, F, K), 1.0 / np.sqrt(K))
         r = K // ratio
         variables = {"senet_part/senet_w1": glorot(rng, (F, r)), "senet_part/senet_w2": glorot(rng, (r, F))}
@@ -235,7 +236,7 @@ def gen_restated():
          source="restated:TF1.14 feature_column semantics (SURVEY A.4-A.6) -- parity unpinned")
 
 
-# ---- inline blocks of model_fns: the cited source lines are read from /root/reference at generation time and exec()'d ----
+# ---- inline blocks of model_fns: the cited source lines are read from the reference checkout at generation time and exec()'d ----
 
 class _FakeFC:
     """Stand-in for `tf.feature_column` inside the inline blocks: `fc.input_layer(features, [col])` returns the (B, K)
@@ -364,6 +365,9 @@ def gen_ffm():
 
 
 if __name__ == "__main__":
+    if len(sys.argv) > 1:
+        REF = sys.argv[1]
+    assert os.path.isdir(REF), "usage: make_golden.py <reference checkout>/algorithm (or set RECALG_REFERENCE)"
     gen_cross()
     gen_cin()
     gen_din()

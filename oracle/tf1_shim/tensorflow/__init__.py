@@ -8,14 +8,14 @@ package first on ``sys.path`` lets ``oracle/make_golden.py`` import and run
     DCN/cross_layer.py, xDeepFM/cin_layer.py, DIN/din_attention.py,
     FiBiNET/senet.py, FiBiNET/bilinear_interaction_layer.py
 
-*verbatim from /root/reference* (nothing is copied), eagerly, on injected weights, so the
+*verbatim from the reference checkout* (nothing is copied), eagerly, on injected weights, so the
 reference's own control flow -- loop bounds, pair enumeration, mask/where/scale order,
 reshape index order, variable shapes -- is what produces the golden vectors.  What is NOT
 pinned by this is the arithmetic inside each TF primitive (Eigen summation order etc.);
 each primitive below states the public TF 1.14 semantics it implements.
 
 The same shim also runs the INLINE interaction blocks of DeepFM/NFM/FwFM/AFM model_fns: make_golden.py reads the
-cited line ranges from /root/reference at generation time and exec()s them with a stand-in ``fc.input_layer``.
+cited line ranges from the reference checkout at generation time and exec()s them with a stand-in ``fc.input_layer``.
 
 Only what those files touch is implemented.  Everything evaluates eagerly on
 ``numpy`` arrays in ``_STATE.dtype`` (float32 like the reference, or float64 for the

@@ -1,4 +1,4 @@
-"""recalgorithm_b200 -- Blackwell-native (sm_100a) hot path of tangxyw/RecAlgorithm.
+"""recalgorithm_b200 -- Hopper-native (sm_90a, H100) hot path of tangxyw/RecAlgorithm.
 
 Only the path named in BASELINE.json lives here: the per-field embedding lookup and the
 feature-interaction layers (FM2, cross, CIN, DIN attention, SENET/bilinear), as hand-written CUDA

@@ -80,7 +80,6 @@ SIGNATURES = {
     "ctr_cin_fwd": (c_int, [_P, _P, _P, _I, _I, _I, _I, _I, _P, _P, c_int, _P, _I, _P]),
     "ctr_cin_bwd": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _I, _P]),
     "ctr_cin_bwd_workspace_bytes": (c_int64, [_I, _I, _I, _I, _I]),
-    "ctr_cin_bwd_set_dx_pair": (c_int, [c_int]),
     "ctr_din_attention_fwd": (c_int, [_P] * 9 + [_I, _I, _I, c_int, _P, _P, _P, _P]),
     "ctr_din_attention_bwd": (c_int, [_P] * 11 + [_I, _I, _I, c_int, _P, _P, _P, _P, _P]),
     "ctr_senet_fwd": (c_int, [_P, _P, _P, _I, _I, _I, _I, _P, _P]),

@@ -1,4 +1,4 @@
-"""In-tree build of the sm_100a CUDA library (nvcc cross-compiles without a GPU)."""
+"""In-tree build of the sm_90a (H100) CUDA library (nvcc cross-compiles without a GPU)."""
 from __future__ import annotations
 
 import os

@@ -8,7 +8,7 @@
 // i.e. plain Adam on the densified gradient: every row of the table moves every step.  DIEN alone uses LazyAdam
 // (DIEN/dien.py:328): only the referenced rows are touched.
 //
-// B200 mapping (pure HBM streaming, no tensor cores): the caller de-duplicates rows and sums their values (one
+// H100 mapping (pure HBM streaming, no tensor cores): the caller de-duplicates rows and sums their values (one
 // ctr_rows_scatter_add into a compact buffer); then
 //   ctr_adam_rows        updates m, v, var of the U referenced rows and marks them in a bitmap   (both variants)
 //   ctr_adam_dense_rest  streams over ALL other rows with g = 0: m*=b1, v*=b2, var -= lr_t*m/(sqrt(v)+eps)   (TF variant only)

@@ -5,21 +5,21 @@
 //   (1, hk*m, hk_1) filter == matmul over the last axis; transpose -> (B, hk_1, D).  The reference
 //   materialises the (B, D, hk*m) outer tensor (2 GB at BASELINE config 3, layer 2).
 //
-// B200 mapping -- the one genuinely dense contraction of the hot path, so it runs on the 5th-gen tensor cores:
+// H100 mapping -- the one genuinely dense contraction of the hot path, so it runs on the tensor cores (wgmma):
 //   GEMM view  C[M x N] = A[M x K] . B[K x N],  M = B*D rows r = (b,d),  K = hk*m,  N = hk_1.
-//   * A (the outer product) is never written to HBM: 256 producer threads each own one row r, keep the row's
-//     x0[b,:,d] (m <= 32 values) in registers and, for every K-block i, form the 32 products xk[b,i,d]*x0[b,j,d],
-//     and store them straight into shared memory in the UMMA canonical K-major SWIZZLE_128B layout
+//   * A (the outer product) is never written anywhere: it is formed in registers, directly in the wgmma A-fragment
+//     layout.  Each thread of a consumer warpgroup owns two rows r of the 64-row warpgroup tile, keeps the x0 values of
+//     its fragment columns in registers and, for every K-block i, multiplies them by xk[b,i,d]
 //     (K is re-ordered as i*32 + j, zero padded from m to 32, so one K-block == one i == one 128-byte swizzle row);
 //   * B (the filter) is pre-transposed/padded once per call into that K order (workspace) and streamed by TMA
-//     (cp.async.bulk.tensor, SWIZZLE_128B) through an mbarrier pipeline;
-//   * one elected thread issues tcgen05.mma (kind::tf32, M=128, N=hk_1 padded to 16, K=8); accumulators live in
-//     TMEM (2 M-tiles x N columns per CTA so that every B stage is used twice); tcgen05.commit releases stages;
+//     (cp.async.bulk.tensor, SWIZZLE_128B) through an mbarrier pipeline shared by the CTA's two consumer warpgroups;
+//   * wgmma.mma_async m64nNk8 kind tf32 (A from registers, B from shared memory, N = hk_1 padded to 32/64/128),
+//     fp32 accumulators in registers;
 //   * fp32-class accuracy (north_star: 1e-5) comes from the 3xTF32 split  A.B ~= Ahi.Bhi + Alo.Bhi + Ahi.Blo
-//     with fp32 accumulation in TMEM (error ~2^-22 per product); precision=1 runs a single TF32 pass (~1e-3);
-//   * epilogue: tcgen05.ld -> registers -> (B, hk_1, D) stores + the pooled sum over D by warp shuffles.
+//     with fp32 accumulation (error ~2^-22 per product); precision=1 runs a single TF32 pass (~1e-3);
+//   * epilogue: accumulators -> shared memory -> (B, hk_1, D) stores + the pooled sum over D.
 //   Shapes outside the tensor path's limits (m > 32, hk_1 > 128, D not a power of two <= 32) use a plain
-//   CUDA-core kernel.  The backward pass is CUDA-core in this revision (see DESIGN.md: next step).
+//   CUDA-core kernel.  The backward pass is in cin_bwd.cu.
 #include <stdlib.h>
 
 #include "tc_ptx.cuh"
@@ -28,23 +28,17 @@ namespace ctr {
 namespace cin {
 using namespace ctr::tc;
 
-constexpr int TILES = 2;                 // M tiles per CTA
-constexpr int KB = 32;                   // tf32 per K-block (128 B == swizzle span)
-constexpr int NTHREADS = 384;            // 3 warpgroups: 8 producer/drain warps, then TMA warp + MMA warp (+2 idle)
+constexpr int KB = 32;                    // tf32 per K-block (128 B == swizzle span)
+constexpr int NWG = 2;                    // consumer warpgroups per CTA, 64 rows each
+constexpr int TILE_M = NWG * WG_M;        // rows per CTA tile
+constexpr int NTHREADS = (NWG + 1) * 128;  // + one producer warpgroup (one TMA thread)
+constexpr int EPI_LD = WG_M + 4;          // row stride (floats) of the epilogue staging: conflict-free fragment stores
 
-struct FwdSmem {
-  int stage_bytes, a_bytes_per_tile, b_tile_bytes, bar_off, total;
-};
-__host__ __device__ inline FwdSmem fwd_smem(int NP, int passes, int stages) {
-  FwdSmem s;
-  const int na = passes == 3 ? 2 : 1;
-  s.a_bytes_per_tile = 0;                         // A lives in TMEM (TS-mode MMA)
-  s.b_tile_bytes = NP * 128;
-  s.stage_bytes = na * s.b_tile_bytes;
-  s.bar_off = stages * s.stage_bytes;
-  s.total = s.bar_off + 8 * (2 * stages + 2 * 8 + 2) + 16;
-  return s;
+__host__ __device__ inline int fwd_smem_bytes(int N, int passes, int stages) {
+  return stages * (passes == 3 ? 2 : 1) * N * 128 + NWG * N * EPI_LD * 4 + 8 * 2 * stages;
 }
+// wgmma N of the tensor path: hk_1 padded to 32, 64 or 128 (also the row count of the split filter)
+static inline int npad(int64_t H) { return H <= 32 ? 32 : H <= 64 ? 64 : 128; }
 
 // ------------------------------------------------------------------------------------------------ kernels
 // filter (hk*m, H) -> Wt[2][NP][KP]: [0] = tf32-rounded value, [1] = residual; K order i*32 + j, zero padded.
@@ -62,270 +56,154 @@ __global__ void cin_split_filter_kernel(const float* __restrict__ w, float* __re
   }
 }
 
-// One halving-butterfly step of the sum over the D lanes of a sample: lanes whose bit `o` is clear keep the lower
-// HALF columns, the others the upper HALF; returns the column offset this lane now owns.
-template <int N, int HALF>
-__device__ __forceinline__ int bfly_step(float (&acc)[N], int lane, int o) {
-  const bool up = (lane & o) != 0;
-#pragma unroll
-  for (int q = 0; q < HALF; ++q) {
-    const float keep = up ? acc[q + HALF] : acc[q];
-    const float send = up ? acc[q] : acc[q + HALF];
-    acc[q] = keep + __shfl_xor_sync(0xffffffffu, send, o);
-  }
-  return up ? HALF : 0;
-}
-
-// Accumulation note: the tensor core adds each K=8 product group into the fp32 TMEM accumulator with truncation,
-// so a long accumulation chain drifts by ~0.5 ulp per MMA (measured 3.8e-5 after 1440 MMAs at K = 3840 x 3 passes).
-// The K loop is therefore cut into chunks of `chunk` K-blocks: each chunk accumulates from zero in TMEM and the
-// row-owning threads add the finished chunk into fp32 registers (round-to-nearest).
+// Accumulation note: the tensor core adds each K=8 product group into the fp32 accumulator with truncation, so a long
+// accumulation chain drifts by ~0.5 ulp per MMA.  The K loop is therefore cut into chunks of `chunk` K-blocks: each chunk
+// accumulates from zero and is then added into a second set of fp32 registers (round-to-nearest).
 //
-// Operand placement (second revision): the first version staged A in shared memory; ncu showed it bound by shared
-// memory bandwidth (producer stores + tensor-core operand reads + TMA writes > 128 B/clk) with the proxy fence as the
-// top producer stall.  A now goes registers -> TMEM (tcgen05.st; the row-owning thread IS the TMEM lane) and the MMA
-// runs in TS mode (A from TMEM, B from shared memory), so shared memory only carries the filter tiles.
-//   TMEM columns: [0, TILES*NP) accumulators | [256, 512) A staging: stage sa, tile t at 256 + (sa*TILES + t)*32*NA (+32 = lo)
-// Work items of the persistent forward kernel.  A CTA normally processes PAIRS of 128-row M-tiles (both share every filter
-// stage); with n128 tiles and G CTAs that quantises to ceil(n128 / 2G) rounds (config 3: 3.46 -> 4 rounds, 13 % idle).
-// The last round therefore hands out what is left as evenly as possible: full pairs to the first CTAs, SINGLE tiles to
-// the rest (the second M-tile's warps then only keep the barriers in phase), so the tail costs half a round when it can.
-struct FwdItem { int tile0, nt; };                   // first 128-row tile, number of M-tiles (0: nothing for this CTA)
-__device__ __forceinline__ int fwd_num_items(int n128) {
-  const int G = (int)gridDim.x, R = (n128 / 2) / G;
-  return R + (n128 - 2 * R * G > 0 ? 1 : 0);
-}
-__device__ __forceinline__ FwdItem fwd_item(int it, int n128) {
-  const int G = (int)gridDim.x, c = (int)blockIdx.x, R = (n128 / 2) / G;
-  if (it < R) return FwdItem{2 * (c + it * G), 2};
-  const int base = 2 * R * G, rem = n128 - base;      // 0 < rem < 2G
-  if (rem <= G) return FwdItem{base + c, c < rem ? 1 : 0};
-  const int x = rem - G;                              // CTAs that still get a pair
-  return c < x ? FwdItem{base + 2 * c, 2} : FwdItem{base + 2 * x + (c - x), 1};
-}
-
-template <int PASSES, int SB, int NPT>
+// Persistent CTAs walk 128-row tiles (two warpgroups x 64 rows); both warpgroups consume every filter stage, a stage is
+// released when all eight consumer warps have passed the wgmma.wait that covers it.  While one warpgroup waits for its
+// K-block, the other issues its own, and the TMA warp keeps SB stages in flight.
+template <int PASSES, int SB, int N>
 __global__ void __launch_bounds__(NTHREADS, 1)
 cin_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmap_w, const float* __restrict__ x0,
                   const float* __restrict__ xk, float* __restrict__ out, float* __restrict__ pooled, int B, int m,
-                  int hk, int logD, int H, int NP, int chunk) {
+                  int hk, int logD, int H, int chunk) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // SWIZZLE_128B operands need 1024-byte aligned tiles: align explicitly (the launch adds 1 KB of slack)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  constexpr int NA = PASSES == 3 ? 2 : 1;                 // hi (+ lo) operand copies
-  constexpr int SA = 256 / (TILES * KB * NA);             // A stages that fit TMEM columns [256, 512)
-  const FwdSmem L = fwd_smem(NP, PASSES, SB);
+  constexpr int b_tile_bytes = N * 128;
+  constexpr int stage_bytes = (PASSES == 3 ? 2 : 1) * b_tile_bytes;
+  float* epi = reinterpret_cast<float*>(smem + SB * stage_bytes);
   const uint32_t sbase = smem_u32(smem);
-  const uint32_t bar0 = sbase + L.bar_off;
+  const uint32_t bar0 = sbase + SB * stage_bytes + NWG * N * EPI_LD * 4;
   auto full_b = [&](int s) { return bar0 + 8 * s; };
   auto empty_b = [&](int s) { return bar0 + 8 * (SB + s); };
-  auto full_a = [&](int s) { return bar0 + 8 * (2 * SB + s); };
-  auto empty_a = [&](int s) { return bar0 + 8 * (2 * SB + SA + s); };
-  const uint32_t acc_full = bar0 + 8 * (2 * SB + 2 * SA), acc_empty = acc_full + 8;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(smem + L.bar_off + 8 * (2 * SB + 2 * SA + 2));
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = warp_uniform(threadIdx.x >> 5), lane = threadIdx.x & 31;
   const int D = 1 << logD;
   const long long rows_total = (long long)B * D;
-  const int n128 = (int)((rows_total + BM - 1) / BM);
-  const int n_items = fwd_num_items(n128);
-  const int nch = (hk + chunk - 1) / chunk;
+  const int n_tiles = (int)((rows_total + TILE_M - 1) / TILE_M);
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < SB; ++s) { mbar_init(full_b(s), 1); mbar_init(empty_b(s), 1); }
-    for (int s = 0; s < SA; ++s) { mbar_init(full_a(s), 8); mbar_init(empty_a(s), 1); }
-    mbar_init(acc_full, 1);
-    mbar_init(acc_empty, 8);
+    for (int s = 0; s < SB; ++s) { mbar_init(full_b(s), 1); mbar_init(empty_b(s), NWG * 4); }
     fence_barrier_init();
   }
-  if (warp == 9) tmem_alloc(smem_u32(tmem_ptr), 512u);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  const uint32_t a_stage0 = tmem_base + 256u;
 
-  // Register re-distribution between warpgroups (registers are per SM sub-partition: 3 warps x 168 at launch):
-  // the two row-owning warpgroups hold x0 (32) + the running output row (up to 128) in registers.
-  if (warp < 8) {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
-  } else {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-  }
-  if (warp < 8) {
-    // ============================ A producers (one row each) + chunk drain + epilogue ============================
-    const int t = warp >> 2;
-    const uint32_t lane_sel = (uint32_t)((warp & 3) * 32) << 16;
-    int sa = 0, pha = 0;
-    uint32_t g = 0;                                   // chunk counter (same sequence as the MMA warp)
-    float acc[NPT];
-    auto drain = [&](uint32_t gi, bool on) {          // add finished chunk gi into acc, then hand TMEM back
-      mbar_wait(acc_full, gi & 1u);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + lane_sel + (uint32_t)(t * NP);
-#pragma unroll
-      for (int c0 = 0; c0 < NPT; c0 += 32) {            // two 16-column loads in flight per wait
-        if (c0 < NP && on) {
-          uint32_t v0[16], v1[16];
-          tmem_ld16_nowait(taddr + c0, v0);
-          if (c0 + 16 < NP) tmem_ld16_nowait(taddr + c0 + 16, v1);
-          tmem_wait_ld();
-#pragma unroll
-          for (int q = 0; q < 16; ++q) acc[c0 + q] += __uint_as_float(v0[q]);
-          if (c0 + 16 < NP) {
-#pragma unroll
-            for (int q = 0; q < 16; ++q) acc[c0 + 16 + q] += __uint_as_float(v1[q]);
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(acc_empty);
-    };
-    for (int it = 0; it < n_items; ++it) {
-      const FwdItem item = fwd_item(it, n128);
-      if (item.nt == 0) continue;
-      const bool on = t < item.nt;                     // single-tile item: the second M-tile's warps only keep the barriers in phase
-      const long long r = (long long)(item.tile0 + t) * BM + (warp & 3) * 32 + lane;
-      const bool valid = on && r < rows_total;
-      const int b = valid ? (int)(r >> logD) : 0;
-      const int d = (int)(r & (D - 1));
-      float x0v[KB];
-#pragma unroll
-      for (int j = 0; j < KB; ++j) x0v[j] = (valid && j < m) ? __ldg(x0 + ((size_t)b * m + j) * D + d) : 0.f;
-#pragma unroll
-      for (int n = 0; n < NPT; ++n) acc[n] = 0.f;
-      const float* xkp = xk + (size_t)b * hk * D + d;
-      float xnext = valid ? __ldg(xkp) : 0.f;
-      for (int c = 0; c < nch; ++c, ++g) {
-        const int i_beg = c * chunk, i_end = min(hk, (c + 1) * chunk);
-        const int drain_at = min(SA, i_end - i_beg);  // previous chunk is drained once SA blocks of this one are staged
-        for (int i = i_beg; i < i_end; ++i) {
-          const float xi = xnext;
-          if (i + 1 < hk) xnext = valid ? __ldg(xkp + (size_t)(i + 1) * D) : 0.f;
-          mbar_wait(empty_a(sa), pha ^ 1);
-          tc_fence_after();
-          const uint32_t a_hi = a_stage0 + lane_sel + (uint32_t)((sa * TILES + t) * KB * NA);
-          if (on) {
-#pragma unroll
-          for (int part = 0; part < KB / 8; ++part) {
-            float p[8];
-#pragma unroll
-            for (int q = 0; q < 8; ++q) p[q] = xi * x0v[part * 8 + q];
-            if (PASSES == 3) {
-              float h[8];
-#pragma unroll
-              for (int q = 0; q < 8; ++q) h[q] = tf32_rna(p[q]);
-              tmem_st8(a_hi + part * 8, h);
-#pragma unroll
-              for (int q = 0; q < 8; ++q) p[q] -= h[q];
-              tmem_st8(a_hi + KB + part * 8, p);
-            } else {
-              tmem_st8(a_hi + part * 8, p);
-            }
-          }
-          tmem_wait_st();
-          }
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(full_a(sa));
-          if (++sa == SA) { sa = 0; pha ^= 1; }
-          if (c > 0 && i - i_beg + 1 == drain_at) drain(g - 1, on);
-        }
-      }
-      drain(g - 1, on);
-      // ---------------- epilogue: registers -> out (B,H,D) and pooled (B,H) ----------------
-#pragma unroll
-      for (int n = 0; n < NPT; ++n)
-        if (n < H && valid) out[((size_t)b * H + n) * D + d] = acc[n];
-      if (pooled != nullptr) {
-        // sum over the D lanes of each sample: halving butterfly (after step s a lane keeps NPT >> (s+1) partial columns)
-        int col0 = 0;
-        if (logD > 0) col0 += bfly_step<NPT, NPT / 2>(acc, lane, D >> 1);
-        if (logD > 1) col0 += bfly_step<NPT, NPT / 4>(acc, lane, D >> 2);
-        if (logD > 2) col0 += bfly_step<NPT, NPT / 8>(acc, lane, D >> 3);
-        if (logD > 3) col0 += bfly_step<NPT, NPT / 16>(acc, lane, D >> 4);
-        if (logD > 4) col0 += bfly_step<NPT, NPT / 32>(acc, lane, D >> 5);
-        const int cnt = NPT >> logD;
-#pragma unroll
-        for (int q = 0; q < NPT; ++q)
-          if (q < cnt && valid && col0 + q < H) pooled[(size_t)b * H + col0 + q] = acc[q];
-      }
-    }
-  } else if (warp == 8) {
+  if (warp >= NWG * 4) {
     // ============================ TMA producer for the filter tiles ============================
-    if (lane == 0) {
+    setmaxnreg_dec<40>();
+    if (warp == NWG * 4 && lane == 0) {
       int s = 0, ph = 0;
-      for (int it = 0; it < n_items; ++it) {
-        if (fwd_item(it, n128).nt == 0) continue;
+      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
         for (int i = 0; i < hk; ++i) {
           mbar_wait(empty_b(s), ph ^ 1);
-          const uint32_t b_dst = sbase + s * L.stage_bytes;
-          mbar_expect_tx(full_b(s), (uint32_t)(NA * L.b_tile_bytes));
-          tma_load_2d(b_dst, &tmap_w, i * KB, 0, full_b(s));
-          if (PASSES == 3) tma_load_2d(b_dst + L.b_tile_bytes, &tmap_w, i * KB, NP, full_b(s));
+          const uint32_t dst = sbase + s * stage_bytes;
+          mbar_expect_tx(full_b(s), (uint32_t)stage_bytes);
+          tma_load_2d(dst, &tmap_w, i * KB, 0, full_b(s));
+          if (PASSES == 3) tma_load_2d(dst + b_tile_bytes, &tmap_w, i * KB, N, full_b(s));
           if (++s == SB) { s = 0; ph ^= 1; }
         }
       }
     }
-  } else if (warp == 9) {
-    // ============================ MMA issuer (TS mode: A from TMEM, B from shared memory) ============================
-    {
-      const uint32_t idesc = umma_idesc_tf32(NP);
-      int sb = 0, phb = 0, sa = 0, pha = 0;
-      uint32_t g = 0;
-      for (int it = 0; it < n_items; ++it) {
-        const int nt = fwd_item(it, n128).nt;
-        if (nt == 0) continue;
-        for (int c = 0; c < nch; ++c, ++g) {
-          mbar_wait(acc_empty, (g & 1u) ^ 1u);                 // previous chunk has been drained out of TMEM
-          tc_fence_after();
-          const int i_beg = c * chunk, i_end = min(hk, (c + 1) * chunk);
-          for (int i = i_beg; i < i_end; ++i) {
-            mbar_wait(full_a(sa), pha);
-            mbar_wait(full_b(sb), phb);
-            tc_fence_after();
-            if (elect_one()) {
-            const uint32_t first = (i == i_beg) ? 0u : 1u;
-            const uint32_t st_base = sbase + sb * L.stage_bytes;
-            const uint64_t b_hi = umma_desc_sw128(st_base);
-            const uint64_t b_lo = umma_desc_sw128(st_base + L.b_tile_bytes);
+    return;
+  }
+
+  // ============================ consumer warpgroups: A fragments, wgmma, epilogue ============================
+  setmaxnreg_inc<232>();
+  const int wg = warp >> 2, w = warp & 3, g = lane >> 2, t = lane & 3;
+  float* es = epi + wg * N * EPI_LD;
+  int s = 0, ph = 0;
+  float dacc[N / 2];
 #pragma unroll
-            for (int tt = 0; tt < TILES; ++tt) {
-              if (tt >= nt) break;
-              const uint32_t a_hi = a_stage0 + (uint32_t)((sa * TILES + tt) * KB * NA);
-              const uint32_t a_lo = a_hi + KB;
-              const uint32_t dcol = tmem_base + (uint32_t)(tt * NP);
-              if (PASSES == 3) {
-                // small terms first, the dominant hi*hi term last
+  for (int q = 0; q < N / 2; ++q) dacc[q] = 0.f;
+  for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    const long long base = (long long)tile * TILE_M + wg * WG_M;
+    bool valid[2];
+    const float* xkp[2];
+    float x0v[2][8];                                   // x0[b, j, d] of this thread's fragment columns j = 8c + t + 4h
 #pragma unroll
-                for (int k = 0; k < KB / 8; ++k) umma_tf32_ts(dcol, a_lo + 8 * k, b_hi + 2 * k, idesc, k > 0 ? 1u : first);
+    for (int rr = 0; rr < 2; ++rr) {
+      const long long r = base + w * 16 + g + 8 * rr;
+      valid[rr] = r < rows_total;
+      const int b = valid[rr] ? (int)(r >> logD) : 0;
+      const int d = (int)(r & (D - 1));
 #pragma unroll
-                for (int k = 0; k < KB / 8; ++k) umma_tf32_ts(dcol, a_hi + 8 * k, b_lo + 2 * k, idesc, 1u);
+      for (int q = 0; q < 8; ++q) {
+        const int j = 8 * (q >> 1) + t + 4 * (q & 1);
+        x0v[rr][q] = (valid[rr] && j < m) ? __ldg(x0 + ((size_t)b * m + j) * D + d) : 0.f;
+      }
+      xkp[rr] = xk + (size_t)b * hk * D + d;
+    }
+    float acc[N / 2];
 #pragma unroll
-                for (int k = 0; k < KB / 8; ++k) umma_tf32_ts(dcol, a_hi + 8 * k, b_hi + 2 * k, idesc, 1u);
-              } else {
+    for (int q = 0; q < N / 2; ++q) acc[q] = 0.f;
+    for (int i0 = 0; i0 < hk; i0 += chunk) {
+      const int i1 = min(hk, i0 + chunk);
+      for (int i = i0; i < i1; ++i) {
+        const float xi0 = valid[0] ? __ldg(xkp[0] + (size_t)i * D) : 0.f;
+        const float xi1 = valid[1] ? __ldg(xkp[1] + (size_t)i * D) : 0.f;
+        uint32_t ah[KB / 8][4], al[KB / 8][4];         // A fragments (hi, lo) of the four k-steps of this K-block
 #pragma unroll
-                for (int k = 0; k < KB / 8; ++k) umma_tf32_ts(dcol, a_hi + 8 * k, b_hi + 2 * k, idesc, k > 0 ? 1u : first);
-              }
-            }
-            umma_commit(empty_a(sa));                  // A staging columns free once these MMAs have read them
-            umma_commit(empty_b(sb));                  // and the filter stage
-            if (i + 1 == i_end) umma_commit(acc_full); // chunk complete -> drain
-            }
-            __syncwarp();
-            if (++sa == SA) { sa = 0; pha ^= 1; }
-            if (++sb == SB) { sb = 0; phb ^= 1; }
+        for (int c = 0; c < KB / 8; ++c) {
+          const float a[4] = {xi0 * x0v[0][2 * c], xi1 * x0v[1][2 * c], xi0 * x0v[0][2 * c + 1], xi1 * x0v[1][2 * c + 1]};
+          tf32_split(a, ah[c], al[c]);
+        }
+        mbar_wait(full_b(s), ph);
+        const uint64_t bhi = gmma_desc_kmajor(sbase + s * stage_bytes, 128);
+        const uint64_t blo = gmma_desc_kmajor(sbase + s * stage_bytes + b_tile_bytes, 128);
+        wgmma_fence();
+#pragma unroll
+        for (int c = 0; c < KB / 8; ++c) {
+          const int sc = (i > i0 || c > 0) ? 1 : 0;
+          if (PASSES == 3) {
+            // small terms first, the dominant hi*hi term last
+            wgmma_tf32_rs<N>(dacc, al[c], bhi + 2 * c, sc);
+            wgmma_tf32_rs<N>(dacc, ah[c], blo + 2 * c, 1);
+            wgmma_tf32_rs<N>(dacc, ah[c], bhi + 2 * c, 1);
+          } else {
+            wgmma_tf32_rs<N>(dacc, ah[c], bhi + 2 * c, sc);
           }
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+#pragma unroll
+        for (int c = 0; c < KB / 8; ++c) { wgmma_keep(ah[c]); wgmma_keep(al[c]); }
+        if (lane == 0) mbar_arrive(empty_b(s));        // this warp is done with the stage
+        if (++s == SB) { s = 0; ph ^= 1; }
+      }
+#pragma unroll
+      for (int q = 0; q < N / 2; ++q) acc[q] += dacc[q];
+    }
+    // ---------------- epilogue: fragment -> es[n][row] -> out (B,H,D) and pooled (B,H) ----------------
+#pragma unroll
+    for (int c = 0; c < N / 8; ++c) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        es[(8 * c + 2 * t + e) * EPI_LD + w * 16 + g] = acc[4 * c + e];
+        es[(8 * c + 2 * t + e) * EPI_LD + w * 16 + g + 8] = acc[4 * c + 2 + e];
+      }
+    }
+    wg_bar_sync(1 + wg);
+    const int tw = threadIdx.x & 127;
+    for (int idx = tw; idx < H * WG_M; idx += 128) {
+      const int n = idx / WG_M, row = idx % WG_M;
+      const long long r = base + row;
+      if (r < rows_total) out[((size_t)(r >> logD) * H + n) * D + (int)(r & (D - 1))] = es[n * EPI_LD + row];
+    }
+    if (pooled != nullptr) {
+      const int nb = WG_M >> logD;                     // samples in this warpgroup's rows (D <= 32 divides 64)
+      for (int idx = tw; idx < H * nb; idx += 128) {
+        const int n = idx / nb, bl = idx % nb;
+        const long long b = (base >> logD) + bl;
+        if (b < B) {
+          float sum = 0.f;
+          for (int d = 0; d < D; ++d) sum += es[n * EPI_LD + bl * D + d];
+          pooled[(size_t)b * H + n] = sum;
         }
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 9) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512u);
+    wg_bar_sync(1 + wg);
   }
 }
 
@@ -441,7 +319,6 @@ cin_bwd_dw_kernel(const float* __restrict__ x0, const float* __restrict__ xk, co
 static bool tensor_path_ok(int64_t m, int64_t hk, int64_t D, int64_t H) {
   return m >= 1 && m <= KB && hk >= 1 && H >= 1 && H <= 128 && D >= 1 && D <= 32 && (D & (D - 1)) == 0;
 }
-static int64_t pad16(int64_t h) { return (h + 15) / 16 * 16; }
 
 }  // namespace cin
 }  // namespace ctr
@@ -452,7 +329,7 @@ using namespace ctr::cin;
 extern "C" int64_t ctr_cin_fwd_workspace_bytes(int64_t B, int64_t m, int64_t hk, int64_t D, int64_t H) {
   (void)B;
   if (!tensor_path_ok(m, hk, D, H)) return 0;
-  return 2 * pad16(H) * hk * KB * (int64_t)sizeof(float);
+  return 2 * (int64_t)npad(H) * hk * KB * (int64_t)sizeof(float);
 }
 
 static int check_cin(const char* fn, int64_t B, int64_t m, int64_t hk, int64_t D, int64_t H) {
@@ -481,7 +358,7 @@ extern "C" int ctr_cin_fwd(const float* x0, const float* xk, const float* filter
     CTR_CHECK_LAUNCH("ctr_cin_fwd(simple)");
     return CTR_OK;
   }
-  const int NP = (int)pad16(H);
+  const int NP = npad(H);
   const int64_t need = ctr_cin_fwd_workspace_bytes(B, m, hk, D, H);
   CTR_REQUIRE(workspace != nullptr && workspace_bytes >= need,
               "ctr_cin_fwd: workspace of %lld bytes required (ctr_cin_fwd_workspace_bytes), got %lld", (long long)need,
@@ -514,28 +391,24 @@ extern "C" int ctr_cin_fwd(const float* x0, const float* xk, const float* filter
   int logD = 0;
   while ((1 << logD) < D) ++logD;
   const long long rows_total = (long long)B * D;
-  const int num_pairs = (int)((rows_total + TILES * BM - 1) / (TILES * BM));
-  const int grid = num_pairs < sm_count() ? num_pairs : sm_count();
-  // K-blocks per TMEM accumulation chain of the 3xTF32 path: 12 MMAs each.  The fp32 accumulate of the tensor core truncates
-  // (~2.6e-8 relative per MMA, measured 3.8e-5 after 1440 MMAs).  8 blocks = 96 MMAs.  16 blocks (192 MMAs, half the drains)
-  // was measured in round 2: 2.94 -> 2.88 ms per config-3 step, but the element-wise error reaches 0.9-1.5x the 1e-5 bound
-  // (profiles/r2_cin_chunk16.jsonl) -- not worth 2 %.
+  const int n_tiles = (int)((rows_total + TILE_M - 1) / TILE_M);
+  const int grid = n_tiles < sm_count() ? n_tiles : sm_count();
+  // K-blocks per accumulation chain of the 3xTF32 path: 8 blocks = 96 chained MMAs before the registers take the sum
   constexpr int CHUNK3 = 8;
-#define CIN_LAUNCH(PASSES_, SB_, NPT_, CHUNK_)                                                                        \
+#define CIN_LAUNCH(PASSES_, SB_, N_, CHUNK_)                                                                          \
   {                                                                                                                   \
-    const FwdSmem L = fwd_smem(NP, PASSES_, SB_);                                                                     \
-    auto k = cin_fwd_tc_kernel<PASSES_, SB_, NPT_>;                                                                   \
-    CTR_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, L.total + 1024));                   \
-    k<<<grid, NTHREADS, L.total + 1024, st>>>(tmap, x0, xk, out, pooled, (int)B, (int)m, (int)hk, logD, (int)H, NP,   \
-                                              CHUNK_);                                                                \
+    const int smem = fwd_smem_bytes(N_, PASSES_, SB_) + 1024;                                                         \
+    auto k = cin_fwd_tc_kernel<PASSES_, SB_, N_>;                                                                     \
+    CTR_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));                             \
+    k<<<grid, NTHREADS, smem, st>>>(tmap, x0, xk, out, pooled, (int)B, (int)m, (int)hk, logD, (int)H, CHUNK_);        \
   }
   if (precision == 0) {
-    if (NP <= 32) CIN_LAUNCH(3, 4, 32, CHUNK3) else if (NP <= 64) CIN_LAUNCH(3, 4, 64, CHUNK3) else CIN_LAUNCH(3, 4, 128, CHUNK3)
+    if (NP == 32) CIN_LAUNCH(3, 4, 32, CHUNK3) else if (NP == 64) CIN_LAUNCH(3, 4, 64, CHUNK3) else CIN_LAUNCH(3, 4, 128, CHUNK3)
   } else {
-    if (NP <= 32) CIN_LAUNCH(1, 6, 32, 32) else if (NP <= 64) CIN_LAUNCH(1, 6, 64, 32) else CIN_LAUNCH(1, 6, 128, 32)
+    if (NP == 32) CIN_LAUNCH(1, 6, 32, 32) else if (NP == 64) CIN_LAUNCH(1, 6, 64, 32) else CIN_LAUNCH(1, 6, 128, 32)
   }
 #undef CIN_LAUNCH
-  CTR_CHECK_LAUNCH("ctr_cin_fwd(tcgen05)");
+  CTR_CHECK_LAUNCH("ctr_cin_fwd(wgmma)");
   return CTR_OK;
 }
 

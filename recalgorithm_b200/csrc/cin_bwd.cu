@@ -1,24 +1,25 @@
-// Row CIN, backward on the tensor cores (tcgen05, TS mode) -- gradients of xDeepFM/cin_layer.py:17-30.
+// Row CIN, backward on the tensor cores (wgmma) -- gradients of xDeepFM/cin_layer.py:17-30.
 //
 //   out[b,n,d] = sum_{i,j} xk[b,i,d] x0[b,j,d] W[(i,j),n]            g = dL/dout  (B,H,D)
 //   dZ[r,(i,j)] = sum_n g[b,n,d] W[(i,j),n]      (r = (b,d))
 //   dxk[b,i,d]  = sum_j dZ[r,(i,j)] x0[b,j,d]        dx0[b,j,d] = sum_i dZ[r,(i,j)] xk[b,i,d]
 //   dW[(i,j),n] = sum_r xk[b,i,d] x0[b,j,d] g[b,n,d]
 //
-// Two kernels, both with the operand the threads generate placed in TMEM (the generating thread is the TMEM lane) and
-// the streamed operand delivered by TMA, 3xTF32 split for fp32-class accuracy (see cin.cu for the accuracy notes):
+// Two kernels.  In both the operand the threads generate is the wgmma A operand, held in registers in the A-fragment
+// layout, and the streamed operand is delivered by TMA into swizzled shared memory through an mbarrier pipeline;
+// 3xTF32 split for fp32-class accuracy (see cin.cu for the accuracy notes):
 //
-//  dX kernel   GEMM dZ_i[128 rows x 32 j] = Gt[128 x H] . W_i^T[H x 32]   for every i
-//     A = Gt (hi, lo) written ONCE per 128-row tile into TMEM by the row-owning threads;
-//     B = W rows (i*m .. i*m+31) x H, K-major in the filter's native layout, TMA-streamed (3-D box = 4 swizzled sub-tiles);
-//     D = dZ_i in one of 8 TMEM buffers; the row-owning thread reads its 32 values and does both contractions
-//     (dxk: dot with its x0 registers; dx0: axpy into 32 register accumulators) -- no cross-thread traffic at all.
+//  dX kernel   GEMM dZ_i[64 rows x 64 (i,j)] = G[64 x H] . W^T[H x 64]   for two i per step
+//     A = G: each thread loads the g values of its two rows once per tile into registers;
+//     B = W rows (i0*m .. i0*m+63) x H, K-major in the filter's native layout, TMA-streamed (4-D box = HP/32 swizzled sub-tiles);
+//     dZ stays in the accumulator registers: the thread does both contractions on its fragment (dxk: dot with its x0
+//     registers + a reduction over the 4 threads that share a row; dx0: axpy into register accumulators).
 //
-//  dW kernel   GEMM dW_blk[128 (i,j) x H] += Z^T[128 (i,j) x D] . G_b^T[D x H]   for every sample b
-//     A = Z^T: thread (i,j) forms xk[b,i,:] * x0[b,j,:] (two contiguous D-vectors) -> TMEM;
+//  dW kernel   GEMM dW_blk[64 (i,j) x H] += Z^T[64 (i,j) x D] . G_b^T[D x H]   for every sample b
+//     A = Z^T: thread (i,j) forms xk[b,i,d] * x0[b,j,d] for the d of its fragment columns;
 //     B = g[b] as [H rows x D] K-major tiles (TMA 3-D box, swizzle width = D*4 bytes);
-//     each CTA owns 2 blocks of 128 (i,j) rows (8 consecutive i) and a slice of the batch; accumulation chains are cut every
-//     CHUNK samples and added into fp32 registers (round-to-nearest); one vector red.global.add per element at the end.
+//     each CTA owns 4 consecutive i (two warpgroups x 64 (i,j) rows) and a slice of the batch; accumulation chains are cut
+//     every `chunk` samples and added into fp32 registers (round-to-nearest); one atomic add per element at the end.
 #include <stdlib.h>
 
 #include "tc_ptx.cuh"
@@ -28,6 +29,8 @@ namespace cinb {
 using namespace ctr::tc;
 
 constexpr int KB = 32;
+constexpr int NWG = 2;                      // consumer warpgroups per CTA
+constexpr int NTHREADS = (NWG + 1) * 128;   // + one producer warpgroup (one TMA thread)
 
 // ================================================================================================= prep kernels
 // filter (hk*m, H) -> ws[2][KRP][HP]  (tf32-rounded value | residual), zero padded rows/cols.
@@ -53,47 +56,12 @@ __global__ void split_grad_kernel(const float* __restrict__ g, float* __restrict
 }
 
 // ================================================================================================= dX kernel
-constexpr int DX_THREADS = 192;     // 4 row-owner warps + TMA warp + MMA warp
-constexpr int DX_IPS = 2;           // i's per MMA step: N = 64 keeps the single issuing thread ahead of the tensor pipe
-constexpr int DX_N = DX_IPS * KB;   // 64 columns of dZ per step
-constexpr int DX_DBUF = 4;          // dZ buffers of 64 TMEM columns at columns [256, 512)
+constexpr int DX_IPS = 2;           // i's per step
+constexpr int DX_N = DX_IPS * KB;   // 64 columns of dZ per step (wgmma N)
+constexpr int DX_TILE = NWG * WG_M; // rows per CTA tile
 
-// 4-D TMA view of the split filter (n_inner 32 | row | i-in-step | n_outer): one box lands as
-//   [n_outer kb][i_t][32 rows][128 B]  = per kb one K-major [64 rows x 128 B] SWIZZLE_128B operand tile.
-__device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2, int c3, uint32_t bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
-      ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(bar)
-      : "memory");
-}
-
-__device__ __forceinline__ void tma_load_4d_mc(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2, int c3,
-                                               uint32_t bar, uint16_t cta_mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes.multicast::cluster"
-      " [%0], [%1, {%2, %3, %4, %5}], [%6], %7;"
-      ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(bar), "h"(cta_mask)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_mc(uint32_t bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(bar), "h"(cta_mask) : "memory");
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-
-// MC: launched as 2-CTA clusters; the two CTAs work on different row tiles in lockstep and share every filter stage --
-// rank 0 TMA-multicasts the hi copy, rank 1 the lo copy, into BOTH CTAs' shared memory (halves the L2->SM traffic the
-// kernel is bound by); a stage is released when both CTAs' MMAs have consumed it (multicast commit, count 2).
-template <int SB, int NKB, bool MC>
-__global__ void __launch_bounds__(DX_THREADS, 1)
+template <int SB, int NKB>
+__global__ void __launch_bounds__(NTHREADS, 1)
 cin_bwd_dx_tc_kernel(const __grid_constant__ CUtensorMap tmap_w, const float* __restrict__ x0,
                      const float* __restrict__ xk, const float* __restrict__ g, float* __restrict__ dx0,
                      float* __restrict__ dxk, int B, int m, int hk, int logD, int H, int KRP) {
@@ -106,557 +74,171 @@ cin_bwd_dx_tc_kernel(const __grid_constant__ CUtensorMap tmap_w, const float* __
   const uint32_t bar0 = sbase + SB * stage_bytes;
   auto full_b = [&](int s) { return bar0 + 8 * s; };
   auto empty_b = [&](int s) { return bar0 + 8 * (SB + s); };
-  auto d_full = [&](int q) { return bar0 + 8 * (2 * SB + q); };
-  auto d_empty = [&](int q) { return bar0 + 8 * (2 * SB + DX_DBUF + q); };
-  const uint32_t a_full = bar0 + 8 * (2 * SB + 2 * DX_DBUF), a_empty = a_full + 8;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(smem + SB * stage_bytes + 8 * (2 * SB + 2 * DX_DBUF + 2));
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = warp_uniform(threadIdx.x >> 5), lane = threadIdx.x & 31;
   const int D = 1 << logD;
   const long long rows_total = (long long)B * D;
-  const int num_tiles = (int)((rows_total + BM - 1) / BM);
-  const int tile_iters = (num_tiles + (int)gridDim.x - 1) / (int)gridDim.x;   // identical for every CTA (lockstep in a cluster)
+  const int num_tiles = (int)((rows_total + DX_TILE - 1) / DX_TILE);
   const int nsteps = (hk + DX_IPS - 1) / DX_IPS;
-  const uint32_t cta_rank = MC ? cluster_ctarank() : 0u;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < SB; ++s) { mbar_init(full_b(s), 1); mbar_init(empty_b(s), MC ? 2 : 1); }
-    for (int q = 0; q < DX_DBUF; ++q) { mbar_init(d_full(q), 1); mbar_init(d_empty(q), 4); }
-    mbar_init(a_full, 4);
-    mbar_init(a_empty, 1);
+    for (int s = 0; s < SB; ++s) { mbar_init(full_b(s), 1); mbar_init(empty_b(s), NWG * 4); }
     fence_barrier_init();
   }
-  if (warp == 5) tmem_alloc(smem_u32(tmem_ptr), 512u);
-  tc_fence_before();
   __syncthreads();
-  if (MC) cluster_sync_all();                          // the peer's barriers are initialised before anything is sent to them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  const uint32_t d_col0 = tmem_base + 256u;
 
-  if (warp < 4) {
-    // ============================ row owners: stage Gt once per tile, then consume dZ of two i per step ============================
-    const uint32_t lane_sel = (uint32_t)(warp * 32) << 16;
-    uint32_t di = 0;                                   // dZ buffer use counter (same sequence as the MMA warp)
-    int lt = 0;
-    for (int ti = 0; ti < tile_iters; ++ti, ++lt) {
-      const int tile = blockIdx.x + ti * gridDim.x;          // may be past the end: an all-invalid tile keeps the pipeline in step
-      const long long r = (long long)tile * BM + warp * 32 + lane;
-      const bool valid = tile < num_tiles && r < rows_total;
-      const int b = valid ? (int)(r >> logD) : 0;
-      const int d = (int)(r & (D - 1));
-      float x0v[KB], dx0acc[KB];
-#pragma unroll
-      for (int j = 0; j < KB; ++j) {
-        x0v[j] = (valid && j < m) ? __ldg(x0 + ((size_t)b * m + j) * D + d) : 0.f;
-        dx0acc[j] = 0.f;
-      }
-      mbar_wait(a_empty, (lt & 1) ^ 1);                // MMAs of the previous tile no longer read the A columns
-      tc_fence_after();
-      const float* gp = g + (size_t)b * H * D + d;
-#pragma unroll 1
-      for (int n0 = 0; n0 < HP; n0 += 8) {
-        float v[8], h[8];
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          v[q] = (valid && n0 + q < H) ? __ldg(gp + (size_t)(n0 + q) * D) : 0.f;
-          h[q] = tf32_rna(v[q]);
-          v[q] -= h[q];
-        }
-        tmem_st8(tmem_base + lane_sel + (uint32_t)n0, h);
-        tmem_st8(tmem_base + lane_sel + (uint32_t)(HP + n0), v);
-      }
-      tmem_wait_st();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(a_full);
-      const float* xkp = xk + (size_t)b * hk * D + d;
-      for (int st = 0; st < nsteps; ++st, ++di) {
-        const int i0 = st * DX_IPS;
-        float xi[DX_IPS];
-#pragma unroll
-        for (int t = 0; t < DX_IPS; ++t) xi[t] = (valid && i0 + t < hk) ? __ldg(xkp + (size_t)(i0 + t) * D) : 0.f;
-        const uint32_t q = di % DX_DBUF;
-        mbar_wait(d_full(q), (di / DX_DBUF) & 1u);
-        tc_fence_after();
-        uint32_t raw[DX_IPS * 2][16];                   // all four 16-column loads in flight, one wait
-#pragma unroll
-        for (int t = 0; t < DX_IPS * 2; ++t) tmem_ld16_nowait(d_col0 + lane_sel + q * DX_N + t * 16, raw[t]);
-        tmem_wait_ld();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(d_empty(q));         // buffer may be overwritten by a later step
-#pragma unroll
-        for (int t = 0; t < DX_IPS; ++t) {
-          float s4[4] = {0.f, 0.f, 0.f, 0.f};            // four independent partial sums (ILP) for the dxk dot product
-#pragma unroll
-          for (int j = 0; j < KB; ++j) {
-            const float dzv = __uint_as_float(raw[t * 2 + (j >> 4)][j & 15]);
-            s4[j & 3] += dzv * x0v[j];                   // x0v[j >= m] == 0 masks the rows that belong to the next i
-            dx0acc[j] += dzv * xi[t];                    // xi == 0 for i >= hk
-          }
-          if (valid && i0 + t < hk) dxk[((size_t)b * hk + i0 + t) * D + d] = (s4[0] + s4[1]) + (s4[2] + s4[3]);
-        }
-      }
-      if (valid) {
-#pragma unroll
-        for (int j = 0; j < KB; ++j)
-          if (j < m) dx0[((size_t)b * m + j) * D + d] = dx0acc[j];
-      }
-    }
-  } else if (warp == 4) {
+  if (warp >= NWG * 4) {
     // ============================ TMA: filter rows of i0 and i0+1 (hi and lo copies) ============================
-    if (lane == 0) {
+    setmaxnreg_dec<40>();
+    if (warp == NWG * 4 && lane == 0) {
       int s = 0, ph = 0;
-      for (int ti = 0; ti < tile_iters; ++ti) {
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         for (int st = 0; st < nsteps; ++st) {
           mbar_wait(empty_b(s), ph ^ 1);
           const uint32_t dst = sbase + s * stage_bytes;
           mbar_expect_tx(full_b(s), (uint32_t)stage_bytes);
-          if (MC) {
-            if (cta_rank == 0) tma_load_4d_mc(dst, &tmap_w, 0, st * DX_IPS * m, 0, 0, full_b(s), (uint16_t)3);
-            else tma_load_4d_mc(dst + b_copy_bytes, &tmap_w, 0, KRP + st * DX_IPS * m, 0, 0, full_b(s), (uint16_t)3);
-          } else {
-            tma_load_4d(dst, &tmap_w, 0, st * DX_IPS * m, 0, 0, full_b(s));
-            tma_load_4d(dst + b_copy_bytes, &tmap_w, 0, KRP + st * DX_IPS * m, 0, 0, full_b(s));
-          }
+          tma_load_4d(dst, &tmap_w, 0, st * DX_IPS * m, 0, 0, full_b(s));
+          tma_load_4d(dst + b_copy_bytes, &tmap_w, 0, KRP + st * DX_IPS * m, 0, 0, full_b(s));
           if (++s == SB) { s = 0; ph ^= 1; }
         }
       }
     }
-  } else {
-    // ============================ MMA issuer (fully unrolled: 3 passes x NKB x 4 MMAs of 128x64x8) ============================
-    {
-      const uint32_t idesc = umma_idesc_tf32(DX_N);
-      int s = 0, ph = 0, lt = 0;
-      uint32_t di = 0;
-      for (int ti = 0; ti < tile_iters; ++ti, ++lt) {
-        mbar_wait(a_full, lt & 1);
-        tc_fence_after();
-        for (int st = 0; st < nsteps; ++st, ++di) {
-          const uint32_t q = di % DX_DBUF;
-          mbar_wait(d_empty(q), ((di / DX_DBUF) & 1u) ^ 1u);
-          mbar_wait(full_b(s), ph);
-          tc_fence_after();
-          if (elect_one()) {
-          const uint32_t dcol = d_col0 + q * DX_N;
-          const uint64_t b_hi = umma_desc_sw128(sbase + s * stage_bytes);
-          const uint64_t b_lo = umma_desc_sw128(sbase + s * stage_bytes + b_copy_bytes);
-          const uint32_t a_hi = tmem_base, a_lo = tmem_base + (uint32_t)HP;
-          // small terms first: Glo.Whi, Ghi.Wlo, then Ghi.Whi ; sub-tile kb starts DX_N*128 bytes (>>4 = 512) further
+    return;
+  }
+
+  // ============================ consumers: G fragments once per tile, then dZ of two i per step ============================
+  setmaxnreg_inc<232>();
+  const int wg = warp >> 2, w = warp & 3, gq = lane >> 2, t = lane & 3;
+  int s = 0, ph = 0;
+  for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    const long long base = (long long)tile * DX_TILE + wg * WG_M;
+    bool valid[2];
+    int bb[2], dd[2];
+    float x0v[2][8], dx0acc[2][8];                   // fragment columns j = 8c + 2t + e  ->  [2c + e]
+    uint32_t gh[HP / 8][4], gl[HP / 8][4];           // A fragments of G (hi, lo): k-step s, columns n = 8s + t (+4)
 #pragma unroll
-          for (int kb = 0; kb < NKB; ++kb)
+    for (int rr = 0; rr < 2; ++rr) {
+      const long long r = base + w * 16 + gq + 8 * rr;
+      valid[rr] = r < rows_total;
+      bb[rr] = valid[rr] ? (int)(r >> logD) : 0;
+      dd[rr] = (int)(r & (D - 1));
 #pragma unroll
-            for (int k = 0; k < 4; ++k)
-              umma_tf32_ts(dcol, a_lo + (uint32_t)(kb * KB + 8 * k), b_hi + (uint64_t)(kb * (DX_N * 128 / 16) + 2 * k), idesc,
-                           (kb | k) != 0 ? 1u : 0u);
+      for (int q = 0; q < 8; ++q) {
+        const int j = 8 * (q >> 1) + 2 * t + (q & 1);
+        x0v[rr][q] = (valid[rr] && j < m) ? __ldg(x0 + ((size_t)bb[rr] * m + j) * D + dd[rr]) : 0.f;
+        dx0acc[rr][q] = 0.f;
+      }
+    }
 #pragma unroll
-          for (int kb = 0; kb < NKB; ++kb)
+    for (int ks = 0; ks < HP / 8; ++ks) {
+      float ga[4];
 #pragma unroll
-            for (int k = 0; k < 4; ++k)
-              umma_tf32_ts(dcol, a_hi + (uint32_t)(kb * KB + 8 * k), b_lo + (uint64_t)(kb * (DX_N * 128 / 16) + 2 * k), idesc, 1u);
+      for (int q = 0; q < 4; ++q) {
+        const int rr = q & 1, n = 8 * ks + t + 4 * (q >> 1);
+        ga[q] = (valid[rr] && n < H) ? __ldg(g + ((size_t)bb[rr] * H + n) * D + dd[rr]) : 0.f;
+      }
+      tf32_split(ga, gh[ks], gl[ks]);                // split once per tile: the wgmmas in flight read these registers
+    }
+    auto load_xi = [&](int i0, float (&xi)[2][DX_IPS]) {
 #pragma unroll
-          for (int kb = 0; kb < NKB; ++kb)
+      for (int rr = 0; rr < 2; ++rr)
 #pragma unroll
-            for (int k = 0; k < 4; ++k)
-              umma_tf32_ts(dcol, a_hi + (uint32_t)(kb * KB + 8 * k), b_hi + (uint64_t)(kb * (DX_N * 128 / 16) + 2 * k), idesc, 1u);
-          if (MC) umma_commit_mc(empty_b(s), (uint16_t)3); else umma_commit(empty_b(s));
-          umma_commit(d_full(q));
-          if (st + 1 == nsteps) umma_commit(a_empty);
+        for (int h = 0; h < DX_IPS; ++h)
+          xi[rr][h] = (valid[rr] && i0 + h < hk) ? __ldg(xk + ((size_t)bb[rr] * hk + i0 + h) * D + dd[rr]) : 0.f;
+    };
+    float xi[2][DX_IPS];
+    load_xi(0, xi);
+    for (int st = 0; st < nsteps; ++st) {
+      const int i0 = st * DX_IPS;
+      mbar_wait(full_b(s), ph);
+      const uint64_t bhi = gmma_desc_kmajor(sbase + s * stage_bytes, 128);
+      const uint64_t blo = gmma_desc_kmajor(sbase + s * stage_bytes + b_copy_bytes, 128);
+      float dz[DX_N / 2];
+#pragma unroll
+      for (int q = 0; q < DX_N / 2; ++q) dz[q] = 0.f;
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < HP / 8; ++ks) {
+        // sub-tile kb of a copy starts DX_N*128 bytes (>>4 = 512) further; small terms first
+        const uint64_t off = (uint64_t)((ks >> 2) * (DX_N * 128 / 16) + 2 * (ks & 3));
+        wgmma_tf32_rs<DX_N>(dz, gl[ks], bhi + off, ks > 0 ? 1 : 0);
+        wgmma_tf32_rs<DX_N>(dz, gh[ks], blo + off, 1);
+        wgmma_tf32_rs<DX_N>(dz, gh[ks], bhi + off, 1);
+      }
+      wgmma_commit();
+      float xin[2][DX_IPS];                            // the next step's xk values, loaded while this group runs
+      load_xi(i0 + DX_IPS, xin);
+      wgmma_wait<0>();                                 // gh / gl are not rewritten before the next tile, after this wait
+      if (lane == 0) mbar_arrive(empty_b(s));
+      if (++s == SB) { s = 0; ph ^= 1; }
+      // dz[4c + 2rr + e] = dZ[row rr][column 8c + 2t + e]; columns 0..31 belong to i0, 32..63 to i0 + 1
+#pragma unroll
+      for (int h = 0; h < DX_IPS; ++h) {
+#pragma unroll
+        for (int rr = 0; rr < 2; ++rr) {
+          float p = 0.f;
+#pragma unroll
+          for (int q = 0; q < 8; ++q) {
+            const float v = dz[4 * (4 * h + (q >> 1)) + 2 * rr + (q & 1)];
+            p += v * x0v[rr][q];                       // x0v[j >= m] == 0 masks the rows that belong to the next i
+            dx0acc[rr][q] += v * xi[rr][h];            // xi == 0 for i >= hk
           }
-          __syncwarp();
-          if (++s == SB) { s = 0; ph ^= 1; }
+          p += __shfl_xor_sync(0xffffffffu, p, 1);
+          p += __shfl_xor_sync(0xffffffffu, p, 2);
+          if (t == 0 && valid[rr] && i0 + h < hk) dxk[((size_t)bb[rr] * hk + i0 + h) * D + dd[rr]] = p;
         }
+      }
+#pragma unroll
+      for (int rr = 0; rr < 2; ++rr)
+#pragma unroll
+        for (int h = 0; h < DX_IPS; ++h) xi[rr][h] = xin[rr][h];
+    }
+#pragma unroll
+    for (int rr = 0; rr < 2; ++rr) {
+#pragma unroll
+      for (int q = 0; q < 8; ++q) {
+        const int j = 8 * (q >> 1) + 2 * t + (q & 1);
+        if (valid[rr] && j < m) dx0[((size_t)bb[rr] * m + j) * D + dd[rr]] = dx0acc[rr][q];
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (MC) cluster_sync_all();                          // nobody leaves while the peer may still multicast into it
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512u);
-  }
-}
-
-// ================================================================================================= dX kernel, CTA pair
-// cta_group::2 form of the kernel above (round 2).  Measured bound of the single-CTA kernel: TS-mode kind::tf32 at M = 128
-// reads its B operand from shared memory at 64 B/clk and the TMA fill of a stage that serves ONE row tile adds 42 B/clk --
-// 104 of the SM's 128 B/clk, tensor pipe 49 % busy.  Here two CTAs of a cluster form one M = 256 MMA: every CTA keeps its own
-// 128 rows of Gt in its TMEM and its own dZ buffers, but holds only HALF of each filter stage (the rows of ONE i: N = 64 =
-// 2 x 32, rank r loads i0 + r), so operand reads and TMA fill per SM halve.  The leader (rank 0) issues every MMA and
-// commits to both CTAs' barriers (multicast); the peer's TMA completes on the leader's `full` barrier (cta_group::2 copy),
-// the peer's row owners arrive remotely on the leader's a_full / d_empty barriers.
-__device__ __forceinline__ uint32_t mapa_rank(uint32_t addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_2sm(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2, int c3, uint32_t leader_bar) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];"
-      ::"r"(dst), "l"(map), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(leader_bar)
-      : "memory");
-}
-__device__ __forceinline__ void umma_tf32_ts_2sm(uint32_t tmem_d, uint32_t tmem_a, uint64_t bdesc, uint32_t idesc, uint32_t acc) {
-  asm volatile(
-      "{\n"
-      ".reg .pred p;\n"
-      "setp.ne.b32 p, %4, 0;\n"
-      "tcgen05.mma.cta_group::2.kind::tf32 [%0], [%1], %2, %3, p;\n"
-      "}\n" ::"r"(tmem_d), "r"(tmem_a), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_2sm(uint32_t bar, uint16_t cta_mask) {
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-               ::"r"(bar), "h"(cta_mask) : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_2sm(uint32_t dst_smem, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(ncols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_2sm(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-// instruction descriptor of the pair MMA: D = f32, A = B = tf32, both K-major, M = 256, N
-__device__ __forceinline__ uint32_t umma_idesc_tf32_m256(int n) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(256 >> 4) << 24);
-}
-
-template <int SB, int NKB>
-__global__ void __launch_bounds__(DX_THREADS, 1)
-cin_bwd_dx_tc2_kernel(const __grid_constant__ CUtensorMap tmap_half, const float* __restrict__ x0,
-                      const float* __restrict__ xk, const float* __restrict__ g, float* __restrict__ dx0,
-                      float* __restrict__ dxk, int B, int m, int hk, int logD, int H, int KRP) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  constexpr int HP = NKB * KB;
-  constexpr int half_copy_bytes = NKB * KB * 128;           // one (hi or lo) copy of THIS CTA's 32 filter rows: NKB sub-tiles of [32 x 128 B]
-  constexpr int stage_bytes = 2 * half_copy_bytes;
-  const uint32_t sbase = smem_u32(smem);
-  const uint32_t bar0 = sbase + SB * stage_bytes;
-  auto full_b = [&](int s) { return bar0 + 8 * s; };
-  auto empty_b = [&](int s) { return bar0 + 8 * (SB + s); };
-  auto d_full = [&](int q) { return bar0 + 8 * (2 * SB + q); };
-  auto d_empty = [&](int q) { return bar0 + 8 * (2 * SB + DX_DBUF + q); };
-  const uint32_t a_full = bar0 + 8 * (2 * SB + 2 * DX_DBUF), a_empty = a_full + 8;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(smem + SB * stage_bytes + 8 * (2 * SB + 2 * DX_DBUF + 2));
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int D = 1 << logD;
-  const long long rows_total = (long long)B * D;
-  const int num_tiles = (int)((rows_total + BM - 1) / BM);
-  const int tile_iters = (num_tiles + (int)gridDim.x - 1) / (int)gridDim.x;   // identical for both CTAs of a pair (lockstep)
-  const int nsteps = (hk + DX_IPS - 1) / DX_IPS;
-  const uint32_t cta_rank = cluster_ctarank();
-  const bool leader = cta_rank == 0;
-
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < SB; ++s) { mbar_init(full_b(s), 1); mbar_init(empty_b(s), 1); }
-    for (int q = 0; q < DX_DBUF; ++q) { mbar_init(d_full(q), 1); mbar_init(d_empty(q), 8); }   // 4 row-owner warps x 2 CTAs
-    mbar_init(a_full, 8);
-    mbar_init(a_empty, 1);
-    fence_barrier_init();
-  }
-  if (warp == 5) tmem_alloc_2sm(smem_u32(tmem_ptr), 512u);
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();                                  // both CTAs' barriers exist before anything is sent to them
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  const uint32_t d_col0 = tmem_base + 256u;
-
-  if (warp < 4) {
-    // ============================ row owners: stage Gt once per tile, then consume dZ of two i per step ============================
-    const uint32_t lane_sel = (uint32_t)(warp * 32) << 16;
-    const uint32_t a_full_leader = mapa_rank(a_full, 0);
-    uint32_t di = 0;
-    int lt = 0;
-    for (int ti = 0; ti < tile_iters; ++ti, ++lt) {
-      const int tile = blockIdx.x + ti * gridDim.x;          // may be past the end: an all-invalid tile keeps the pipeline in step
-      const long long r = (long long)tile * BM + warp * 32 + lane;
-      const bool valid = tile < num_tiles && r < rows_total;
-      const int b = valid ? (int)(r >> logD) : 0;
-      const int d = (int)(r & (D - 1));
-      float x0v[KB], dx0acc[KB];
-#pragma unroll
-      for (int j = 0; j < KB; ++j) {
-        x0v[j] = (valid && j < m) ? __ldg(x0 + ((size_t)b * m + j) * D + d) : 0.f;
-        dx0acc[j] = 0.f;
-      }
-      mbar_wait(a_empty, (lt & 1) ^ 1);                // MMAs of the previous tile pair no longer read the A columns
-      tc_fence_after();
-      const float* gp = g + (size_t)b * H * D + d;
-#pragma unroll 1
-      for (int n0 = 0; n0 < HP; n0 += 8) {
-        float v[8], h[8];
-#pragma unroll
-        for (int q = 0; q < 8; ++q) {
-          v[q] = (valid && n0 + q < H) ? __ldg(gp + (size_t)(n0 + q) * D) : 0.f;
-          h[q] = tf32_rna(v[q]);
-          v[q] -= h[q];
-        }
-        tmem_st8(tmem_base + lane_sel + (uint32_t)n0, h);
-        tmem_st8(tmem_base + lane_sel + (uint32_t)(HP + n0), v);
-      }
-      tmem_wait_st();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive_cluster(a_full_leader);
-      const float* xkp = xk + (size_t)b * hk * D + d;
-      for (int st = 0; st < nsteps; ++st, ++di) {
-        const int i0 = st * DX_IPS;
-        float xi[DX_IPS];
-#pragma unroll
-        for (int t = 0; t < DX_IPS; ++t) xi[t] = (valid && i0 + t < hk) ? __ldg(xkp + (size_t)(i0 + t) * D) : 0.f;
-        const uint32_t q = di % DX_DBUF;
-        mbar_wait(d_full(q), (di / DX_DBUF) & 1u);
-        tc_fence_after();
-        uint32_t raw[DX_IPS * 2][16];
-#pragma unroll
-        for (int t = 0; t < DX_IPS * 2; ++t) tmem_ld16_nowait(d_col0 + lane_sel + q * DX_N + t * 16, raw[t]);
-        tmem_wait_ld();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive_cluster(mapa_rank(d_empty(q), 0));     // the leader may overwrite buffer q in BOTH CTAs
-#pragma unroll
-        for (int t = 0; t < DX_IPS; ++t) {
-          float s4[4] = {0.f, 0.f, 0.f, 0.f};
-#pragma unroll
-          for (int j = 0; j < KB; ++j) {
-            const float dzv = __uint_as_float(raw[t * 2 + (j >> 4)][j & 15]);
-            s4[j & 3] += dzv * x0v[j];
-            dx0acc[j] += dzv * xi[t];
-          }
-          if (valid && i0 + t < hk) dxk[((size_t)b * hk + i0 + t) * D + d] = (s4[0] + s4[1]) + (s4[2] + s4[3]);
-        }
-      }
-      if (valid) {
-#pragma unroll
-        for (int j = 0; j < KB; ++j)
-          if (j < m) dx0[((size_t)b * m + j) * D + d] = dx0acc[j];
-      }
-    }
-  } else if (warp == 4) {
-    // ============================ TMA: this CTA's half of every filter stage (the rows of i0 + rank), hi and lo ============================
-    if (lane == 0) {
-      int s = 0, ph = 0;
-      for (int ti = 0; ti < tile_iters; ++ti) {
-        for (int st = 0; st < nsteps; ++st) {
-          mbar_wait(empty_b(s), ph ^ 1);
-          const uint32_t dst = sbase + s * stage_bytes;
-          const uint32_t leader_full = mapa_rank(full_b(s), 0);
-          if (leader) mbar_expect_tx(full_b(s), (uint32_t)(2 * stage_bytes));      // both CTAs' halves complete on the leader's barrier
-          tma_load_4d_2sm(dst, &tmap_half, 0, st * DX_IPS * m, (int)cta_rank, 0, leader_full);
-          tma_load_4d_2sm(dst + half_copy_bytes, &tmap_half, 0, KRP + st * DX_IPS * m, (int)cta_rank, 0, leader_full);
-          if (++s == SB) { s = 0; ph ^= 1; }
-        }
-      }
-    }
-  } else if (leader) {
-    // ============================ MMA issuer of the pair: 3 passes x NKB x 4 MMAs of 256x64x8 ============================
-    {
-      const uint32_t idesc = umma_idesc_tf32_m256(DX_N);
-      int s = 0, ph = 0, lt = 0;
-      uint32_t di = 0;
-      for (int ti = 0; ti < tile_iters; ++ti, ++lt) {
-        mbar_wait(a_full, lt & 1);
-        tc_fence_after();
-        for (int st = 0; st < nsteps; ++st, ++di) {
-          const uint32_t q = di % DX_DBUF;
-          mbar_wait(d_empty(q), ((di / DX_DBUF) & 1u) ^ 1u);
-          mbar_wait(full_b(s), ph);
-          tc_fence_after();
-          if (elect_one()) {
-          const uint32_t dcol = d_col0 + q * DX_N;
-          const uint64_t b_hi = umma_desc_sw128(sbase + s * stage_bytes);
-          const uint64_t b_lo = umma_desc_sw128(sbase + s * stage_bytes + half_copy_bytes);
-          const uint32_t a_hi = tmem_base, a_lo = tmem_base + (uint32_t)HP;
-          // sub-tile kb of a CTA's half starts KB*128 bytes (>>4 = 256) further
-#pragma unroll
-          for (int kb = 0; kb < NKB; ++kb)
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-              umma_tf32_ts_2sm(dcol, a_lo + (uint32_t)(kb * KB + 8 * k), b_hi + (uint64_t)(kb * (KB * 128 / 16) + 2 * k), idesc,
-                               (kb | k) != 0 ? 1u : 0u);
-#pragma unroll
-          for (int kb = 0; kb < NKB; ++kb)
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-              umma_tf32_ts_2sm(dcol, a_hi + (uint32_t)(kb * KB + 8 * k), b_lo + (uint64_t)(kb * (KB * 128 / 16) + 2 * k), idesc, 1u);
-#pragma unroll
-          for (int kb = 0; kb < NKB; ++kb)
-#pragma unroll
-            for (int k = 0; k < 4; ++k)
-              umma_tf32_ts_2sm(dcol, a_hi + (uint32_t)(kb * KB + 8 * k), b_hi + (uint64_t)(kb * (KB * 128 / 16) + 2 * k), idesc, 1u);
-          umma_commit_2sm(empty_b(s), (uint16_t)3);
-          umma_commit_2sm(d_full(q), (uint16_t)3);
-          if (st + 1 == nsteps) umma_commit_2sm(a_empty, (uint16_t)3);
-          }
-          __syncwarp();
-          if (++s == SB) { s = 0; ph ^= 1; }
-        }
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  cluster_sync_all();                                  // nobody leaves while the peer may still signal or read it
-  if (warp == 5) {
-    tc_fence_after();
-    tmem_dealloc_2sm(tmem_base, 512u);
   }
 }
 
 // ================================================================================================= dW kernel
-constexpr int DW_THREADS = 384;     // 8 (i,j)-row warps + TMA warp + MMA warp (+2 idle, completes the third warpgroup)
-constexpr int DW_BLOCKS = 2;        // (i,j) blocks of 128 rows per CTA  (= 8 consecutive i)
+constexpr int DW_IPC = NWG * 2;     // i per CTA: each warpgroup owns 64 (i,j) rows = 2 i x 32 j
 
-template <int SB, int NPT, int D>
-__global__ void __launch_bounds__(DW_THREADS, 1)
+template <int N, int D>
+__global__ void __launch_bounds__(NTHREADS, 1)
 cin_bwd_dw_tc_kernel(const __grid_constant__ CUtensorMap tmap_g, const float* __restrict__ x0,
-                     const float* __restrict__ xk, float* __restrict__ dw, int B, int m, int hk, int H, int NP,
-                     int ngroups, int nslices, int chunk) {
+                     const float* __restrict__ xk, float* __restrict__ dw, int B, int m, int hk, int H,
+                     int ngroups, int nslices, int chunk, int SB) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   constexpr int row_bytes = D * 4;                         // one sample's D values of one n-row (= swizzle width)
-  const int b_copy_bytes = NP * row_bytes;
-  const int stage_bytes = 2 * b_copy_bytes;
-  constexpr int SA = 256 / (DW_BLOCKS * 2 * D);            // A stages in TMEM columns [256, 512)
+  constexpr int b_copy_bytes = N * row_bytes;
+  constexpr int stage_bytes = 2 * b_copy_bytes;
   const uint32_t sbase = smem_u32(smem);
   const uint32_t bar0 = sbase + SB * stage_bytes;
   auto full_b = [&](int s) { return bar0 + 8 * s; };
   auto empty_b = [&](int s) { return bar0 + 8 * (SB + s); };
-  auto full_a = [&](int s) { return bar0 + 8 * (2 * SB + s); };
-  auto empty_a = [&](int s) { return bar0 + 8 * (2 * SB + 16 + s); };
-  const uint32_t acc_full = bar0 + 8 * (2 * SB + 32), acc_empty = acc_full + 8;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(smem + SB * stage_bytes + 8 * (2 * SB + 34));
 
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int warp = warp_uniform(threadIdx.x >> 5), lane = threadIdx.x & 31;
   const int group = blockIdx.x % ngroups, slice = blockIdx.x / ngroups;
   const int per_slice = (B + nslices - 1) / nslices;
   const int b_beg = min(B, slice * per_slice), b_end = min(B, b_beg + per_slice);
-  const int nsamp = (slice < nslices) ? b_end - b_beg : 0;
-  const int nch = (nsamp + chunk - 1) / chunk;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < SB; ++s) { mbar_init(full_b(s), 1); mbar_init(empty_b(s), 1); }
-    for (int s = 0; s < 16; ++s) { mbar_init(full_a(s), 8); mbar_init(empty_a(s), 1); }
-    mbar_init(acc_full, 1);
-    mbar_init(acc_empty, 8);
+    for (int s = 0; s < SB; ++s) { mbar_init(full_b(s), 1); mbar_init(empty_b(s), NWG * 4); }
     fence_barrier_init();
   }
-  if (warp == 9) tmem_alloc(smem_u32(tmem_ptr), 512u);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-  const uint32_t a_stage0 = tmem_base + 256u;
 
-  if (warp < 8) {
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
-  } else {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
-  }
-  if (warp < 8) {
-    // ============================ (i,j)-row owners: produce Z^T, drain chunks, final reduction ============================
-    const int t = warp >> 2;                               // block inside the CTA
-    const int row = (warp & 3) * 32 + lane;                // row inside the block = i_local * 32 + j
-    const int i = group * (DW_BLOCKS * 4) + t * 4 + (row >> 5);
-    const int j = row & 31;
-    const bool live = i < hk && j < m;                     // padding rows produce zeros and are never stored
-    const uint32_t lane_sel = (uint32_t)((warp & 3) * 32) << 16;
-    float acc[NPT];
-#pragma unroll
-    for (int n = 0; n < NPT; ++n) acc[n] = 0.f;
-    auto drain = [&](uint32_t gi) {
-      mbar_wait(acc_full, gi & 1u);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + lane_sel + (uint32_t)(t * NP);
-#pragma unroll
-      for (int c0 = 0; c0 < NPT; c0 += 32) {            // two 16-column loads in flight per wait
-        if (c0 < NP) {
-          uint32_t v0[16], v1[16];
-          tmem_ld16_nowait(taddr + c0, v0);
-          if (c0 + 16 < NP) tmem_ld16_nowait(taddr + c0 + 16, v1);
-          tmem_wait_ld();
-#pragma unroll
-          for (int q = 0; q < 16; ++q) acc[c0 + q] += __uint_as_float(v0[q]);
-          if (c0 + 16 < NP) {
-#pragma unroll
-            for (int q = 0; q < 16; ++q) acc[c0 + 16 + q] += __uint_as_float(v1[q]);
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(acc_empty);
-    };
-    int sa = 0, pha = 0;
-    uint32_t gch = 0;
-    float4 pa[D / 4], pb[D / 4];                              // prefetched xk[b,i,:] and x0[b,j,:] (zeros for padding rows)
-#pragma unroll
-    for (int q = 0; q < D / 4; ++q) { pa[q] = make_float4(0.f, 0.f, 0.f, 0.f); pb[q] = pa[q]; }
-    if (live && nsamp > 0) {
-      const float4* xkv = reinterpret_cast<const float4*>(xk + ((size_t)b_beg * hk + i) * D);
-      const float4* x0v = reinterpret_cast<const float4*>(x0 + ((size_t)b_beg * m + j) * D);
-#pragma unroll
-      for (int q = 0; q < D / 4; ++q) { pa[q] = __ldg(xkv + q); pb[q] = __ldg(x0v + q); }
-    }
-    for (int c = 0; c < nch; ++c, ++gch) {
-      const int s_beg = b_beg + c * chunk, s_end = min(b_end, s_beg + chunk);
-      const int drain_at = min(SA, s_end - s_beg);
-      for (int b = s_beg; b < s_end; ++b) {
-        // operands of this sample were requested one sample ago (pa/pb)
-        mbar_wait(empty_a(sa), pha ^ 1);
-        tc_fence_after();
-        const uint32_t a_hi = a_stage0 + lane_sel + (uint32_t)((sa * DW_BLOCKS + t) * 2 * D);
-#pragma unroll
-        for (int c8 = 0; c8 < D; c8 += 8) {
-          float p[8], h[8];
-          const float4 a0 = pa[c8 / 4], a1 = pa[c8 / 4 + 1], b0 = pb[c8 / 4], b1 = pb[c8 / 4 + 1];
-          p[0] = a0.x * b0.x; p[1] = a0.y * b0.y; p[2] = a0.z * b0.z; p[3] = a0.w * b0.w;
-          p[4] = a1.x * b1.x; p[5] = a1.y * b1.y; p[6] = a1.z * b1.z; p[7] = a1.w * b1.w;
-#pragma unroll
-          for (int q = 0; q < 8; ++q) { h[q] = tf32_rna(p[q]); p[q] -= h[q]; }
-          tmem_st8(a_hi + c8, h);
-          tmem_st8(a_hi + D + c8, p);
-        }
-        if (live && b + 1 < b_end) {                       // request the next sample's operands (a whole step ahead of use)
-          const float4* xkv = reinterpret_cast<const float4*>(xk + ((size_t)(b + 1) * hk + i) * D);
-          const float4* x0v = reinterpret_cast<const float4*>(x0 + ((size_t)(b + 1) * m + j) * D);
-#pragma unroll
-          for (int q = 0; q < D / 4; ++q) { pa[q] = __ldg(xkv + q); pb[q] = __ldg(x0v + q); }
-        }
-        tmem_wait_st();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(full_a(sa));
-        if (++sa == SA) { sa = 0; pha ^= 1; }
-        if (c > 0 && b - s_beg + 1 == drain_at) drain(gch - 1);
-      }
-    }
-    if (nch > 0) drain(gch - 1);
-    if (live && nch > 0) {
-      float* dst = dw + ((size_t)i * m + j) * H;
-      if ((H & 3) == 0) {
-#pragma unroll
-        for (int n = 0; n < NPT; n += 4)
-          if (n < H) atomicAdd(reinterpret_cast<float4*>(dst + n), make_float4(acc[n], acc[n + 1], acc[n + 2], acc[n + 3]));
-      } else {
-#pragma unroll
-        for (int n = 0; n < NPT; ++n)
-          if (n < H) atomicAdd(dst + n, acc[n]);
-      }
-    }
-  } else if (warp == 8) {
-    // ============================ TMA: g[b] as [NP rows x D] tiles (hi and lo) ============================
-    if (lane == 0) {
+  if (warp >= NWG * 4) {
+    // ============================ TMA: g[b] as [N rows x D] tiles (hi and lo) ============================
+    setmaxnreg_dec<40>();
+    if (warp == NWG * 4 && lane == 0) {
       int s = 0, ph = 0;
-      for (int b = b_beg; b < b_beg + nsamp; ++b) {
+      for (int b = b_beg; b < b_end; ++b) {
         mbar_wait(empty_b(s), ph ^ 1);
         const uint32_t dst = sbase + s * stage_bytes;
         mbar_expect_tx(full_b(s), (uint32_t)stage_bytes);
@@ -665,53 +247,81 @@ cin_bwd_dw_tc_kernel(const __grid_constant__ CUtensorMap tmap_g, const float* __
         if (++s == SB) { s = 0; ph ^= 1; }
       }
     }
-  } else if (warp == 9) {
-    // ============================ MMA issuer ============================
-    {
-      const uint32_t idesc = umma_idesc_tf32(NP);
-      int sb = 0, phb = 0, sa = 0, pha = 0;
-      uint32_t gch = 0;
-      for (int c = 0; c < nch; ++c, ++gch) {
-        mbar_wait(acc_empty, (gch & 1u) ^ 1u);
-        tc_fence_after();
-        const int s_beg = b_beg + c * chunk, s_end = min(b_end, s_beg + chunk);
-        for (int b = s_beg; b < s_end; ++b) {
-          mbar_wait(full_a(sa), pha);
-          mbar_wait(full_b(sb), phb);
-          tc_fence_after();
-          if (elect_one()) {
-          const uint32_t first = (b == s_beg) ? 0u : 1u;
-          const uint32_t st = sbase + sb * stage_bytes;
-          const uint64_t b_hi = umma_desc_kmajor(st, row_bytes);
-          const uint64_t b_lo = umma_desc_kmajor(st + b_copy_bytes, row_bytes);
+    return;
+  }
+
+  // ============================ (i,j)-row owners: Z^T fragments, wgmma, chunk drains, final reduction ============================
+  setmaxnreg_inc<232>();
+  const int wg = warp >> 2, w = warp & 3, gq = lane >> 2, t = lane & 3;
+  const int i = group * DW_IPC + wg * 2 + (w >> 1);        // rows 16w + gq (+8) of the warpgroup = i_local * 32 + j
+  const int j0 = (w & 1) * 16 + gq, j1 = j0 + 8;
+  const bool live0 = i < hk && j0 < m, live1 = i < hk && j1 < m;   // padding rows produce zeros and are never stored
+  float acc[N / 2], dacc[N / 2];
 #pragma unroll
-          for (int tt = 0; tt < DW_BLOCKS; ++tt) {
-            const uint32_t a_hi = a_stage0 + (uint32_t)((sa * DW_BLOCKS + tt) * 2 * D);
-            const uint32_t a_lo = a_hi + (uint32_t)D;
-            const uint32_t dcol = tmem_base + (uint32_t)(tt * NP);
+  for (int q = 0; q < N / 2; ++q) { acc[q] = 0.f; dacc[q] = 0.f; }
+  int s = 0, ph = 0;
+  // A fragments (hi, lo) of the D/8 k-steps of sample b; fragment columns d = 8k + t + 4h  ->  [2k + h]
+  auto form = [&](int b, uint32_t (&fh)[D / 8][4], uint32_t (&fl)[D / 8][4]) {
+    float xa[D / 4], xb0[D / 4], xb1[D / 4];
 #pragma unroll
-            for (int k = 0; k < D / 8; ++k) umma_tf32_ts(dcol, a_lo + 8 * k, b_hi + 2 * k, idesc, k > 0 ? 1u : first);
+    for (int q = 0; q < D / 4; ++q) {
+      const int d = 8 * (q >> 1) + t + 4 * (q & 1);
+      xa[q] = i < hk ? __ldg(xk + ((size_t)b * hk + i) * D + d) : 0.f;
+      xb0[q] = live0 ? __ldg(x0 + ((size_t)b * m + j0) * D + d) : 0.f;
+      xb1[q] = live1 ? __ldg(x0 + ((size_t)b * m + j1) * D + d) : 0.f;
+    }
 #pragma unroll
-            for (int k = 0; k < D / 8; ++k) umma_tf32_ts(dcol, a_hi + 8 * k, b_lo + 2 * k, idesc, 1u);
+    for (int k = 0; k < D / 8; ++k) {
+      const float a[4] = {xa[2 * k] * xb0[2 * k], xa[2 * k] * xb1[2 * k], xa[2 * k + 1] * xb0[2 * k + 1],
+                          xa[2 * k + 1] * xb1[2 * k + 1]};
+      tf32_split(a, fh[k], fl[k]);
+    }
+  };
+  uint32_t ah[D / 8][4], al[D / 8][4];
+  if (b_end > b_beg) form(b_beg, ah, al);
+  for (int b = b_beg; b < b_end; ++b) {
+    const bool chunk_start = (b - b_beg) % chunk == 0;
+    mbar_wait(full_b(s), ph);
+    const uint64_t bhi = gmma_desc_kmajor(sbase + s * stage_bytes, row_bytes);
+    const uint64_t blo = gmma_desc_kmajor(sbase + s * stage_bytes + b_copy_bytes, row_bytes);
+    wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < D / 8; ++k) umma_tf32_ts(dcol, a_hi + 8 * k, b_hi + 2 * k, idesc, 1u);
-          }
-          umma_commit(empty_a(sa));
-          umma_commit(empty_b(sb));
-          if (b + 1 == s_end) umma_commit(acc_full);
-          }
-          __syncwarp();
-          if (++sa == SA) { sa = 0; pha ^= 1; }
-          if (++sb == SB) { sb = 0; phb ^= 1; }
+    for (int k = 0; k < D / 8; ++k) {
+      const int sc = (chunk_start && k == 0) ? 0 : 1;
+      wgmma_tf32_rs<N>(dacc, al[k], bhi + 2 * k, sc);
+      wgmma_tf32_rs<N>(dacc, ah[k], blo + 2 * k, 1);
+      wgmma_tf32_rs<N>(dacc, ah[k], bhi + 2 * k, 1);
+    }
+    wgmma_commit();
+    // the next sample's loads and fragments overlap this group (ah / al stay live until after the wait)
+    uint32_t bh[D / 8][4], bl[D / 8][4];
+    form(b + 1 < b_end ? b + 1 : b, bh, bl);
+    wgmma_wait<0>();
+#pragma unroll
+    for (int k = 0; k < D / 8; ++k) { wgmma_keep(ah[k]); wgmma_keep(al[k]); }
+    if (lane == 0) mbar_arrive(empty_b(s));
+    if (++s == SB) { s = 0; ph ^= 1; }
+    if ((b + 1 - b_beg) % chunk == 0 || b + 1 == b_end) {
+#pragma unroll
+      for (int q = 0; q < N / 2; ++q) acc[q] += dacc[q];
+    }
+#pragma unroll
+    for (int k = 0; k < D / 8; ++k)
+#pragma unroll
+      for (int q = 0; q < 4; ++q) { ah[k][q] = bh[k][q]; al[k][q] = bl[k][q]; }
+  }
+  if (b_end > b_beg) {
+#pragma unroll
+    for (int c = 0; c < N / 8; ++c) {
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int n = 8 * c + 2 * t + e;
+        if (n < H) {
+          if (live0) atomicAdd(dw + ((size_t)i * m + j0) * H + n, acc[4 * c + e]);
+          if (live1) atomicAdd(dw + ((size_t)i * m + j1) * H + n, acc[4 * c + 2 + e]);
         }
       }
     }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 9) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, 512u);
   }
 }
 
@@ -722,15 +332,6 @@ static int64_t pad_to(int64_t v, int64_t q) { return (v + q - 1) / q * q; }
 
 using namespace ctr;
 using namespace ctr::cinb;
-
-// dX kernel choice: CTA pairs (cta_group::2, default) or the single-CTA multicast form.  Internal; tools/bench_layers.py flips it
-// through ctr_cin_bwd_set_dx_pair for A/B timings (no environment variable is read anywhere in the library).
-static bool g_dx_pair = true;
-extern "C" __attribute__((visibility("default"))) int ctr_cin_bwd_set_dx_pair(int on) {
-  const int old = g_dx_pair ? 1 : 0;
-  g_dx_pair = on != 0;
-  return old;
-}
 
 // Shapes the tensor-core backward serves; everything else goes to the CUDA-core kernels in cin.cu.
 // (internal, not part of the public ABI)
@@ -748,7 +349,8 @@ extern "C" int64_t ctr_cin_bwd_workspace_bytes(int64_t B, int64_t m, int64_t hk,
 int ctr_cin_bwd_tc(const float* x0, const float* xk, const float* filter, const float* g_out, int64_t B, int64_t m,
                    int64_t hk, int64_t D, int64_t H, float* dx0, float* dxk, float* dfilter, void* workspace,
                    cudaStream_t st) {
-  const int HP = (int)pad_to(H, 32), NP = (int)pad_to(H, 16), KRP = (int)((hk + 2) * m + 32);
+  const int HP = (int)pad_to(H, 32), KRP = (int)((hk + 2) * m + 32);
+  const int NP = H <= 32 ? 32 : H <= 64 ? 64 : 128;        // wgmma N of the dW kernel
   float* ws_w = static_cast<float*>(workspace);
   float* ws_g = ws_w + (size_t)(2 * KRP + m) * HP;          // + m rows so the i-in-step window of the lo copy stays inside
   {
@@ -781,75 +383,24 @@ int ctr_cin_bwd_tc(const float* x0, const float* xk, const float* filter, const 
       set_error("ctr_cin_bwd: cuTensorMapEncodeTiled(filter) failed with CUresult %d", (int)cr);
       return CTR_ERR_CUDA;
     }
-    // the same tensor with a ONE-i box: what one CTA of a cta_group::2 pair loads per stage
-    CUtensorMap tmap_half;
-    const cuuint32_t box_half[4] = {32, 32, 1, (cuuint32_t)(HP / 32)};
-    cr = enc(&tmap_half, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, ws_w, gdim, gstr, box_half, es, CU_TENSOR_MAP_INTERLEAVE_NONE,
-             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) {
-      set_error("ctr_cin_bwd: cuTensorMapEncodeTiled(filter, half box) failed with CUresult %d", (int)cr);
-      return CTR_ERR_CUDA;
-    }
     constexpr int SB = 3;
     const int nkb = HP / 32;
-    const int stage_bytes = 2 * nkb * DX_N * 128;
-    const int smem = SB * stage_bytes + 8 * (2 * SB + 2 * DX_DBUF + 2) + 16 + 1024;
+    const int smem = SB * 2 * nkb * DX_N * 128 + 8 * 2 * SB + 1024;
     const long long rows = (long long)B * D;
-    const int tiles = (int)((rows + BM - 1) / BM);
+    const int tiles = (int)((rows + DX_TILE - 1) / DX_TILE);
     const int grid = tiles < sm_count() ? tiles : sm_count();
-    const bool mc = tiles >= 2;
-    if (mc && g_dx_pair) {
-      // CTA pairs (cta_group::2): SB = 6 stages of half the size fit the same shared memory
-      constexpr int SB2 = 6;
-      const int smem2 = SB2 * (stage_bytes / 2) + 8 * (2 * SB2 + 2 * DX_DBUF + 2) + 16 + 1024;
-      int grid2 = grid & ~1;
-      if (grid2 < 2) grid2 = 2;
-#define DX2_LAUNCH(NKB_)                                                                                             \
-  {                                                                                                                  \
-    auto k = cin_bwd_dx_tc2_kernel<SB2, NKB_>;                                                                       \
-    CTR_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem2));                           \
-    cudaLaunchConfig_t cfg = {};                                                                                     \
-    cfg.gridDim = dim3((unsigned)grid2);                                                                             \
-    cfg.blockDim = dim3(DX_THREADS);                                                                                 \
-    cfg.dynamicSmemBytes = (size_t)smem2;                                                                            \
-    cfg.stream = st;                                                                                                 \
-    cudaLaunchAttribute at[1];                                                                                       \
-    at[0].id = cudaLaunchAttributeClusterDimension;                                                                  \
-    at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;                              \
-    cfg.attrs = at; cfg.numAttrs = 1;                                                                                \
-    CTR_CUDA(cudaLaunchKernelEx(&cfg, k, tmap_half, x0, xk, g_out, dx0, dxk, (int)B, (int)m, (int)hk, logD, (int)H, KRP)); \
-  }
-      if (nkb == 1) DX2_LAUNCH(1) else if (nkb == 2) DX2_LAUNCH(2) else if (nkb == 3) DX2_LAUNCH(3) else DX2_LAUNCH(4)
-#undef DX2_LAUNCH
-      CTR_CHECK_LAUNCH("ctr_cin_bwd(dx, tcgen05 cta_group::2)");
-    } else {
-    int grid_mc = grid & ~1;                               // whole 2-CTA clusters
-    if (grid_mc < 2) grid_mc = 2;
 #define DX_LAUNCH(NKB_)                                                                                              \
-  if (mc) {                                                                                                          \
-    auto k = cin_bwd_dx_tc_kernel<SB, NKB_, true>;                                                                   \
+  {                                                                                                                  \
+    auto k = cin_bwd_dx_tc_kernel<SB, NKB_>;                                                                         \
     CTR_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));                            \
-    cudaLaunchConfig_t cfg = {};                                                                                     \
-    cfg.gridDim = dim3((unsigned)grid_mc);                                                                           \
-    cfg.blockDim = dim3(DX_THREADS);                                                                                 \
-    cfg.dynamicSmemBytes = (size_t)smem;                                                                             \
-    cfg.stream = st;                                                                                                 \
-    cudaLaunchAttribute at[1];                                                                                       \
-    at[0].id = cudaLaunchAttributeClusterDimension;                                                                  \
-    at[0].val.clusterDim.x = 2; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;                              \
-    cfg.attrs = at; cfg.numAttrs = 1;                                                                                \
-    CTR_CUDA(cudaLaunchKernelEx(&cfg, k, tmap, x0, xk, g_out, dx0, dxk, (int)B, (int)m, (int)hk, logD, (int)H, KRP)); \
-  } else {                                                                                                           \
-    auto k = cin_bwd_dx_tc_kernel<SB, NKB_, false>;                                                                  \
-    CTR_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));                            \
-    k<<<grid, DX_THREADS, smem, st>>>(tmap, x0, xk, g_out, dx0, dxk, (int)B, (int)m, (int)hk, logD, (int)H, KRP);    \
+    k<<<grid, NTHREADS, smem, st>>>(tmap, x0, xk, g_out, dx0, dxk, (int)B, (int)m, (int)hk, logD, (int)H, KRP);      \
   }
     if (nkb == 1) DX_LAUNCH(1) else if (nkb == 2) DX_LAUNCH(2) else if (nkb == 3) DX_LAUNCH(3) else DX_LAUNCH(4)
 #undef DX_LAUNCH
-    CTR_CHECK_LAUNCH("ctr_cin_bwd(dx, tcgen05)");
-    }
+    CTR_CHECK_LAUNCH("ctr_cin_bwd(dx, wgmma)");
   }
   // ---- dW: g (hi | lo stacked along the batch axis) as a 3-D tensor (d | n | b); box = one sample's [NP x D] tile
+  //      (rows n >= H are out of bounds and arrive as zeros)
   {
     CUtensorMap tmap;
     const cuuint64_t gdim[3] = {(cuuint64_t)D, (cuuint64_t)H, (cuuint64_t)(2 * B)};
@@ -864,28 +415,29 @@ int ctr_cin_bwd_tc(const float* x0, const float* xk, const float* filter, const 
       set_error("ctr_cin_bwd: cuTensorMapEncodeTiled(grad) failed with CUresult %d", (int)cr);
       return CTR_ERR_CUDA;
     }
-    constexpr int SB = 8;
     const int stage_bytes = 2 * NP * (int)D * 4;
-    const int smem = SB * stage_bytes + 8 * (2 * SB + 34) + 16 + 1024;
-    const int ngroups = (int)((hk + DW_BLOCKS * 4 - 1) / (DW_BLOCKS * 4));
+    int sb = (192 * 1024) / stage_bytes;                      // as many stages as 192 KB of shared memory hold, at most 8
+    if (sb > 8) sb = 8;
+    const int smem = sb * stage_bytes + 8 * 2 * sb + 1024;
+    const int ngroups = (int)((hk + DW_IPC - 1) / DW_IPC);
     int nslices = sm_count() / ngroups;
     if (nslices < 1) nslices = 1;
     if (nslices > B) nslices = (int)B;
     const int grid = ngroups * nslices;
     const int chunk = (int)(256 / D);                        // 96 chained MMAs per accumulator before a drain (see cin.cu CHUNK3)
-#define DW_LAUNCH(NPT_, D_)                                                                                          \
+#define DW_LAUNCH(N_, D_)                                                                                            \
   {                                                                                                                  \
-    auto k = cin_bwd_dw_tc_kernel<SB, NPT_, D_>;                                                                     \
+    auto k = cin_bwd_dw_tc_kernel<N_, D_>;                                                                           \
     CTR_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));                            \
-    k<<<grid, DW_THREADS, smem, st>>>(tmap, x0, xk, dfilter, (int)B, (int)m, (int)hk, (int)H, NP, ngroups, nslices,  \
-                                      chunk);                                                                        \
+    k<<<grid, NTHREADS, smem, st>>>(tmap, x0, xk, dfilter, (int)B, (int)m, (int)hk, (int)H, ngroups, nslices, chunk, \
+                                    sb);                                                                             \
   }
-#define DW_LAUNCH_D(NPT_)                                                                                            \
-  if (D == 8) DW_LAUNCH(NPT_, 8) else if (D == 16) DW_LAUNCH(NPT_, 16) else DW_LAUNCH(NPT_, 32)
-    if (NP <= 32) { DW_LAUNCH_D(32) } else if (NP <= 64) { DW_LAUNCH_D(64) } else { DW_LAUNCH_D(128) }
+#define DW_LAUNCH_D(N_)                                                                                              \
+  if (D == 8) DW_LAUNCH(N_, 8) else if (D == 16) DW_LAUNCH(N_, 16) else DW_LAUNCH(N_, 32)
+    if (NP == 32) { DW_LAUNCH_D(32) } else if (NP == 64) { DW_LAUNCH_D(64) } else { DW_LAUNCH_D(128) }
 #undef DW_LAUNCH_D
 #undef DW_LAUNCH
-    CTR_CHECK_LAUNCH("ctr_cin_bwd(dw, tcgen05)");
+    CTR_CHECK_LAUNCH("ctr_cin_bwd(dw, wgmma)");
   }
   return CTR_OK;
 }

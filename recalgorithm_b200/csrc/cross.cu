@@ -3,7 +3,7 @@
 // Reference: cross_layer(x0, xl, index) -- DCN/cross_layer.py:21-24 -- stacked by the loop at
 // DCN/dcn.py:157-160:   x_{l+1} = x0 * (x_l . w_l) + b_l + x_l   (w_l, b_l are (d,1) variables).
 //
-// B200 mapping (HBM/L2-bound, 20*d bytes per sample fwd+bwd; no tensor cores):
+// H100 mapping (HBM/L2-bound, 20*d bytes per sample fwd+bwd; no tensor cores):
 //   forward : one warp per sample, x0 and x_l live in registers (d/32 values per lane), w/b of all layers
 //             staged once per CTA in shared memory, the (B,d)x(d,1) product is a warp-shuffle dot.
 //   backward: phase 1 (warp per sample) re-runs the forward recurrence to get s_l = x_l.w_l, then walks

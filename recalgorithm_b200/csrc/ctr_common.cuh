@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a CTR kernels: error reporting, launch accounting, warp primitives,
+// Shared helpers for the sm_90a CTR kernels: error reporting, launch accounting, warp primitives,
 // cache-hinted 128-bit global accesses.
 #pragma once
 #include <cuda_runtime.h>

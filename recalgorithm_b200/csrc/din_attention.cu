@@ -5,7 +5,7 @@
 //   mask by sequence_mask(keys_length, T); default: weights*mask; softmax variant: fill -2**32+1, THEN /sqrt(H),
 //   softmax over T; out = weights^T . keys  (B,H).
 //
-// B200 mapping (FP32-FMA-bound, CUDA cores; north_star keeps tensor cores for CIN only):
+// H100 mapping (FP32-FMA-bound, CUDA cores; north_star keeps tensor cores for CIN only):
 //   * one warp per sample; the sample's keys (T x H) are staged once in shared memory;
 //   * layer 1 is algebraically folded per sample:  cross@W1 = q@(W1a+W1c) + k@(W1b-W1c) + (q*k)@W1d
 //       = qpart + k @ Weff,  Weff[h,c] = (W1b-W1c)[h,c] + q[h]*W1d[h,c]   (H x 64 per sample, in registers)

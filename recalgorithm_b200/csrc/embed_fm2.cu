@@ -1,12 +1,12 @@
 // Row L + Row FM2 (SURVEY.md section 8a): fused per-field embedding lookup + DeepFM second-order term.
 //
-// Reference semantics being replaced (paths relative to /root/reference/algorithm):
+// Reference semantics being replaced (paths relative to the reference's algorithm/ directory):
 //   * fc.input_layer(features, [embedding_column]) once per field  -- DeepFM/deepfm.py:187-190
 //     (row gather; pruned id -> zero vector; TF-internal, SURVEY A.5)
 //   * square(add_n(e)), add_n(square(e)), reduce_sum(0.5*(a-b), axis=1) -- DeepFM/deepfm.py:192-200
 //   * the gather's IndexedSlices gradient + d(FM2)/d(e) = g*(S - e)
 //
-// B200 mapping (HBM-bound gather; no tensor cores):
+// H100 mapping (HBM-bound gather; no tensor cores):
 //   one warp per sample; a row of D fp32 is LPR = D/4 lanes x 128-bit, so one warp-level LDG.128
 //   fetches RPW = 32/LPR complete rows (D=32: 4 rows x 128 B = 4 full cache lines).  The ids of up
 //   to 32 fields are read with ONE coalesced 8-byte load per lane and distributed by shuffle, so all

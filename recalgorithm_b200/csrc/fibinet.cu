@@ -7,7 +7,7 @@
 //       p_(i,j) = (x_i @ W) * x_j  for (i,j) in combinations(range(F-1), 2)  -> (B, (F-1)(F-2)/2, K)
 //       W = w (K,K) ['all'] | w[i] ['each'] | w[pair index] ['interaction']
 //
-// B200 mapping: both layers are small, HBM/L2-bound CUDA-core kernels (K x K = 16 x 16 weights); SENET runs one
+// H100 mapping: both layers are small, HBM/L2-bound CUDA-core kernels (K x K = 16 x 16 weights); SENET runs one
 // warp per sample with the squeeze/excite vectors in shared memory, bilinear runs one CTA per sample with the
 // sample's (F,K) block and the projected vectors in shared memory and writes the (P,K) output coalesced.
 // Weight gradients are reduced per CTA in shared memory (or registers) and merged with fp32 atomics.
@@ -593,7 +593,7 @@ bilinear_rr_bwd_dw_kernel(const float* __restrict__ x, const float* __restrict__
     const float* xj_p = x + (size_t)j * K + k0;
     const float* g_p = g + (size_t)p * K + k0;
     // software pipeline: the loads of batch n+1 are issued before batch n is multiplied (first form: 81 % of the stall samples sat
-    // on the first use of the loaded g / x_j values -- every batch waited a full DRAM latency, profiles/r2_bilinear_tournament_ncu_full)
+    // on the first use of the loaded g / x_j values -- every batch waited a full DRAM latency)
     auto load = [&](int s0, float (&xi)[SUB][KT], float (&xj)[SUB][KT], float (&gv)[SUB][KT]) {
 #pragma unroll
       for (int u = 0; u < SUB; ++u) {

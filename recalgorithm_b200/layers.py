@@ -10,7 +10,7 @@ below keep those names, argument meanings, variable names/shapes and error behav
         for i in range(params["num_cross_layer"]):
             cross_vec = cross_layer(x0=concat_all, xl=cross_vec, index=i)
 
-Each call is one launch of the matching sm_100a kernel (through recalgorithm_b200.autograd); there
+Each call is one launch of the matching sm_90a kernel (through recalgorithm_b200.autograd); there
 is no other implementation behind these names.
 """
 from __future__ import annotations

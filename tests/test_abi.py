@@ -62,7 +62,7 @@ def test_every_compute_entry_rejects_null_pointers_with_an_error_string():
     from recalgorithm_b200 import _lib
     h = _lib.lib()
     helpers = {"ctr_version", "ctr_last_error", "ctr_kernel_launches", "ctr_device_info", "ctr_enable_peer_access",
-               "ctr_bilinear_set_rr", "ctr_cin_bwd_set_dx_pair", "ctr_cin_fwd_workspace_bytes", "ctr_cin_bwd_workspace_bytes",
+               "ctr_bilinear_set_rr", "ctr_cin_fwd_workspace_bytes", "ctr_cin_bwd_workspace_bytes",
                "ctr_bst_param_count", "ctr_peer_free", "ctr_ipc_close", "ctr_vmm_free", "ctr_vmm_alloc", "ctr_vmm_import",
                "ctr_vmm_granularity"}
     checked = 0

@@ -37,7 +37,7 @@ def test_cross_matches_reference(name):
     assert rel(g["out_f32"], g["out_f64"]) < 1e-6
 
 
-@pytest.mark.parametrize("name", ["cin_m8_D8_50x50x50", "cin_m30_D16_128x128", "cin_m8_D16_17"])
+@pytest.mark.parametrize("name", ["cin_m8_D8_50x50x50", "cin_m10_D16_128x128", "cin_m8_D16_17"])
 def test_cin_matches_reference(name):
     g = load(name)
     n = int(g["n_layers"])
@@ -370,24 +370,40 @@ def test_adam_restatement_agrees_with_torch_adam(lazy):
         p_prev = var.copy()
 
 
-@pytest.mark.skipif(not os.path.isdir("/root/reference/algorithm"), reason="the reference checkout only exists in the builder container")
+def _array_digest(a):
+    import hashlib
+    return f"{a.dtype.str}:{'x'.join(map(str, a.shape))}:{hashlib.sha256(a.tobytes()).hexdigest()}"
+
+
 def test_fixtures_regenerate_bit_identically_from_the_reference(tmp_path):
-    """oracle/make_golden.py imports / exec()s the reference's own files over the TF1 shim: run it again (in a subprocess, into a
-    scratch directory) and compare every .npz with the committed fixture, array by array, bit for bit."""
+    """oracle/make_golden.py imports / exec()s the reference's own files over the TF1 shim.  Every array of every committed
+    fixture must be bit-identical to that run of the reference, recorded as SHA-256 digests in reference_digests.json.  With
+    RECALG_REFERENCE pointing at a reference checkout's algorithm/ directory the script is also run again (in a subprocess,
+    into a scratch directory) and its output is held to the same digests."""
+    import json
     import subprocess
     import sys
+    want = json.load(open(os.path.join(G, "reference_digests.json")))
+    committed = sorted(glob.glob(os.path.join(G, "*.npz")))
+    assert [os.path.basename(p) for p in committed] == sorted(want) and len(committed) >= 28
+
+    def check(paths):
+        for p in paths:
+            z = np.load(p, allow_pickle=False)
+            assert {k: _array_digest(z[k]) for k in z.files} == want[os.path.basename(p)], os.path.basename(p)
+
+    check(committed)
+    ref = os.environ.get("RECALG_REFERENCE")
+    if not ref:
+        return
     root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
     code = ("import sys, runpy; sys.argv=['make_golden']; import importlib.util as u;"
             f"s=u.spec_from_file_location('mg', r'{root}/oracle/make_golden.py'); m=u.module_from_spec(s); s.loader.exec_module(m);"
             f"m.OUT=r'{tmp_path}';"
             "[getattr(m, f)() for f in ('gen_cross','gen_cin','gen_din','gen_fibinet','gen_restated','gen_inline','gen_bst','gen_ffm')]")
-    out = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=900, cwd=root)
+    out = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, timeout=900, cwd=root,
+                         env={**os.environ, "RECALG_REFERENCE": ref})
     assert out.returncode == 0, out.stderr[-2000:]
     made = sorted(glob.glob(os.path.join(str(tmp_path), "*.npz")))
-    committed = sorted(glob.glob(os.path.join(G, "*.npz")))
-    assert [os.path.basename(p) for p in made] == [os.path.basename(p) for p in committed] and len(made) >= 28
-    for a, b in zip(made, committed):
-        x, y = np.load(a, allow_pickle=False), np.load(b, allow_pickle=False)
-        assert sorted(x.files) == sorted(y.files), os.path.basename(a)
-        for k in x.files:
-            assert x[k].dtype == y[k].dtype and x[k].shape == y[k].shape and x[k].tobytes() == y[k].tobytes(), (os.path.basename(a), k)
+    assert [os.path.basename(p) for p in made] == sorted(want)
+    check(made)

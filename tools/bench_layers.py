@@ -2,7 +2,7 @@
 """Per-layer timings of the non-headline BASELINE configs (2: DCN cross, 3: xDeepFM CIN, 4: DIN attention) and FiBiNET.
 
 Each kernel is timed alone with CUDA events; an L2 flush (a 256 MB write) runs between timed iterations because these
-working sets fit the 126 MB L2.  Prints one JSON line per measurement; meant to be redirected into profiles/.
+working sets are flushed from the 50 MB L2.  Prints one JSON line per measurement.
 
     python tools/bench_layers.py [--iters 20] [--only cin,dcn,din,fibinet]
 """
@@ -20,11 +20,10 @@ from recalgorithm_b200 import ops  # noqa: E402
 
 
 def peaks():
-    try:
-        d = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-        return d["hbm_gbs"], d["bf16_tflops"], "measured"
-    except Exception:
-        return 6650.0, 1590.0, "fallback"
+    """HBM GB/s and bf16 TFLOP/s: MEASURED_PEAKS.json when present, else the H100 SXM data sheet (bench.measured_peaks)."""
+    from bench import measured_peaks
+    d = measured_peaks()
+    return d["hbm_gbs"], d["bf16_tflops"], d["source"]
 
 
 def timeit(fn, iters, flush):
@@ -33,7 +32,7 @@ def timeit(fn, iters, flush):
     torch.cuda.synchronize()
     times = []
     for _ in range(iters):
-        flush.zero_()                                   # 256 MB write: evicts the 126 MB L2
+        flush.zero_()                                   # 256 MB write: evicts the 50 MB L2
         a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         a.record(); fn(); b.record()
         torch.cuda.synchronize()
@@ -92,14 +91,10 @@ def main():
             emit(f"cin_fwd_layer1_{tag}", {"B": B, "m": mm, "hk": mm, "D": D, "H": H}, m, bst, flops=2.0 * B * D * mm * mm * H)
             m, bst = timeit(lambda: ops.cin_fwd(x0, x1, w2, want_pooled=True, precision=prec), args.iters, flush)
             emit(f"cin_fwd_layer2_{tag}", {"B": B, "m": mm, "hk": H, "D": D, "H": H}, m, bst, flops=2.0 * B * D * H * mm * H)
-        for pair in (1, 0):
-            ops._lib.lib().ctr_cin_bwd_set_dx_pair(pair)
-            tag = "dx=cta_group::2 pairs" if pair else "dx=single CTA + multicast"
-            m, bst = timeit(lambda: ops.cin_bwd(x0, x0, w1, g), max(3, args.iters // 4), flush)
-            emit("cin_bwd_layer1", {"B": B, "m": mm, "hk": mm, "D": D, "H": H, "variant": tag}, m, bst, flops=4.0 * B * D * mm * mm * H)
-            m, bst = timeit(lambda: ops.cin_bwd(x0, x1, w2, g), max(3, args.iters // 4), flush)
-            emit("cin_bwd_layer2", {"B": B, "m": mm, "hk": H, "D": D, "H": H, "variant": tag}, m, bst, flops=4.0 * B * D * H * mm * H)
-        ops._lib.lib().ctr_cin_bwd_set_dx_pair(1)
+        m, bst = timeit(lambda: ops.cin_bwd(x0, x0, w1, g), max(3, args.iters // 4), flush)
+        emit("cin_bwd_layer1", {"B": B, "m": mm, "hk": mm, "D": D, "H": H}, m, bst, flops=4.0 * B * D * mm * mm * H)
+        m, bst = timeit(lambda: ops.cin_bwd(x0, x1, w2, g), max(3, args.iters // 4), flush)
+        emit("cin_bwd_layer2", {"B": B, "m": mm, "hk": H, "D": D, "H": H}, m, bst, flops=4.0 * B * D * H * mm * H)
 
     if "din" in only:   # BASELINE config 4: DIN attention, seq_len 50, H=16, batch 4096
         B, T, H = 4096, 50, 16

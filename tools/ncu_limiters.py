@@ -2,7 +2,7 @@
 """What bounds each kernel, from `ncu --set full` captures: issue-slot use, the top warp-stall reasons (warps stalled per issued
 instruction), achieved occupancy, cache hit rates and the DRAM / tensor-pipe / FMA-pipe utilisation, one row per kernel.
 
-    python tools/ncu_limiters.py gpurun_out/a.ncu-rep [gpurun_out/b.ncu-rep ...] > profiles/r2_kernel_limiters.md
+    python tools/ncu_limiters.py a.ncu-rep [b.ncu-rep ...] > kernel_limiters.md
 """
 import csv
 import os

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Summarise an .ncu-rep (captured under gpurun) into a small CSV that is committed under profiles/.
+"""Summarise an Nsight Compute report (.ncu-rep) into a small CSV.
 
-    python tools/ncu_summary.py gpurun_out/prof.ncu-rep profiles/r1_xxx.summary.csv
+    python tools/ncu_summary.py prof.ncu-rep prof.summary.csv
 """
 import csv
 import subprocess

@@ -1,7 +1,7 @@
-// Peer-memory micro-benchmark for the row-sharded path (SURVEY 8e): how fast can one B200 PULL random 128-byte rows
+// Peer-memory micro-benchmark for the row-sharded path (SURVEY 8e): how fast can one H100 PULL random 128-byte rows
 // from / PUSH 128-byte rows to its NVLink peers, by access method?  Standalone (no torch): one process drives all GPUs.
 //
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -std=c++17 -o tools/peerbench tools/peerbench.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -std=c++17 -o tools/peerbench tools/peerbench.cu
 //   tools/peerbench [shard_GB=8] [nreq=2621440] [reps=5]
 //
 // Every GPU runs the same kernel at the same time (all-to-all pattern: rank r pulls from / pushes to all other ranks,

@@ -2,7 +2,7 @@
 """Registers / stack / static shared memory of every kernel in the in-tree objects (cuobjdump --dump-resource-usage), demangled:
 the static side of occupancy -- no GPU needed.
 
-    python tools/resource_usage.py > profiles/r2_resource_usage.txt
+    python tools/resource_usage.py
 """
 import glob
 import os
@@ -18,7 +18,7 @@ def demangle(names):
 
 
 def main():
-    print("# cuobjdump --dump-resource-usage of recalgorithm_b200/csrc/*.o (sm_100a); produced by tools/resource_usage.py")
+    print("# cuobjdump --dump-resource-usage of recalgorithm_b200/csrc/*.o (sm_90a); produced by tools/resource_usage.py")
     print("# 64 K registers and 64 resident warps per SM: a CTA of W warps at R registers/thread fits floor(65536 / (32*W*ceil8(R))) times")
     for obj in sorted(glob.glob(os.path.join(ROOT, "recalgorithm_b200", "csrc", "*.o"))):
         txt = subprocess.run(["cuobjdump", "--dump-resource-usage", obj], capture_output=True, text=True).stdout

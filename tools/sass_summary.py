@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""Counts the Blackwell-specific SASS mnemonics per object of libctr_b200.so (evidence for the tcgen05 / TMA / TMEM claims;
-B200_PROFILING.md "What proves a Blackwell-native kernel").  Runs without a GPU:
+"""Counts the Hopper-specific SASS mnemonics per object of libctr_b200.so (evidence that the tensor-core kernels issue wgmma
+(HGMMA) and TMA (UTMALDG) and wait on mbarriers (SYNCS)).  Runs without a GPU:
 
-    python tools/sass_summary.py > profiles/r2_sass_summary.txt
+    python tools/sass_summary.py
 """
 from __future__ import annotations
 
@@ -15,9 +15,9 @@ import sys
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "recalgorithm_b200", "csrc")
-PATTERNS = [("UTCHMMA", r"\bUTCHMMA"), ("UTCHMMA.2CTA", r"\bUTCHMMA\.2CTA"), ("BRA.U.ANY(elect retry loops)", r"BRA\.U\.ANY"), ("UTC*MMA(other)", r"\bUTC(?!HMMA|BAR)[A-Z]*MMA"), ("LDTM", r"\bLDTM"), ("STTM", r"\bSTTM"),
-            ("UTMALDG", r"\bUTMALDG"), ("UTMALDG.MULTICAST", r"\bUTMALDG\S*MULTICAST"), ("UTMASTG", r"\bUTMASTG"), ("UBLKCP", r"\bUBLKCP"),
-            ("UTCBAR", r"\bUTCBAR"), ("SYNCS", r"\bSYNCS"), ("LDGSTS", r"\bLDGSTS"), ("HMMA(legacy)", r"\bHMMA"),
+PATTERNS = [("HGMMA", r"\bHGMMA"), ("WARPGROUP.ARRIVE", r"\bWARPGROUP\.ARRIVE"), ("WARPGROUP.DEPBAR", r"\bWARPGROUP\.DEPBAR"),
+            ("UTMALDG", r"\bUTMALDG"), ("UTMASTG", r"\bUTMASTG"), ("UBLKCP", r"\bUBLKCP"),
+            ("SYNCS", r"\bSYNCS"), ("LDGSTS", r"\bLDGSTS"), ("HMMA(mma.sync)", r"\bHMMA"),
             ("LDG.E.128", r"\bLDG\.E\S*\.128"), ("STG.E.128", r"\bSTG\.E\S*\.128"), ("RED/ATOM", r"\b(RED|ATOM)G?\.")]
 
 
@@ -25,7 +25,7 @@ def main():
     objs = sorted(glob.glob(os.path.join(CSRC, "*.o")))
     if not objs:
         sys.exit("no objects: run `python -c 'import __graft_entry__ as g; g.build()'` first")
-    print("# SASS mnemonic counts per object (cuobjdump -sass, sm_100a); produced by tools/sass_summary.py")
+    print("# SASS mnemonic counts per object (cuobjdump -sass, sm_90a); produced by tools/sass_summary.py")
     print("# columns: " + ", ".join(n for n, _ in PATTERNS))
     for o in objs:
         sass = subprocess.run(["cuobjdump", "-sass", o], capture_output=True, text=True).stdout
@@ -47,7 +47,7 @@ def main():
             tot.update(c)
         print(f"\n## {os.path.basename(o)}: {len(per_kernel)} kernels; " + ", ".join(f"{n}={tot[n]}" for n, _ in PATTERNS if tot[n]))
         for k, c in per_kernel.items():
-            hot = {n: c[n] for n in ("UTCHMMA", "UTCHMMA.2CTA", "BRA.U.ANY(elect retry loops)", "UTC*MMA(other)", "LDTM", "STTM", "UTMALDG", "UTMASTG", "UBLKCP", "UTCBAR", "HMMA(legacy)") if c[n]}
+            hot = {n: c[n] for n in ("HGMMA", "WARPGROUP.ARRIVE", "UTMALDG", "UTMASTG", "UBLKCP", "HMMA(mma.sync)") if c[n]}
             if hot:
                 dem = subprocess.run(["cu++filt", k], capture_output=True, text=True).stdout.strip() or k
                 print(f"   {dem[:150]}: " + ", ".join(f"{n}={v}" for n, v in hot.items()))

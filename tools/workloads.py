@@ -4,6 +4,7 @@ dcn_cfg2|xdeepfm_cfg3|din_cfg4` and the `configs` key of the default line) and t
 Every builder returns a dict:
     step(ev=None)   one forward+backward pass of the chain on the current stream; `ev` (list of CUDA events, len = n_marks)
                     is recorded between the stages so the caller can split the step per kernel
+    outputs         name -> tensor: what the last step computed (bench.py --dump-outputs)
     marks           names of the stages between consecutive events
     B, config       batch and the config keys for the JSON line
     roofline(ms_by_stage, ms_step, peaks) -> dict   the roofline object of the dominant kernel
@@ -22,7 +23,7 @@ import torch  # noqa: E402
 
 from recalgorithm_b200 import ops  # noqa: E402
 
-FP32_FMA_TFLOPS = 148 * 128 * 2 * 1.965e9 / 1e12     # 148 SMs x 128 FMA lanes x 2 FLOP x 1.965 GHz = 74.4 TFLOP/s (nominal)
+FP32_FMA_TFLOPS = 132 * 128 * 2 * 1.98e9 / 1e12      # H100 SXM: 132 SMs x 128 FMA lanes x 2 FLOP x 1.98 GHz = 66.9 TFLOP/s (nominal)
 
 
 def _rn(gen, *s, std=1.0):
@@ -46,13 +47,15 @@ def build_dcn_cfg2(rows=1_000_000, B=4096):
     k = [0]
 
     x0, xl = torch.empty((B, d), device="cuda"), torch.empty((B, d), device="cuda")
+    outputs = {"x0": x0, "cross_out": xl}
 
     def step(ev=None):
         k[0] += 1
         _rec(ev, 0)
         ops.embed_cross_fwd(table, off, ids[k[0] % 4], w, bb, x0=x0, out=xl)     # input_layer gather + the cross loop, ONE launch
         _rec(ev, 1)
-        dx0, _, _, _ = ops.cross_bwd(x0, w, bb, g)
+        dx0, _, dw, db = ops.cross_bwd(x0, w, bb, g)
+        outputs.update(d_x0=dx0, d_w=dw, d_b=db)
         _rec(ev, 2)
         # lookup backward of a plain gather (no FM2 term): the IndexedSlices values ARE dx0.view(B,F,D) -- no kernel, no bytes
         _rec(ev, 3)
@@ -66,15 +69,15 @@ def build_dcn_cfg2(rows=1_000_000, B=4096):
                 "unit": "GB/s", "frac": ach / peaks["hbm_gbs"], "traffic": None, "algorithmic_bytes_per_launch": B * 3 * d * 4,
                 "avg_launch_ms": ms["cross_bwd"], "step_algorithmic_GBps": step_gbs, "step_frac": step_gbs / peaks["hbm_gbs"],
                 "step_bytes_per_sample": bytes_step // B,
-                "note": "79 MB per step fits the 126 MB L2; two kernel launches (fused lookup+cross forward, cross backward) + 2 memsets: launch/latency-bound, see DESIGN 4.3"}
+                "note": "79 MB per step (more than the 50 MB L2); two kernel launches (fused lookup+cross forward, cross backward) + 2 memsets: launch/latency-bound, see DESIGN 4.3"}
 
-    return {"step": step, "marks": ["lookup+cross_fwd", "cross_bwd", "lookup_bwd"], "B": B, "roofline": roofline,
+    return {"step": step, "outputs": outputs, "marks": ["lookup+cross_fwd", "cross_bwd", "lookup_bwd"], "B": B, "roofline": roofline,
             "config": {"workload": "dcn_cfg2", "model": "DCN lookup + 3 cross layers", "B": B, "F": F, "D": D, "d": d, "L": L,
                        "rows_per_field": rows, "ids": "uniform int64"}, "dtype": "f32"}
 
 
 def build_xdeepfm_cfg3(rows=1_000_000, B=8192):
-    """Config 3: xDeepFM CIN [128,128], 30 fields x 16 (xDeepFM/xdeepfm.py:166-175), 3xTF32 on tcgen05."""
+    """Config 3: xDeepFM CIN [128,128], 30 fields x 16 (xDeepFM/xdeepfm.py:166-175), 3xTF32 on wgmma."""
     gen = torch.Generator(device="cuda").manual_seed(1234)
     F, D, H = 30, 16, 128
     table = _rn(gen, rows * F, D, std=D ** -0.5)
@@ -83,6 +86,7 @@ def build_xdeepfm_cfg3(rows=1_000_000, B=8192):
     w1, w2 = _rn(gen, F * F, H, std=0.05), _rn(gen, H * F, H, std=0.05)
     gp = _rn(gen, B, 2 * H)
     k = [0]
+    outputs = {}
 
     def step(ev=None):
         k[0] += 1
@@ -93,12 +97,13 @@ def build_xdeepfm_cfg3(rows=1_000_000, B=8192):
         x2, p2 = ops.cin_fwd(x0, x1, w2, want_pooled=True)
         _rec(ev, 2)
         g2 = gp[:, H:].unsqueeze(-1).expand(B, H, D).contiguous()          # d(pooled)/d(out) broadcast over D
-        dx0b, dx1, _ = ops.cin_bwd(x0, x1, w2, g2)
+        dx0b, dx1, dw2 = ops.cin_bwd(x0, x1, w2, g2)
         g1 = dx1 + gp[:, :H].unsqueeze(-1)
-        dx0a, dxk, _ = ops.cin_bwd(x0, x0, w1, g1.contiguous())
+        dx0a, dxk, dw1 = ops.cin_bwd(x0, x0, w1, g1.contiguous())
         _rec(ev, 3)
-        _values = dx0a + dxk + dx0b                                         # sum of the three paths into x0 = the IndexedSlices values
+        values = dx0a + dxk + dx0b                                          # sum of the three paths into x0 = the IndexedSlices values
         _rec(ev, 4)
+        outputs.update(x2=x2, pooled_1=p1, pooled_2=p2, d_filter_1=dw1, d_filter_2=dw2, d_x0=values)
 
     flops_fwd = 2.0 * B * D * (F * F * H + H * F * H)
     flops_step = 3.0 * flops_fwd                                          # backward = dX + dW = 2x forward
@@ -106,7 +111,7 @@ def build_xdeepfm_cfg3(rows=1_000_000, B=8192):
     def roofline(ms, ms_step, peaks):
         ach = flops_step / ((ms["cin_fwd"] + ms["cin_bwd"]) * 1e-3) / 1e12
         pk = peaks["bf16_tflops_sustained"]
-        return {"bound": "tensor", "kernel": "cin_fwd_tc_kernel + cin_bwd_dx/dw_tc_kernel (tcgen05 kind::tf32, 3xTF32)",
+        return {"bound": "tensor", "kernel": "cin_fwd_tc_kernel + cin_bwd_dx/dw_tc_kernel (wgmma kind tf32, 3xTF32)",
                 "achieved": ach, "peak": pk, "unit": "TFLOP/s", "frac": ach / pk, "traffic": None,
                 "algorithmic_flops_per_step": flops_step, "cin_fwd_ms": ms["cin_fwd"], "cin_bwd_ms": ms["cin_bwd"],
                 "executed_over_algorithmic": 3.0, "tf32_rate_over_bf16": 0.5,
@@ -114,7 +119,7 @@ def build_xdeepfm_cfg3(rows=1_000_000, B=8192):
                 "note": "fp32-class accuracy costs 3 TF32 MMAs per product at half the bf16 rate: the ceiling of this "
                         "formulation is peak/6; peak = bf16_tflops_sustained (kernels timed inside a step)"}
 
-    return {"step": step, "marks": ["lookup_fwd", "cin_fwd", "cin_bwd", "lookup_bwd"], "B": B, "roofline": roofline,
+    return {"step": step, "outputs": outputs, "marks": ["lookup_fwd", "cin_fwd", "cin_bwd", "lookup_bwd"], "B": B, "roofline": roofline,
             "config": {"workload": "xdeepfm_cfg3", "model": "xDeepFM lookup + CIN [128,128]", "B": B, "m": F, "D": D, "cin": [H, H],
                        "rows_per_field": rows, "ids": "uniform int64", "precision": "3xTF32 (fp32-class, <=1e-5)"}, "dtype": "f32 (3xTF32 MMA)"}
 
@@ -138,6 +143,7 @@ def build_din_cfg4(rows=1_000_000, B=4096):
           _rn(gen, 32, 1, std=0.3), _rn(gen, 1, std=0.1)]
     go = _rn(gen, B, Hd)
     k = [0]
+    outputs = {}
 
     def step(ev=None):
         k[0] += 1
@@ -148,8 +154,9 @@ def build_din_cfg4(rows=1_000_000, B=4096):
         _rec(ev, 1)
         out, att = ops.din_attention_fwd(q2, k3, lens, *ws, want_weights=True)
         _rec(ev, 2)
-        dq, dk, _ = ops.din_attention_bwd(q2, k3, lens, *ws, go, att_w=att)
+        dq, dk, dws = ops.din_attention_bwd(q2, k3, lens, *ws, go, att_w=att)
         _rec(ev, 3)
+        outputs.update(out=out, att_weights=att, d_query=dq, d_keys=dk, **{f"d_w{i}": t for i, t in enumerate(dws)})
         # lookup backward of a plain gather: the IndexedSlices values are dk / dq themselves (no kernel, no bytes)
         _rec(ev, 4)
 
@@ -167,10 +174,10 @@ def build_din_cfg4(rows=1_000_000, B=4096):
                 "frac": ach / FP32_FMA_TFLOPS, "traffic": None, "executed_flops_bwd": fl_bwd_exec, "executed_flops_fwd": fl_fwd_exec,
                 "reference_counted_flops_fwd": fl_ref, "fwd_TFLOPs_executed": fl_fwd_exec / (ms["din_fwd"] * 1e-3) / 1e12,
                 "fwd_GBps": by_fwd / (ms["din_fwd"] * 1e-3) / 1e9, "din_fwd_ms": ms["din_fwd"], "din_bwd_ms": ms["din_bwd"],
-                "peak_source": "nominal: 148 SMs x 128 FMA/clk x 2 x 1.965 GHz (no measured fp32 peak in MEASURED_PEAKS.json)",
+                "peak_source": "nominal: 132 SMs x 128 FMA/clk x 2 x 1.98 GHz (no measured fp32 peak in MEASURED_PEAKS.json)",
                 "note": "FLOPs are the EXECUTED ones (folded layer 1, masked positions skipped), not the reference's count"}
 
-    return {"step": step, "marks": ["lookup_fwd", "din_fwd", "din_bwd", "lookup_bwd"], "B": B, "roofline": roofline,
+    return {"step": step, "outputs": outputs, "marks": ["lookup_fwd", "din_fwd", "din_bwd", "lookup_bwd"], "B": B, "roofline": roofline,
             "config": {"workload": "din_cfg4", "model": "DIN lookup + attention", "B": B, "T": T, "H": Hd, "rows": rows,
                        "lengths": "uniform{0..50}", "ids": "uniform int64", "softmax": False}, "dtype": "f32"}
 

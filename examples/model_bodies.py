@@ -102,3 +102,24 @@ def fibinet_logit(dense_input, category_input, embedding_dim: int, reduction_rat
             net = dense(net, unit, activation=torch.relu, name=f"dense_{i}" if i else "dense")
         fibinet = dense(net, 1, name="logit")
     return linear_logit + fibinet                                                         # :199
+
+
+def pnn_logit(fields_embeddings, num_fields: int, embedding_dim: int, output_dimension: int = 1024, product_method: str = "IPNN",
+              hidden_units=(64, 32), weight_regularizer: float = 0.0):
+    """PNN/pnn.py:125-193.  fields_embeddings: (B, F*K) concatenated input_layer outputs (or the (B, F, K) tile).  Returns
+    (logit, regularization_loss): the reference's l2_regularizer(scale) on linear_w and the product weight (:137,150,164)
+    contributes scale * sum(w**2) / 2 per weight to REGULARIZATION_LOSSES when scale > 0, and nothing at the default 0.0."""
+    product_final = L.pnn_product_layer(fields_embeddings, num_fields, embedding_dim, output_dimension,
+                                        product_method=product_method)                        # :125-181, one kernel
+    with L.variable_scope("fcn"):                                                         # :184-193 (TF names dense, dense_1, ...)
+        net = product_final
+        for i, unit in enumerate(hidden_units):
+            net = dense(net, unit, activation=torch.relu, name=f"dense_{i}" if i else "dense")
+        logit = dense(net, 1, name=f"dense_{len(hidden_units)}" if hidden_units else "dense")
+    reg = logit.new_zeros(())
+    if weight_regularizer > 0:
+        store = L.default_store()
+        prod = "product_part/inner_product_w" if product_method == "IPNN" else "product_part/outer_product_w"
+        for name in ("linear_part/linear_w", prod):
+            reg = reg + weight_regularizer * 0.5 * store.vars[store.full_name(name)].pow(2).sum()
+    return logit, reg

@@ -273,6 +273,25 @@ int ctr_cin_bwd(const float* x0, const float* xk, const float* filter, const flo
                 void* workspace, int64_t workspace_bytes, void* stream);
 int64_t ctr_cin_bwd_workspace_bytes(int64_t B, int64_t m, int64_t hk, int64_t D, int64_t H);
 
+/* ---- PNN product layer (IPNN / OPNN) ---------------------------------------------------------------
+ * Replaces the product layer of pnn_model_fn (PNN/pnn.py:125-181):
+ *   out = relu(e_flat . wlin + lp + bias)  (B,N),  e (B, F*K) = the fields' embeddings concatenated (field f = columns
+ *   f*K .. f*K+K-1), wlin (F*K, N) = linear_part/linear_w, bias (N,);
+ *   method 0 = IPNN: wprod = product_part/inner_product_w theta (N,F),  lp[b,n] = sum_k (sum_f theta[n,f] e[b,f,k])^2;
+ *   method 1 = OPNN: wprod = product_part/outer_product_w W (N,K,K), s = sum_f e_f,
+ *                    lp[b,n] = sum_kl s_k s_l W[n, min(k,l), max(k,l)]   (only the upper triangle of each W_n is read).
+ * fp32-class accuracy (3xTF32 on the tensor cores where F*K + Q + 1 <= 128, Q = F(F+1)/2 (IPNN) or K(K+1)/2 (OPNN), and
+ * N % 4 == 0; CUDA-core kernels otherwise).  workspace: ctr_pnn_workspace_bytes() bytes, 128-byte aligned; it holds the
+ * derived weights and the weight-gradient accumulator.  The backward takes the forward's out (its relu mask) and g_out
+ * (B,N) -- 16-byte aligned on the tensor path -- and overwrites d_e (B, F*K), d_wlin (F*K, N), d_wprod (the shape of
+ * wprod; the strictly lower triangle of each OPNN W_n gets exactly 0) and d_bias (N,). */
+int ctr_pnn_workspace_bytes(int64_t F, int64_t K, int64_t N, int method, int64_t* bytes);
+int ctr_pnn_fwd(const float* e, const float* wlin, const float* wprod, const float* bias, int64_t B, int64_t F, int64_t K,
+                int64_t N, int method, float* out, void* workspace, int64_t workspace_bytes, void* stream);
+int ctr_pnn_bwd(const float* e, const float* wlin, const float* wprod, const float* out, const float* g_out, int64_t B,
+                int64_t F, int64_t K, int64_t N, int method, float* d_e, float* d_wlin, float* d_wprod, float* d_bias,
+                void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ---- Row DIN-ATT: DIN attention unit -----------------------------------------------------------------
  * Replaces din_attention(query, keys, keys_length, is_softmax) (DIN/din_attention.py:17-43).
  * query (B,H); keys (B,T,H); keys_length int64 (B); dense layers f1_att (4H->64, relu), f2_att (64->32,

@@ -87,6 +87,9 @@ SIGNATURES = {
     "ctr_bilinear_fwd": (c_int, [_P, _P, _I, _I, _I, c_int, _P, _P]),
     "ctr_bilinear_bwd": (c_int, [_P, _P, _P, _I, _I, _I, c_int, _P, _P, _P]),
     "ctr_bilinear_set_rr": (c_int, [c_int]),
+    "ctr_pnn_workspace_bytes": (c_int, [_I, _I, _I, c_int, POINTER(c_int64)]),
+    "ctr_pnn_fwd": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, c_int, _P, _P, _I, _P]),
+    "ctr_pnn_bwd": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, c_int, _P, _P, _P, _P, _P, _I, _P]),
 }
 
 

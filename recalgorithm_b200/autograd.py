@@ -389,3 +389,24 @@ class _FFM(torch.autograd.Function):
 def ffm(tile: torch.Tensor) -> torch.Tensor:
     """(B, F, F-1, K) field/slot tile -> FFM second-order logit (B,1)."""
     return _FFM.apply(tile)
+
+
+class _PNN(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, e, wlin, wprod, bias, method):
+        e, wlin, wprod, bias = e.contiguous(), wlin.contiguous(), wprod.contiguous(), bias.contiguous()
+        out = ops.pnn_fwd(e, wlin, wprod, bias, method)
+        ctx.save_for_backward(e, wlin, wprod, out)           # out carries the relu mask of the backward
+        ctx.method = method
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        e, wlin, wprod, out = ctx.saved_tensors
+        d_e, d_wlin, d_wprod, d_bias = ops.pnn_bwd(e, wlin, wprod, out, g.contiguous(), ctx.method)
+        return d_e, d_wlin, d_wprod, d_bias, None
+
+
+def pnn(e: torch.Tensor, wlin: torch.Tensor, wprod: torch.Tensor, bias: torch.Tensor, method: int) -> torch.Tensor:
+    """PNN product layer: (B,F,K) field embeddings -> relu(lz + lp + bias) (B,N); method 0 = IPNN, 1 = OPNN."""
+    return _PNN.apply(e, wlin, wprod, bias, method)

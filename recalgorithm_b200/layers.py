@@ -244,6 +244,33 @@ def bst_transformer(queries: torch.Tensor, keys: torch.Tensor, values: torch.Ten
     return autograd.bst_transformer(queries, keys, values, keys_length.to(torch.int64), p, heads, max_length, use_position_embedding)
 
 
+# --------------------------------------------------------------------------------------------------- PNN
+def pnn_product_layer(fields_embeddings: torch.Tensor, num_fields: int, embedding_dim: int, output_dimension: int,
+                      product_method: str = "IPNN") -> torch.Tensor:
+    """The product layer of PNN/pnn.py:125-181 in one kernel each way: ``fields_embeddings`` (B, F*K) (the input_layer
+    outputs concatenated, or (B,F,K)) -> ``product_final`` = relu(lz + lp + bias) (B, output_dimension).
+
+    Creates ``linear_part/linear_w`` (F*K, N), then ``product_part/inner_product_w`` (N, F) when ``product_method`` is
+    exactly ``"IPNN"`` and ``product_part/outer_product_w`` (N, K, K) for ANY other value (the reference's ``else`` branch,
+    :160 -- ``"ipnn"`` builds the OPNN variable, with no error), then ``bias`` (N,) in the caller's scope.  All four are
+    default (glorot-uniform) initialised; the bias is not zero.  The reference's ``weight_regularizer``
+    (``l2_regularizer(scale)`` on the three weight matrices, :137,150,164) adds ``scale * sum(w**2) / 2`` per weight to the
+    loss when scale > 0 and nothing at the default 0.0: it is a loss-side term the caller adds in torch (see
+    examples/model_bodies.py), no kernel."""
+    F, K, N = int(num_fields), int(embedding_dim), int(output_dimension)
+    method = 0 if product_method == "IPNN" else 1
+    with variable_scope("linear_part"):
+        linear_w = get_variable("linear_w", shape=(F * K, N))
+    with variable_scope("product_part"):
+        if method == 0:
+            wprod = get_variable("inner_product_w", shape=(N, F))
+        else:
+            wprod = get_variable("outer_product_w", shape=(N, K, K))
+    bias = get_variable("bias", shape=(N,))
+    e = fields_embeddings.reshape(-1, F, K)
+    return autograd.pnn(e, linear_w, wprod, bias, method)
+
+
 # --------------------------------------------------------------------------------------------------- DIN loss-side term
 def mini_batch_aware_regularization(embedding_tensors, l2_lambda: float) -> torch.Tensor:
     """DIN/din.py:254-257 (SURVEY parity note 7): ``l2_lambda * tf.nn.l2_loss(concat(tensors, -1)) / batch`` -- an L2 on the

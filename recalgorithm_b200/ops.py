@@ -5,6 +5,7 @@ into libctr_b200.so.  Functions validate devices/dtypes and raise instead of fal
 """
 from __future__ import annotations
 
+import ctypes
 from typing import Optional, Tuple
 
 import torch
@@ -595,3 +596,51 @@ def ffm_bwd(tile: torch.Tensor, g: torch.Tensor) -> torch.Tensor:
     d_tile = torch.empty_like(tile)
     _lib.check(_lib.lib().ctr_ffm_bwd(_ptr(tile), _ptr(g), B, F, K, _ptr(d_tile), _stream()))
     return d_tile
+
+
+# ------------------------------------------------------------------------------------ PNN product layer
+PNN_METHODS = {"IPNN": 0, "OPNN": 1}
+
+
+def pnn_wprod_shape(F: int, K: int, N: int, method: int):
+    """Shape of the product weight: inner_product_w theta (N,F) for IPNN (0), outer_product_w (N,K,K) for OPNN (1)."""
+    return (N, F) if method == 0 else (N, K, K)
+
+
+def _pnn_args(e, wlin, wprod, method):
+    if method not in (0, 1):
+        raise ValueError(f"method must be 0 (IPNN) or 1 (OPNN), got {method!r}")
+    B, F, K = e.shape
+    N = wlin.shape[1]
+    _chk(e, F32, "e"); _chk(wlin, F32, "wlin", (F * K, N)); _chk(wprod, F32, "wprod", pnn_wprod_shape(F, K, N, method))
+    return B, F, K, N
+
+
+def _pnn_workspace(F, K, N, method, device):
+    nbytes = ctypes.c_int64(0)
+    _lib.check(_lib.lib().ctr_pnn_workspace_bytes(F, K, N, method, ctypes.byref(nbytes)))
+    return _cin_workspace(int(nbytes.value), device), int(nbytes.value)
+
+
+def pnn_fwd(e: torch.Tensor, wlin: torch.Tensor, wprod: torch.Tensor, bias: torch.Tensor, method: int) -> torch.Tensor:
+    """PNN product layer (PNN/pnn.py:125-181): e (B,F,K) field embeddings, wlin (F*K,N), wprod (N,F) | (N,K,K), bias (N,)
+    -> product_final = relu(lz + lp + bias) (B,N).  method 0 = IPNN, 1 = OPNN."""
+    B, F, K, N = _pnn_args(e, wlin, wprod, method)
+    _chk(bias, F32, "bias", (N,))
+    out = torch.empty((B, N), dtype=F32, device=e.device)
+    ws, nbytes = _pnn_workspace(F, K, N, method, e.device)
+    _lib.check(_lib.lib().ctr_pnn_fwd(_ptr(e), _ptr(wlin), _ptr(wprod), _ptr(bias), B, F, K, N, method, _ptr(out), _ptr(ws),
+                                      nbytes, _stream()))
+    return out
+
+
+def pnn_bwd(e, wlin, wprod, out, g_out, method: int):
+    """Gradients of pnn_fwd given its output `out` (the relu mask) and g_out (B,N): (d_e (B,F,K), d_wlin, d_wprod, d_bias)."""
+    B, F, K, N = _pnn_args(e, wlin, wprod, method)
+    _chk(out, F32, "out", (B, N)); _chk(g_out, F32, "g_out", (B, N))
+    d_e, d_wlin, d_wprod = torch.empty_like(e), torch.empty_like(wlin), torch.empty_like(wprod)
+    d_bias = torch.empty((N,), dtype=F32, device=e.device)
+    ws, nbytes = _pnn_workspace(F, K, N, method, e.device)
+    _lib.check(_lib.lib().ctr_pnn_bwd(_ptr(e), _ptr(wlin), _ptr(wprod), _ptr(out), _ptr(g_out), B, F, K, N, method, _ptr(d_e),
+                                      _ptr(d_wlin), _ptr(d_wprod), _ptr(d_bias), _ptr(ws), nbytes, _stream()))
+    return d_e, d_wlin, d_wprod, d_bias

@@ -4,7 +4,7 @@
 Each kernel is timed alone with CUDA events; an L2 flush (a 256 MB write) runs between timed iterations because these
 working sets are flushed from the 50 MB L2.  Prints one JSON line per measurement.
 
-    python tools/bench_layers.py [--iters 20] [--only cin,dcn,din,fibinet]
+    python tools/bench_layers.py [--iters 20] [--only cin,dcn,din,fibinet]     (also: pairwise, bst, adam, pnn)
 """
 import argparse
 import json
@@ -38,6 +38,78 @@ def timeit(fn, iters, flush):
         torch.cuda.synchronize()
         times.append(a.elapsed_time(b))
     return statistics.median(times), min(times)
+
+
+def pnn_rows(iters, flush, rn, hbm):
+    """IPNN / OPNN forward and backward at the reference batch (1024) and at 65 536, next to plain torch running the same
+    feature-row form (fp32 matmul, TF32 off).  Tensor figures are executed 3xTF32 FLOP/s (3 passes x 2 x B x WP x N, WP = the
+    feature width 101 padded to 128) against the H100 SXM data-sheet dense TF32 rate (495 TFLOP/s), labelled as such."""
+    tf32_peak = 495.0
+    F, K, N = 8, 8, 1024
+    WP = 128
+    iu_f, iu_k = torch.triu_indices(F, F, device="cuda"), torch.triu_indices(K, K, device="cuda")
+
+    def torch_form(e, wlin, wprod, bias, method):
+        B = e.shape[0]
+        if method == 0:
+            q = torch.einsum("bik,bjk->bij", e, e)[:, iu_f[0], iu_f[1]]
+            c = torch.where(iu_f[0] == iu_f[1], 1.0, 2.0)
+            wq = c[:, None] * (wprod[:, iu_f[0]] * wprod[:, iu_f[1]]).t()
+        else:
+            s = e.sum(1)
+            q = s[:, iu_k[0]] * s[:, iu_k[1]]
+            c = torch.where(iu_k[0] == iu_k[1], 1.0, 2.0)
+            wq = c[:, None] * wprod[:, iu_k[0], iu_k[1]].t()
+        xt = torch.cat([e.reshape(B, -1), q, torch.ones((B, 1), device=e.device)], 1)
+        return torch.relu(xt @ torch.cat([wlin, wq, bias[None, :]], 0))
+
+    prev_tf32 = torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cuda.matmul.allow_tf32 = False
+    try:
+        for method, tag in ((0, "ipnn"), (1, "opnn")):
+            wlin = rn(F * K, N, std=0.05)
+            wprod = rn(N, F, std=0.1) if method == 0 else rn(N, K, K, std=0.1)
+            bias = rn(N, std=0.05)
+            for B in (1024, 65536):
+                e, g = rn(B, F, K, std=K ** -0.5), rn(B, N)
+                cfg = {"method": tag.upper(), "B": B, "F": F, "K": K, "N": N}
+                out = ops.pnn_fwd(e, wlin, wprod, bias, method)
+                flops_fwd = 3 * 2.0 * B * WP * N
+                m, bst = timeit(lambda: ops.pnn_fwd(e, wlin, wprod, bias, method), iters, flush)
+                line = {"kernel": f"pnn_fwd_{tag}", "config": cfg, "ms_median": m, "ms_best": bst, "l2": "flushed between iterations",
+                        "algorithmic_GBps": B * (F * K + N) * 4 / (m * 1e-3) / 1e9, "executed_3xTF32_TFLOPs": flops_fwd / (m * 1e-3) / 1e12,
+                        "note": "bytes: read e, write out; FLOPs vs the H100 SXM data-sheet dense TF32 rate (495 TFLOP/s)"}
+                line["frac_of_hbm_peak"] = line["algorithmic_GBps"] / hbm
+                line["frac_of_tf32_datasheet"] = line["executed_3xTF32_TFLOPs"] / tf32_peak
+                print(json.dumps(line), flush=True)
+                m, bst = timeit(lambda: ops.pnn_bwd(e, wlin, wprod, out, g, method), iters, flush)
+                line = {"kernel": f"pnn_bwd_{tag}", "config": cfg, "ms_median": m, "ms_best": bst, "l2": "flushed between iterations",
+                        "algorithmic_GBps": B * (2 * F * K + 4 * N) * 4 / (m * 1e-3) / 1e9,
+                        "executed_3xTF32_TFLOPs": 2 * flops_fwd / (m * 1e-3) / 1e12,
+                        "note": "bytes: e read, d_e written, g_out and out read once by each of the two GEMM passes"}
+                line["frac_of_hbm_peak"] = line["algorithmic_GBps"] / hbm
+                line["frac_of_tf32_datasheet"] = line["executed_3xTF32_TFLOPs"] / tf32_peak
+                print(json.dumps(line), flush=True)
+                ref = torch_form(e, wlin, wprod, bias, method)
+                diff = float((ref - out).abs().max() / ref.abs().max())
+                m, bst = timeit(lambda: torch_form(e, wlin, wprod, bias, method), iters, flush)
+                print(json.dumps({"kernel": f"torch_fp32_fwd_{tag}", "config": cfg, "ms_median": m, "ms_best": bst,
+                                  "max_rel_diff_vs_kernel": diff, "within_1e-5": diff <= 1e-5,
+                                  "note": "same feature-row form in torch, fp32 matmul, TF32 disabled"}), flush=True)
+                ps = [t.clone().requires_grad_() for t in (e, wlin, wprod, bias)]
+                ref_out = torch_form(*ps, method)
+
+                def torch_bwd():
+                    return torch.autograd.grad(ref_out, ps, g, retain_graph=True)
+                grads = torch_bwd()
+                kg = ops.pnn_bwd(e, wlin, wprod, out, g, method)
+                gdiff = max(float((a - b).abs().max() / b.abs().max()) for a, b in zip(kg, grads))
+                m, bst = timeit(torch_bwd, iters, flush)
+                print(json.dumps({"kernel": f"torch_fp32_bwd_{tag}", "config": cfg, "ms_median": m, "ms_best": bst,
+                                  "max_rel_diff_vs_kernel": gdiff, "within_1e-5": gdiff <= 1e-5,
+                                  "note": "autograd of the same torch form (backward only), fp32, TF32 disabled"}), flush=True)
+    finally:
+        torch.backends.cuda.matmul.allow_tf32 = prev_tf32
 
 
 def main():
@@ -211,6 +283,9 @@ def main():
         by_f = n * 8 + 2 * n * D * 4 + 6 * n * D * 4
         emit("bwd_plus_lazy_adam_fused", {"B": B, "F": F, "D": D, "rows_per_field": rows}, m_, bst, bytes_=by_f,
              note="ctr_embed_fm2_bwd_adam: read tile, d_tile; RMW m, v, var; row_grads only for rows with duplicates")
+
+    if "pnn" in only:   # PNN product layer at the reference defaults (F = 8 fields, K = 8, output_dimension 1024); not in the default list
+        pnn_rows(args.iters, flush, rn, hbm)
 
 
 if __name__ == "__main__" and "--configs" not in sys.argv:

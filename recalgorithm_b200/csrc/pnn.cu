@@ -14,7 +14,7 @@
 //   dxt  = G . Wm^T       (per sample; the chain rule through q turns it into d_e)
 //   dWm^T = G^T . xt      (over the batch; the fold kernel turns it into d_linear_w, d_product_w and d_bias)
 //
-// H100 mapping (the CIN kernels' pattern, csrc/tc_ptx.cuh): two consumer warpgroups of 64 rows + one TMA producer warp,
+// H100 mapping (the CIN kernels' pipeline, csrc/tc_ptx.cuh): two consumer warpgroups of 64 rows + one TMA producer warp,
 // wgmma m64nNk8 kind tf32 with the generated operand in registers, 3xTF32 split for fp32-class accuracy, fp32 accumulators
 // drained every 96 chained MMAs, every output overwritten.
 //   pnn_fwd_tc_kernel     A = xt (rows = samples), formed once per tile from the staged e rows and reused over the N loop;
@@ -35,11 +35,8 @@ namespace ctr {
 namespace pnn {
 using namespace ctr::tc;
 
-constexpr int NWG = 2;
-constexpr int NTHREADS = (NWG + 1) * 128;
 constexpr int TILE = NWG * WG_M;             // samples per CTA tile (forward, dx)
 constexpr int FWD_NT = 64;                   // n per forward B tile (wgmma N)
-constexpr int KB = 32;                       // tf32 per 128-byte swizzle row
 constexpr int DW_BC = 32;                    // samples per dW chunk
 constexpr int DW_NC = NWG * WG_M;            // n per dW CTA
 constexpr int CHUNK_KS = 32;                 // k-steps per accumulation chain: 32 x 3 = 96 MMAs
@@ -48,8 +45,6 @@ __host__ __device__ inline int pair_index(int i, int j, int n) { return i * n - 
 __host__ __device__ inline int64_t num_pairs(int64_t F, int64_t K, int method) {
   return method == 0 ? F * (F + 1) / 2 : K * (K + 1) / 2;
 }
-static inline int wpad(int64_t WX) { return WX <= 32 ? 32 : WX <= 64 ? 64 : 128; }
-static inline int64_t pad_to(int64_t v, int64_t q) { return (v + q - 1) / q * q; }
 
 __device__ __forceinline__ void consumers_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
@@ -87,13 +82,8 @@ __global__ void pnn_prep_kernel(const float* __restrict__ wlin, const float* __r
     const int r = (int)(idx / cols), c = (int)(idx % cols);
     const int k = k_rows ? r : c, n = k_rows ? c : r;
     const float v = (k < WX && n < N) ? wm_value(wlin, wprod, bias, k, n, F, K, N, method) : 0.f;
-    if (split) {
-      const float hi = tf32_rna(v);
-      dst[idx] = hi;
-      dst[total + idx] = v - hi;
-    } else {
-      dst[idx] = v;
-    }
+    if (split) store_split(dst, total, idx, v);
+    else dst[idx] = v;
   }
 }
 
@@ -162,7 +152,7 @@ __global__ void __launch_bounds__(NTHREADS, 1)
 pnn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmap_w, const float* __restrict__ e, float* __restrict__ out, int B,
                   int F, int K, int N, int NP, int nsplit) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* smem = align_1024(smem_raw);
   constexpr int stage_bytes = 2 * (WP / KB) * FWD_NT * 128;
   constexpr int copy_bytes = stage_bytes / 2;
   const int FK = F * K, FKP = FK + 1;
@@ -171,9 +161,7 @@ pnn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmap_w, const float* __res
   float* ssm = esm + NWG * WG_M * FKP;                                       // [2][64][16]
   int2* cinfo = reinterpret_cast<int2*>(ssm + NWG * WG_M * 16);              // [WP]
   const uint32_t sbase = smem_u32(smem);
-  const uint32_t bar0 = smem_u32(cinfo + WP);
-  auto full_b = [&](int s) { return bar0 + 8 * s; };
-  auto empty_b = [&](int s) { return bar0 + 8 * (SB + s); };
+  Ring ring(smem_u32(cinfo + WP), SB);
 
   const int warp = warp_uniform(threadIdx.x >> 5), lane = threadIdx.x & 31;
   const int n_btiles = (B + TILE - 1) / TILE, NT = NP / FWD_NT;
@@ -181,40 +169,27 @@ pnn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmap_w, const float* __res
   const int n_items = n_btiles * nsplit;
 
   for (int c = threadIdx.x; c < WP; c += blockDim.x) cinfo[c] = column_info(c, FK, Q, METHOD == 0 ? F : K);
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < SB; ++s) { mbar_init(full_b(s), 1); mbar_init(empty_b(s), NWG * 4); }
-    fence_barrier_init();
-  }
-  __syncthreads();
-
-  if (warp >= NWG * 4) {
-    // ============================ TMA producer: Wm^T tiles [64 n x WP] (hi, lo) ============================
-    setmaxnreg_dec<40>();
-    if (warp == NWG * 4 && lane == 0) {
-      int s = 0, ph = 0;
-      for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
-        const int nt0 = (item % nsplit) * per_split, nt1 = min(NT, nt0 + per_split);
-        for (int nt = nt0; nt < nt1; ++nt) {
-          mbar_wait(empty_b(s), ph ^ 1);
-          const uint32_t dst = sbase + s * stage_bytes;
-          mbar_expect_tx(full_b(s), (uint32_t)stage_bytes);
-          for (int kb = 0; kb < WP / KB; ++kb) {
-            tma_load_2d(dst + kb * FWD_NT * 128, &tmap_w, kb * KB, nt * FWD_NT, full_b(s));
-            tma_load_2d(dst + copy_bytes + kb * FWD_NT * 128, &tmap_w, kb * KB, NP + nt * FWD_NT, full_b(s));
+  ring.init();
+  // ============================ TMA producer: Wm^T tiles [64 n x WP] (hi, lo) ============================
+  if (producer_role(warp, lane, [&] {
+        for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
+          const int nt0 = (item % nsplit) * per_split, nt1 = min(NT, nt0 + per_split);
+          for (int nt = nt0; nt < nt1; ++nt) {
+            const Ring::Slot slot = ring.acquire(stage_bytes);
+            const uint32_t dst = sbase + slot.stage * stage_bytes;
+            for (int kb = 0; kb < WP / KB; ++kb) {
+              tma_load_2d(dst + kb * FWD_NT * 128, &tmap_w, kb * KB, nt * FWD_NT, slot.full);
+              tma_load_2d(dst + copy_bytes + kb * FWD_NT * 128, &tmap_w, kb * KB, NP + nt * FWD_NT, slot.full);
+            }
           }
-          if (++s == SB) { s = 0; ph ^= 1; }
         }
-      }
-    }
+      }))
     return;
-  }
 
   // ============================ consumers ============================
-  setmaxnreg_inc<232>();
   const int wg = warp >> 2, w = warp & 3, g = lane >> 2, t = lane & 3, tw = threadIdx.x & 127;
   float* er = esm + wg * WG_M * FKP;
   float* sr = ssm + wg * WG_M * 16;
-  int s = 0, ph = 0;
   for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
     const int bt = item / nsplit;
     const int nt0 = (item % nsplit) * per_split, nt1 = min(NT, nt0 + per_split);
@@ -253,23 +228,18 @@ pnn_fwd_tc_kernel(const __grid_constant__ CUtensorMap tmap_w, const float* __res
     float* o1 = o0 + (size_t)8 * N;
     for (int nt = nt0; nt < nt1; ++nt) {
       float d[FWD_NT / 2];
-      mbar_wait(full_b(s), ph);
+      const int s = ring.wait();
       const uint64_t bhi = gmma_desc_kmajor(sbase + s * stage_bytes, 128);
       const uint64_t blo = gmma_desc_kmajor(sbase + s * stage_bytes + copy_bytes, 128);
       wgmma_fence();
 #pragma unroll
       for (int ks = 0; ks < WP / 8; ++ks) {
         const uint64_t off = (uint64_t)((ks >> 2) * (FWD_NT * 128 / 16) + 2 * (ks & 3));
-        wgmma_tf32_rs<FWD_NT>(d, al[ks], bhi + off, ks > 0 ? 1 : 0);     // small terms first
-        wgmma_tf32_rs<FWD_NT>(d, ah[ks], blo + off, 1);
-        wgmma_tf32_rs<FWD_NT>(d, ah[ks], bhi + off, 1);
+        mma_3xtf32<FWD_NT>(d, ah[ks], al[ks], bhi, blo, off, ks > 0 ? 1 : 0);
       }
       wgmma_commit();
-      wgmma_wait<0>();
-#pragma unroll
-      for (int ks = 0; ks < WP / 8; ++ks) { wgmma_keep(ah[ks]); wgmma_keep(al[ks]); }
-      if (lane == 0) mbar_arrive(empty_b(s));
-      if (++s == SB) { s = 0; ph ^= 1; }
+      wgmma_wait_keep(ah, al);
+      ring.release(lane);
 #pragma unroll
       for (int c = 0; c < FWD_NT / 8; ++c) {
 #pragma unroll
@@ -295,7 +265,7 @@ __global__ void __launch_bounds__(NTHREADS, 1)
 pnn_bwd_dx_tc_kernel(const __grid_constant__ CUtensorMap tmap_w, const float* __restrict__ e, const float* __restrict__ outv,
                      const float* __restrict__ g_out, float* __restrict__ d_e, int B, int F, int K, int N, int NPK) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* smem = align_1024(smem_raw);
   constexpr int copy_bytes = WP * 128;
   constexpr int stage_bytes = 2 * copy_bytes;
   constexpr int LD = WP + 1;
@@ -303,44 +273,29 @@ pnn_bwd_dx_tc_kernel(const __grid_constant__ CUtensorMap tmap_w, const float* __
   float* dsm = reinterpret_cast<float*>(smem + SB * stage_bytes);          // [2][64][WP+1]  dxt of the tile
   float* ssm = dsm + NWG * WG_M * LD;                                        // [2][64][16]    s (OPNN)
   const uint32_t sbase = smem_u32(smem);
-  const uint32_t bar0 = smem_u32(ssm + NWG * WG_M * 16);
-  auto full_b = [&](int s) { return bar0 + 8 * s; };
-  auto empty_b = [&](int s) { return bar0 + 8 * (SB + s); };
+  Ring ring(smem_u32(ssm + NWG * WG_M * 16), SB);
 
   const int warp = warp_uniform(threadIdx.x >> 5), lane = threadIdx.x & 31;
   const int n_tiles = (B + TILE - 1) / TILE, nkb = NPK / KB;
 
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < SB; ++s) { mbar_init(full_b(s), 1); mbar_init(empty_b(s), NWG * 4); }
-    fence_barrier_init();
-  }
-  __syncthreads();
-
-  if (warp >= NWG * 4) {
-    // ============================ TMA producer: Wm tiles [WP k x 32 n] (hi, lo) ============================
-    setmaxnreg_dec<40>();
-    if (warp == NWG * 4 && lane == 0) {
-      int s = 0, ph = 0;
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
-        for (int kb = 0; kb < nkb; ++kb) {
-          mbar_wait(empty_b(s), ph ^ 1);
-          const uint32_t dst = sbase + s * stage_bytes;
-          mbar_expect_tx(full_b(s), (uint32_t)stage_bytes);
-          tma_load_2d(dst, &tmap_w, kb * KB, 0, full_b(s));
-          tma_load_2d(dst + copy_bytes, &tmap_w, kb * KB, WP, full_b(s));
-          if (++s == SB) { s = 0; ph ^= 1; }
+  ring.init();
+  // ============================ TMA producer: Wm tiles [WP k x 32 n] (hi, lo) ============================
+  if (producer_role(warp, lane, [&] {
+        for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+          for (int kb = 0; kb < nkb; ++kb) {
+            const Ring::Slot slot = ring.acquire(stage_bytes);
+            const uint32_t dst = sbase + slot.stage * stage_bytes;
+            tma_load_2d(dst, &tmap_w, kb * KB, 0, slot.full);
+            tma_load_2d(dst + copy_bytes, &tmap_w, kb * KB, WP, slot.full);
+          }
         }
-      }
-    }
+      }))
     return;
-  }
 
   // ============================ consumers: G fragments per 32-column block, dxt, chain rule ============================
-  setmaxnreg_inc<232>();
   const int wg = warp >> 2, w = warp & 3, g = lane >> 2, t = lane & 3, tw = threadIdx.x & 127;
   float* ds = dsm + wg * WG_M * LD;
   float* sr = ssm + wg * WG_M * 16;
-  int s = 0, ph = 0;
   for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
     const long long base = (long long)tile * TILE + wg * WG_M;
     const int r0 = w * 16 + g;
@@ -362,27 +317,17 @@ pnn_bwd_dx_tc_kernel(const __grid_constant__ CUtensorMap tmap_w, const float* __
         }
         tf32_split(a, gh[ks], gl[ks]);
       }
-      const bool chain_start = (kb * 4) % CHUNK_KS == 0;
-      mbar_wait(full_b(s), ph);
+      const bool chain_start = chain_first(kb, CHUNK_KS / 4);
+      const int s = ring.wait();
       const uint64_t bhi = gmma_desc_kmajor(sbase + s * stage_bytes, 128);
       const uint64_t blo = gmma_desc_kmajor(sbase + s * stage_bytes + copy_bytes, 128);
       wgmma_fence();
 #pragma unroll
-      for (int ks = 0; ks < 4; ++ks) {
-        wgmma_tf32_rs<WP>(dacc, gl[ks], bhi + 2 * ks, (chain_start && ks == 0) ? 0 : 1);
-        wgmma_tf32_rs<WP>(dacc, gh[ks], blo + 2 * ks, 1);
-        wgmma_tf32_rs<WP>(dacc, gh[ks], bhi + 2 * ks, 1);
-      }
+      for (int ks = 0; ks < 4; ++ks) mma_3xtf32<WP>(dacc, gh[ks], gl[ks], bhi, blo, 2 * ks, (chain_start && ks == 0) ? 0 : 1);
       wgmma_commit();
-      wgmma_wait<0>();
-#pragma unroll
-      for (int ks = 0; ks < 4; ++ks) { wgmma_keep(gh[ks]); wgmma_keep(gl[ks]); }
-      if (lane == 0) mbar_arrive(empty_b(s));
-      if (++s == SB) { s = 0; ph ^= 1; }
-      if (((kb + 1) * 4) % CHUNK_KS == 0 || kb + 1 == nkb) {
-#pragma unroll
-        for (int q = 0; q < WP / 2; ++q) acc[q] += dacc[q];
-      }
+      wgmma_wait_keep(gh, gl);
+      ring.release(lane);
+      if (chain_last(kb, nkb, CHUNK_KS / 4)) chain_drain(acc, dacc);
     }
     // ---------------- epilogue: dxt fragment -> ds[row][col]; d_e = dxt_lin + chain rule through the pair features
 #pragma unroll
@@ -438,7 +383,7 @@ pnn_bwd_dw_tc_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_co
                      const float* __restrict__ e, float* __restrict__ dwt, int B, int F, int K, int N, int WX, int ngroups,
                      int nslices, int SB) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+  uint8_t* smem = align_1024(smem_raw);
   constexpr int xt_bytes = 2 * WP * 128;                      // xt^T tiles [WP k x 32 samples] (hi | lo), 128B-swizzled
   constexpr int go_bytes = DW_BC * DW_NC * 4;                 // one g_out or out chunk [32 samples x 128 n]
   const int FK = F * K, FKP = FK + 1;
@@ -448,9 +393,7 @@ pnn_bwd_dw_tc_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_co
   float* esm = gos + SB * 2 * DW_BC * DW_NC;                               // [32][FK+1]
   float* ssm = esm + DW_BC * FKP;                                          // [32][K+1]
   int2* cinfo = reinterpret_cast<int2*>(ssm + DW_BC * (K + 1));            // [WP]
-  const uint32_t bar0 = smem_u32(cinfo + WP);
-  auto full_b = [&](int s) { return bar0 + 8 * s; };
-  auto empty_b = [&](int s) { return bar0 + 8 * (SB + s); };
+  Ring ring(smem_u32(cinfo + WP), SB);
 
   const int warp = warp_uniform(threadIdx.x >> 5), lane = threadIdx.x & 31;
   const int group = blockIdx.x % ngroups, slice = blockIdx.x / ngroups;
@@ -460,36 +403,23 @@ pnn_bwd_dw_tc_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_co
   const int n0 = group * DW_NC;
 
   for (int c = threadIdx.x; c < WP; c += blockDim.x) cinfo[c] = column_info(c, FK, Q, METHOD == 0 ? F : K);
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < SB; ++s) { mbar_init(full_b(s), 1); mbar_init(empty_b(s), NWG * 4); }
-    fence_barrier_init();
-  }
-  __syncthreads();
-
-  if (warp >= NWG * 4) {
-    // ============================ TMA producer: g_out / out chunks [32 samples x 128 n] ============================
-    setmaxnreg_dec<40>();
-    if (warp == NWG * 4 && lane == 0) {
-      int s = 0, ph = 0;
-      for (int c = c_beg; c < c_end; ++c) {
-        mbar_wait(empty_b(s), ph ^ 1);
-        const uint32_t dst = smem_u32(gos + (size_t)s * 2 * DW_BC * DW_NC);
-        mbar_expect_tx(full_b(s), (uint32_t)(2 * go_bytes));
-        tma_load_2d(dst, &tmap_g, n0, c * DW_BC, full_b(s));
-        tma_load_2d(dst + go_bytes, &tmap_o, n0, c * DW_BC, full_b(s));
-        if (++s == SB) { s = 0; ph ^= 1; }
-      }
-    }
+  ring.init();
+  // ============================ TMA producer: g_out / out chunks [32 samples x 128 n] ============================
+  if (producer_role(warp, lane, [&] {
+        for (int c = c_beg; c < c_end; ++c) {
+          const Ring::Slot slot = ring.acquire(2 * go_bytes);
+          const uint32_t dst = smem_u32(gos + (size_t)slot.stage * 2 * DW_BC * DW_NC);
+          tma_load_2d(dst, &tmap_g, n0, c * DW_BC, slot.full);
+          tma_load_2d(dst + go_bytes, &tmap_o, n0, c * DW_BC, slot.full);
+        }
+      }))
     return;
-  }
 
   // ============================ consumers ============================
-  setmaxnreg_inc<232>();
   const int wg = warp >> 2, w = warp & 3, g = lane >> 2, t = lane & 3, ct = threadIdx.x;   // ct: 0..255
   float acc[WP / 2], dacc[WP / 2];
 #pragma unroll
   for (int q = 0; q < WP / 2; ++q) { acc[q] = 0.f; dacc[q] = 0.f; }
-  int s = 0, ph = 0;
   const int nl0 = wg * WG_M + w * 16 + g;                     // this thread's A rows: n0 + nl0 (+8)
   for (int c = c_beg; c < c_end; ++c) {
     const int b0 = c * DW_BC;
@@ -508,17 +438,14 @@ pnn_bwd_dw_tc_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_co
       }
       consumers_bar();
     }
-    mbar_wait(full_b(s), ph);
+    const int s = ring.wait();
     // 2. xt^T (tf32 hi | lo) into the stage's swizzled B tiles: element (k, b) at byte k*128 + 4b, 16-byte chunk XOR (k & 7)
     uint8_t* xt = xts + s * xt_bytes;
     for (int idx = ct; idx < WP * DW_BC; idx += 256) {
       const int k = idx / DW_BC, b = idx % DW_BC;
       const float v = b0 + b < B ? feature<METHOD>(cinfo[k], esm + b * FKP, ssm + b * (K + 1), K) : 0.f;
-      const float hi = tf32_rna(v);
       const uint32_t o = (uint32_t)(k * 128 + b * 4);
-      const uint32_t so = o ^ (((o >> 7) & 7u) << 4);
-      *reinterpret_cast<float*>(xt + so) = hi;
-      *reinterpret_cast<float*>(xt + WP * 128 + so) = v - hi;
+      store_split(reinterpret_cast<float*>(xt), WP * 32, (o ^ (((o >> 7) & 7u) << 4)) / 4, v);
     }
     fence_proxy_async();                                      // generic-proxy writes -> visible to wgmma
     consumers_bar();
@@ -536,26 +463,16 @@ pnn_bwd_dw_tc_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_co
       }
       tf32_split(a, ah[ks], al[ks]);
     }
-    const bool chain_start = ((c - c_beg) * 4) % CHUNK_KS == 0;
+    const bool chain_start = chain_first(c - c_beg, CHUNK_KS / 4);
     const uint64_t bhi = gmma_desc_kmajor(smem_u32(xt), 128);
     const uint64_t blo = gmma_desc_kmajor(smem_u32(xt + WP * 128), 128);
     wgmma_fence();
 #pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {
-      wgmma_tf32_rs<WP>(dacc, al[ks], bhi + 2 * ks, (chain_start && ks == 0) ? 0 : 1);
-      wgmma_tf32_rs<WP>(dacc, ah[ks], blo + 2 * ks, 1);
-      wgmma_tf32_rs<WP>(dacc, ah[ks], bhi + 2 * ks, 1);
-    }
+    for (int ks = 0; ks < 4; ++ks) mma_3xtf32<WP>(dacc, ah[ks], al[ks], bhi, blo, 2 * ks, (chain_start && ks == 0) ? 0 : 1);
     wgmma_commit();
-    wgmma_wait<0>();
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) { wgmma_keep(ah[ks]); wgmma_keep(al[ks]); }
-    if (lane == 0) mbar_arrive(empty_b(s));
-    if (++s == SB) { s = 0; ph ^= 1; }
-    if (((c - c_beg + 1) * 4) % CHUNK_KS == 0 || c + 1 == c_end) {
-#pragma unroll
-      for (int q = 0; q < WP / 2; ++q) acc[q] += dacc[q];
-    }
+    wgmma_wait_keep(ah, al);
+    ring.release(lane);
+    if (chain_last(c - c_beg, c_end - c_beg, CHUNK_KS / 4)) chain_drain(acc, dacc);
   }
   if (c_end > c_beg) {
 #pragma unroll
@@ -736,7 +653,7 @@ PnnShape shape_of(int64_t F, int64_t K, int64_t N, int method) {
   s.Q = num_pairs(F, K, method);
   s.WX = s.FK + s.Q + 1;
   s.tc = s.WX <= 128 && N % 4 == 0;
-  s.WP = wpad(s.WX);
+  s.WP = pad3(s.WX);
   s.NP = pad_to(N, FWD_NT);
   s.NPK = pad_to(N, KB);
   s.w_floats = s.tc ? 2 * s.WP * (s.NP > s.NPK ? s.NP : s.NPK) : s.WX * N;
@@ -757,40 +674,13 @@ int check_pnn(const char* fn, int64_t B, int64_t F, int64_t K, int64_t N, int me
   return CTR_OK;
 }
 
-int check_workspace(const char* fn, const PnnShape& s, void* workspace, int64_t workspace_bytes) {
-  const int64_t need = workspace_of(s);
-  CTR_REQUIRE(workspace != nullptr && workspace_bytes >= need,
-              "%s: workspace of %lld bytes required (ctr_pnn_workspace_bytes), got %lld", fn, (long long)need,
-              (long long)workspace_bytes);
-  CTR_REQUIRE((reinterpret_cast<uintptr_t>(workspace) & 127) == 0, "%s: workspace must be 128-byte aligned", fn);
-  return CTR_OK;
-}
-
-int grid_for(size_t total, int cap) { return (int)((total + 255) / 256 < (size_t)cap ? (total + 255) / 256 : (size_t)cap); }
-
+// a row-major [outer x inner] float matrix, one box of [box_outer x box_inner]
 int encode_2d(const char* fn, CUtensorMap* map, const void* base, uint64_t inner, uint64_t outer, uint32_t box_inner,
               uint32_t box_outer, CUtensorMapSwizzle sw) {
-  EncodeTiledFn enc = encode_tiled();
-  if (enc == nullptr) {
-    set_error("%s: cuTensorMapEncodeTiled is not available from the driver", fn);
-    return CTR_ERR_CUDA;
-  }
   const cuuint64_t gdim[2] = {(cuuint64_t)inner, (cuuint64_t)outer};
   const cuuint64_t gstr[1] = {(cuuint64_t)inner * sizeof(float)};
   const cuuint32_t box[2] = {box_inner, box_outer};
-  const cuuint32_t es[2] = {1, 1};
-  CUresult cr = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(base), gdim, gstr, box, es,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (cr != CUDA_SUCCESS) {
-    set_error("%s: cuTensorMapEncodeTiled failed with CUresult %d", fn, (int)cr);
-    return CTR_ERR_CUDA;
-  }
-  return CTR_OK;
-}
-
-int set_smem(const void* k, size_t bytes) {
-  if (bytes > 48 * 1024) CTR_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-  return CTR_OK;
+  return encode_tmap(fn, map, 2, base, gdim, gstr, box, sw);
 }
 
 constexpr size_t SMEM_CAP = 226 * 1024;     // dynamic shared memory per CTA on sm_90 (227 KB) less slack
@@ -813,17 +703,16 @@ extern "C" int ctr_pnn_fwd(const float* e, const float* wlin, const float* wprod
   if (rc) return rc;
   CTR_REQUIRE(e && wlin && wprod && bias && out, "ctr_pnn_fwd: null argument");
   const PnnShape s = shape_of(F, K, N, method);
-  rc = check_workspace(fn, s, workspace, workspace_bytes);
+  rc = check_workspace(fn, "ctr_pnn_workspace_bytes", workspace, workspace_bytes, workspace_of(s));
   if (rc) return rc;
   if (B == 0) return CTR_OK;
   cudaStream_t st = as_stream(stream);
   float* ws = static_cast<float*>(workspace);
   const int sms = sm_count();
   if (s.tc) {
-    const size_t total = (size_t)s.NP * s.WP;
-    pnn_prep_kernel<<<grid_for(total, 2048), 256, 0, st>>>(wlin, wprod, bias, ws, (int)F, (int)K, (int)N, method, (int)s.WX,
-                                                         (int)s.NP, s.WP, 0, 1);
-    CTR_CHECK_LAUNCH("ctr_pnn_fwd(prep)");
+    rc = launch("ctr_pnn_fwd(prep)", pnn_prep_kernel, grid_for((size_t)s.NP * s.WP, 2048), 256, 0, st, wlin, wprod, bias, ws,
+                (int)F, (int)K, (int)N, method, (int)s.WX, (int)s.NP, s.WP, 0, 1);
+    if (rc) return rc;
     CUtensorMap tmap;
     rc = encode_2d(fn, &tmap, ws, s.WP, 2 * s.NP, KB, FWD_NT, CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
@@ -833,40 +722,26 @@ extern "C" int ctr_pnn_fwd(const float* e, const float* wlin, const float* wprod
     if (nsplit > NT) nsplit = NT;
     const long long items = (long long)n_btiles * nsplit;
     const int grid = (int)(items < sms ? items : sms);
-#define PNN_FWD(WP_, SB_, M_)                                                                                            \
-  {                                                                                                                      \
-    const size_t smem = fwd_smem_bytes(WP_, SB_, (int)s.FK) + 1024;                                                      \
-    auto k = pnn_fwd_tc_kernel<WP_, SB_, M_>;                                                                            \
-    CTR_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));                           \
-    k<<<grid, NTHREADS, smem, st>>>(tmap, e, out, (int)B, (int)F, (int)K, (int)N, (int)s.NP, nsplit);                    \
-  }
-    if (method == 0) {
-      if (s.WP == 32) PNN_FWD(32, 4, 0) else if (s.WP == 64) PNN_FWD(64, 3, 0) else PNN_FWD(128, 2, 0)
-    } else {
-      if (s.WP == 32) PNN_FWD(32, 4, 1) else if (s.WP == 64) PNN_FWD(64, 3, 1) else PNN_FWD(128, 2, 1)
-    }
-#undef PNN_FWD
-    CTR_CHECK_LAUNCH("ctr_pnn_fwd(wgmma)");
-    return CTR_OK;
+    return with_const<0, 1>(method, [&](auto M) {
+      return with_const<32, 64, 128>(s.WP, [&](auto WP) {
+        constexpr int SB = WP == 32 ? 4 : WP == 64 ? 3 : 2;
+        return launch("ctr_pnn_fwd(wgmma)", pnn_fwd_tc_kernel<WP, SB, M>, grid, NTHREADS,
+                      fwd_smem_bytes(WP, SB, (int)s.FK) + 1024, st, tmap, e, out, (int)B, (int)F, (int)K, (int)N, (int)s.NP,
+                      nsplit);
+      });
+    });
   }
   const size_t smem = sizeof(float) * (size_t)(SIMPLE_SPB * s.WX + s.FK + s.K);
   CTR_UNSUPPORTED(smem > SMEM_CAP, "ctr_pnn_fwd: F*K=%lld too large for the CUDA-core path", (long long)s.FK);
-  pnn_prep_kernel<<<grid_for((size_t)s.WX * N, 4096), 256, 0, st>>>(wlin, wprod, bias, ws, (int)F, (int)K, (int)N, method,
-                                                                   (int)s.WX, (int)s.WX, (int)N, 1, 0);
-  CTR_CHECK_LAUNCH("ctr_pnn_fwd(prep)");
+  rc = launch("ctr_pnn_fwd(prep)", pnn_prep_kernel, grid_for((size_t)s.WX * N, 4096), 256, 0, st, wlin, wprod, bias, ws,
+              (int)F, (int)K, (int)N, method, (int)s.WX, (int)s.WX, (int)N, 1, 0);
+  if (rc) return rc;
   const int64_t groups = (B + SIMPLE_SPB - 1) / SIMPLE_SPB;
   const int grid = (int)(groups < (int64_t)sms * 4 ? groups : (int64_t)sms * 4);
-  if (method == 0) {
-    rc = set_smem((const void*)pnn_fwd_simple_kernel<0>, smem);
-    if (rc) return rc;
-    pnn_fwd_simple_kernel<0><<<grid, 256, smem, st>>>(e, ws, out, (int)B, (int)F, (int)K, (int)N, (int)s.WX);
-  } else {
-    rc = set_smem((const void*)pnn_fwd_simple_kernel<1>, smem);
-    if (rc) return rc;
-    pnn_fwd_simple_kernel<1><<<grid, 256, smem, st>>>(e, ws, out, (int)B, (int)F, (int)K, (int)N, (int)s.WX);
-  }
-  CTR_CHECK_LAUNCH("ctr_pnn_fwd(simple)");
-  return CTR_OK;
+  return with_const<0, 1>(method, [&](auto M) {
+    return launch("ctr_pnn_fwd(simple)", pnn_fwd_simple_kernel<M>, grid, 256, smem, st, e, ws, out, (int)B,
+                  (int)F, (int)K, (int)N, (int)s.WX);
+  });
 }
 
 extern "C" int ctr_pnn_bwd(const float* e, const float* wlin, const float* wprod, const float* out, const float* g_out,
@@ -877,7 +752,7 @@ extern "C" int ctr_pnn_bwd(const float* e, const float* wlin, const float* wprod
   if (rc) return rc;
   CTR_REQUIRE(e && wlin && wprod && out && g_out && d_e && d_wlin && d_wprod && d_bias, "ctr_pnn_bwd: null argument");
   const PnnShape s = shape_of(F, K, N, method);
-  rc = check_workspace(fn, s, workspace, workspace_bytes);
+  rc = check_workspace(fn, "ctr_pnn_workspace_bytes", workspace, workspace_bytes, workspace_of(s));
   if (rc) return rc;
   cudaStream_t st = as_stream(stream);
   float* ws = static_cast<float*>(workspace);
@@ -886,100 +761,61 @@ extern "C" int ctr_pnn_bwd(const float* e, const float* wlin, const float* wprod
   CTR_CUDA(cudaMemsetAsync(dwt, 0, sizeof(float) * (size_t)N * s.WX, st));
   if (B > 0 && s.tc) {
     CTR_REQUIRE(aligned16(out) && aligned16(g_out), "ctr_pnn_bwd: out and g_out must be 16-byte aligned");
-    const size_t total = (size_t)s.WP * s.NPK;
-    pnn_prep_kernel<<<grid_for(total, 2048), 256, 0, st>>>(wlin, wprod, nullptr, ws, (int)F, (int)K, (int)N, method,
-                                                         (int)s.WX, s.WP, (int)s.NPK, 1, 1);
-    CTR_CHECK_LAUNCH("ctr_pnn_bwd(prep)");
+    rc = launch("ctr_pnn_bwd(prep)", pnn_prep_kernel, grid_for((size_t)s.WP * s.NPK, 2048), 256, 0, st, wlin, wprod,
+                nullptr, ws, (int)F, (int)K, (int)N, method, (int)s.WX, s.WP, (int)s.NPK, 1, 1);
+    if (rc) return rc;
     // ---- d_e: Wm (hi | lo) as [2 WP rows x NPK], one [WP x 32] swizzled box per K-block
-    {
-      CUtensorMap tmap;
-      rc = encode_2d(fn, &tmap, ws, s.NPK, 2 * s.WP, KB, s.WP, CU_TENSOR_MAP_SWIZZLE_128B);
-      if (rc) return rc;
-      const int tiles = (int)((B + TILE - 1) / TILE);
-      const int grid = tiles < sms ? tiles : sms;
-#define PNN_DX(WP_, M_)                                                                                                \
-  {                                                                                                                    \
-    const size_t smem = dx_smem_bytes(WP_, 4) + 1024;                                                                  \
-    auto k = pnn_bwd_dx_tc_kernel<WP_, 4, M_>;                                                                         \
-    CTR_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));                         \
-    k<<<grid, NTHREADS, smem, st>>>(tmap, e, out, g_out, d_e, (int)B, (int)F, (int)K, (int)N, (int)s.NPK);             \
-  }
-      if (method == 0) {
-        if (s.WP == 32) PNN_DX(32, 0) else if (s.WP == 64) PNN_DX(64, 0) else PNN_DX(128, 0)
-      } else {
-        if (s.WP == 32) PNN_DX(32, 1) else if (s.WP == 64) PNN_DX(64, 1) else PNN_DX(128, 1)
-      }
-#undef PNN_DX
-      CTR_CHECK_LAUNCH("ctr_pnn_bwd(dx, wgmma)");
-    }
+    CUtensorMap tw;
+    rc = encode_2d(fn, &tw, ws, s.NPK, 2 * s.WP, KB, s.WP, CU_TENSOR_MAP_SWIZZLE_128B);
+    if (rc) return rc;
+    const int tiles = (int)((B + TILE - 1) / TILE);
     // ---- dWm^T: g_out and out as [B rows x N], boxes of [32 samples x 128 n] (out-of-range rows / columns arrive as zeros)
-    {
-      CUtensorMap tg, to;
-      rc = encode_2d(fn, &tg, g_out, N, B, DW_NC, DW_BC, CU_TENSOR_MAP_SWIZZLE_NONE);
-      if (rc) return rc;
-      rc = encode_2d(fn, &to, out, N, B, DW_NC, DW_BC, CU_TENSOR_MAP_SWIZZLE_NONE);
-      if (rc) return rc;
-      const int ngroups = (int)((N + DW_NC - 1) / DW_NC);
-      const int64_t chunks = (B + DW_BC - 1) / DW_BC;
-      int nslices = sms / ngroups;
-      if (nslices < 1) nslices = 1;
-      if (nslices > chunks) nslices = (int)chunks;
-      const int grid = ngroups * nslices;
-      const size_t fixed = dw_smem_bytes(s.WP, 0, (int)s.FK, (int)s.K) + 1024;
-      const size_t stage = (size_t)dw_smem_bytes(s.WP, 1, (int)s.FK, (int)s.K) + 1024 - fixed;
-      int sb = (int)((SMEM_CAP - fixed) / stage);
-      if (sb > 4) sb = 4;
-      const size_t smem = fixed + sb * stage;
-#define PNN_DW(WP_, M_)                                                                                                \
-  {                                                                                                                    \
-    auto k = pnn_bwd_dw_tc_kernel<WP_, M_>;                                                                            \
-    CTR_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));                         \
-    k<<<grid, NTHREADS, smem, st>>>(tg, to, e, dwt, (int)B, (int)F, (int)K, (int)N, (int)s.WX, ngroups, nslices, sb);  \
-  }
-      if (method == 0) {
-        if (s.WP == 32) PNN_DW(32, 0) else if (s.WP == 64) PNN_DW(64, 0) else PNN_DW(128, 0)
-      } else {
-        if (s.WP == 32) PNN_DW(32, 1) else if (s.WP == 64) PNN_DW(64, 1) else PNN_DW(128, 1)
-      }
-#undef PNN_DW
-      CTR_CHECK_LAUNCH("ctr_pnn_bwd(dw, wgmma)");
-    }
+    CUtensorMap tg, to;
+    rc = encode_2d(fn, &tg, g_out, N, B, DW_NC, DW_BC, CU_TENSOR_MAP_SWIZZLE_NONE);
+    if (rc) return rc;
+    rc = encode_2d(fn, &to, out, N, B, DW_NC, DW_BC, CU_TENSOR_MAP_SWIZZLE_NONE);
+    if (rc) return rc;
+    const int ngroups = (int)((N + DW_NC - 1) / DW_NC);
+    const int64_t chunks = (B + DW_BC - 1) / DW_BC;
+    int nslices = sms / ngroups;
+    if (nslices < 1) nslices = 1;
+    if (nslices > chunks) nslices = (int)chunks;
+    const size_t fixed = dw_smem_bytes(s.WP, 0, (int)s.FK, (int)s.K) + 1024;
+    const size_t stage = (size_t)dw_smem_bytes(s.WP, 1, (int)s.FK, (int)s.K) + 1024 - fixed;
+    int sb = (int)((SMEM_CAP - fixed) / stage);
+    if (sb > 4) sb = 4;
+    rc = with_const<0, 1>(method, [&](auto M) {
+      return with_const<32, 64, 128>(s.WP, [&](auto WP) {
+        if (int r = launch("ctr_pnn_bwd(dx, wgmma)", pnn_bwd_dx_tc_kernel<WP, 4, M>, tiles < sms ? tiles : sms, NTHREADS,
+                           dx_smem_bytes(WP, 4) + 1024, st, tw, e, out, g_out, d_e, (int)B, (int)F, (int)K, (int)N, (int)s.NPK))
+          return r;
+        return launch("ctr_pnn_bwd(dw, wgmma)", pnn_bwd_dw_tc_kernel<WP, M>, ngroups * nslices, NTHREADS, fixed + sb * stage,
+                      st, tg, to, e, dwt, (int)B, (int)F, (int)K, (int)N, (int)s.WX, ngroups, nslices, sb);
+      });
+    });
+    if (rc) return rc;
   } else if (B > 0) {
     const size_t smem_dx = sizeof(float) * (size_t)(N + s.FK + s.K + s.WX);
     const size_t smem_dw = sizeof(float) * (size_t)(s.FK + s.K + SIMPLE_PC);
     CTR_UNSUPPORTED(smem_dx > SMEM_CAP, "ctr_pnn_bwd: N + F*K too large for the CUDA-core path");
-    pnn_prep_kernel<<<grid_for((size_t)s.WX * N, 4096), 256, 0, st>>>(wlin, wprod, nullptr, ws, (int)F, (int)K, (int)N,
-                                                                     method, (int)s.WX, (int)N, (int)s.WX, 0, 0);
-    CTR_CHECK_LAUNCH("ctr_pnn_bwd(prep)");
+    rc = launch("ctr_pnn_bwd(prep)", pnn_prep_kernel, grid_for((size_t)s.WX * N, 4096), 256, 0, st, wlin, wprod,
+                nullptr, ws, (int)F, (int)K, (int)N, method, (int)s.WX, (int)N, (int)s.WX, 0, 0);
+    if (rc) return rc;
     const int gdx = (int)(B < (int64_t)sms * 4 ? B : (int64_t)sms * 4);
     const int gx = (int)((s.WX + SIMPLE_PC - 1) / SIMPLE_PC), gy = (int)((N + 255) / 256);
     int gz = (int)((int64_t)sms * 4 / ((int64_t)gx * gy));
     if (gz < 1) gz = 1;
     if (gz > B) gz = (int)B;
-    if (method == 0) {
-      rc = set_smem((const void*)pnn_bwd_dx_simple_kernel<0>, smem_dx);
-      if (rc) return rc;
-      pnn_bwd_dx_simple_kernel<0><<<gdx, 256, smem_dx, st>>>(e, ws, out, g_out, d_e, (int)B, (int)F, (int)K, (int)N, (int)s.WX);
-      CTR_CHECK_LAUNCH("ctr_pnn_bwd(dx, simple)");
-      rc = set_smem((const void*)pnn_bwd_dw_simple_kernel<0>, smem_dw);
-      if (rc) return rc;
-      pnn_bwd_dw_simple_kernel<0><<<dim3(gx, gy, gz), 256, smem_dw, st>>>(e, out, g_out, dwt, (int)B, (int)F, (int)K, (int)N,
-                                                                          (int)s.WX);
-    } else {
-      rc = set_smem((const void*)pnn_bwd_dx_simple_kernel<1>, smem_dx);
-      if (rc) return rc;
-      pnn_bwd_dx_simple_kernel<1><<<gdx, 256, smem_dx, st>>>(e, ws, out, g_out, d_e, (int)B, (int)F, (int)K, (int)N, (int)s.WX);
-      CTR_CHECK_LAUNCH("ctr_pnn_bwd(dx, simple)");
-      rc = set_smem((const void*)pnn_bwd_dw_simple_kernel<1>, smem_dw);
-      if (rc) return rc;
-      pnn_bwd_dw_simple_kernel<1><<<dim3(gx, gy, gz), 256, smem_dw, st>>>(e, out, g_out, dwt, (int)B, (int)F, (int)K, (int)N,
-                                                                          (int)s.WX);
-    }
-    CTR_CHECK_LAUNCH("ctr_pnn_bwd(dw, simple)");
+    rc = with_const<0, 1>(method, [&](auto M) {
+      if (int r = launch("ctr_pnn_bwd(dx, simple)", pnn_bwd_dx_simple_kernel<M>, gdx, 256, smem_dx, st, e, ws, out, g_out,
+                         d_e, (int)B, (int)F, (int)K, (int)N, (int)s.WX))
+        return r;
+      return launch("ctr_pnn_bwd(dw, simple)", pnn_bwd_dw_simple_kernel<M>, dim3(gx, gy, gz), 256, smem_dw, st, e, out,
+                    g_out, dwt, (int)B, (int)F, (int)K, (int)N, (int)s.WX);
+    });
+    if (rc) return rc;
   }
   const size_t total = (size_t)s.FK * N + N + (method == 0 ? (size_t)N * F : (size_t)N * K * K);
-  pnn_fold_kernel<<<grid_for(total, 4096), 256, 0, st>>>(dwt, wprod, d_wlin, d_wprod, d_bias, (int)F, (int)K, (int)N, method,
-                                                        (int)s.WX);
-  CTR_CHECK_LAUNCH("ctr_pnn_bwd(fold)");
-  return CTR_OK;
+  return launch("ctr_pnn_bwd(fold)", pnn_fold_kernel, grid_for(total, 4096), 256, 0, st, dwt, wprod, d_wlin,
+                d_wprod, d_bias, (int)F, (int)K, (int)N, method, (int)s.WX);
 }

@@ -1,6 +1,10 @@
-// wgmma / TMA / mbarrier PTX wrappers shared by the tensor-core kernels (sm_90a).
+// wgmma / TMA / mbarrier PTX wrappers shared by the tensor-core kernels (sm_90a), the pipeline mechanics built on them
+// (shared-memory alignment, the mbarrier ring, the producer / consumer role split, the 3xTF32 k-step, accumulation chains)
+// and the host side of a launch (tensor-map encoding, shared-memory attribute, compile-time shape dispatch).
 #pragma once
 #include <cuda.h>
+
+#include <type_traits>
 
 #include "ctr_common.cuh"
 
@@ -8,6 +12,9 @@ namespace ctr {
 namespace tc {
 
 constexpr int WG_M = 64;                 // rows of one warpgroup MMA (wgmma m64nNk8)
+constexpr int KB = 32;                   // tf32 per 128-byte swizzle row
+constexpr int NWG = 2;                   // consumer warpgroups per CTA
+constexpr int NTHREADS = (NWG + 1) * 128;  // + one producer warpgroup (one TMA thread)
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
@@ -131,21 +138,176 @@ __device__ __forceinline__ void wgmma_tf32_rs<128>(float (&d)[64], const uint32_
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(scale_d));
 }
 
+// One 3xTF32 k-step, D (+)= (ah + al) . (bhi + blo), with B `off` descriptor units into its hi and lo tiles: the small terms
+// first, the dominant hi.hi term last.  scale_d == 0 starts a new accumulation chain.
+template <int N>
+__device__ __forceinline__ void mma_3xtf32(float (&d)[N / 2], const uint32_t (&ah)[4], const uint32_t (&al)[4], uint64_t bhi,
+                                           uint64_t blo, uint64_t off, int scale_d) {
+  wgmma_tf32_rs<N>(d, al, bhi + off, scale_d);
+  wgmma_tf32_rs<N>(d, ah, blo + off, 1);
+  wgmma_tf32_rs<N>(d, ah, bhi + off, 1);
+}
+// Waits for every committed wgmma group, then releases the A fragments (hi, lo) those groups read.
+template <int NK>
+__device__ __forceinline__ void wgmma_wait_keep(uint32_t (&ah)[NK][4], uint32_t (&al)[NK][4]) {
+  wgmma_wait<0>();
+#pragma unroll
+  for (int k = 0; k < NK; ++k) { wgmma_keep(ah[k]); wgmma_keep(al[k]); }
+}
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
-                                  const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
-                                  CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+// Accumulation chains: the tensor core adds each K=8 product group into the fp32 accumulator with truncation, so a long
+// chain drifts by ~0.5 ulp per MMA.  Kernels therefore accumulate `len` steps from zero into dacc and then add dacc into
+// acc (round-to-nearest).  Step i of n: the first of a chain overwrites dacc (scale_d 0), the last one drains it.
+__device__ __forceinline__ bool chain_first(int i, int len) { return i % len == 0; }
+__device__ __forceinline__ bool chain_last(int i, int n, int len) { return (i + 1) % len == 0 || i + 1 == n; }
+template <int N>
+__device__ __forceinline__ void chain_drain(float (&acc)[N], const float (&dacc)[N]) {
+#pragma unroll
+  for (int q = 0; q < N; ++q) acc[q] += dacc[q];
+}
 
-inline EncodeTiledFn encode_tiled() {
-  static EncodeTiledFn fn = nullptr;
-  if (fn == nullptr) {
+// 3xTF32 operand in memory: dst[idx] = tf32(v) (the hi copy), dst[total + idx] = v - tf32(v) (the lo copy)
+__device__ __forceinline__ void store_split(float* dst, size_t total, size_t idx, float v) {
+  const float hi = tf32_rna(v);
+  dst[idx] = hi;
+  dst[total + idx] = v - hi;
+}
+
+// SWIZZLE_128B tiles must be 1024-byte aligned: the kernels align their dynamic shared memory here, and every launch
+// asks for 1 KB of slack on top of the layout.
+__device__ __forceinline__ uint8_t* align_1024(uint8_t* smem_raw) {
+  return smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
+}
+
+// The ring of SB shared-memory stages between the TMA producer thread and the 4 NWG consumer warps.  Stage s has a `full`
+// barrier (one arrival + the bytes of its TMA loads) and an `empty` barrier (one arrival per consumer warp); bar0 points
+// at 2 SB 8-byte barriers.  The producer and every consumer thread walk the stages in the same order, each with its own
+// copy of the (stage, phase) position.
+struct Ring {
+  uint32_t bar0;
+  int nstages;
+  int s = 0;
+  uint32_t ph = 0;
+
+  __device__ __forceinline__ Ring(uint32_t bar0_, int nstages_) : bar0(bar0_), nstages(nstages_) {}
+  __device__ __forceinline__ uint32_t full() const { return bar0 + 8 * s; }
+  __device__ __forceinline__ uint32_t empty() const { return bar0 + 8 * (nstages + s); }
+  __device__ __forceinline__ void advance() {
+    if (++s == nstages) { s = 0; ph ^= 1; }
+  }
+  // every thread of the CTA: thread 0 initialises the barriers, all return once they are visible
+  __device__ __forceinline__ void init() const {
+    if (threadIdx.x == 0) {
+      for (int i = 0; i < nstages; ++i) { mbar_init(bar0 + 8 * i, 1); mbar_init(bar0 + 8 * (nstages + i), NWG * 4); }
+      fence_barrier_init();
+    }
+    __syncthreads();
+  }
+  struct Slot {
+    int stage;
+    uint32_t full;      // the barrier the stage's TMA loads complete on
+  };
+  // producer: waits until the next stage is free and arms it for `bytes`
+  __device__ __forceinline__ Slot acquire(uint32_t bytes) {
+    mbar_wait(empty(), ph ^ 1);
+    mbar_expect_tx(full(), bytes);
+    const Slot slot = {s, full()};
+    advance();
+    return slot;
+  }
+  // consumer: waits until the current stage has landed and returns its index
+  __device__ __forceinline__ int wait() const {
+    mbar_wait(full(), ph);
+    return s;
+  }
+  // consumer warp: done with the current stage (after the wgmma.wait that covers it)
+  __device__ __forceinline__ void release(int lane) {
+    if (lane == 0) mbar_arrive(empty());
+    advance();
+  }
+};
+
+// Role split of a CTA of NTHREADS: the producer warpgroup drops to 40 registers per thread and its first thread runs
+// `producer`; the consumer warpgroups (warps 0 .. 4 NWG - 1) get 232.  Returns true on the producer warpgroup, which then
+// has nothing left to do.
+template <class Producer>
+__device__ __forceinline__ bool producer_role(int warp, int lane, Producer&& producer) {
+  if (warp >= NWG * 4) {
+    setmaxnreg_dec<40>();
+    if (warp == NWG * 4 && lane == 0) producer();
+    return true;
+  }
+  setmaxnreg_inc<232>();
+  return false;
+}
+
+// ------------------------------------------------------------------------------------------------ host
+static inline int64_t pad_to(int64_t v, int64_t q) { return (v + q - 1) / q * q; }
+// wgmma N (or K) class of a width v <= 128: 32, 64 or 128
+static inline int pad3(int64_t v) { return v <= 32 ? 32 : v <= 64 ? 64 : 128; }
+// CTAs of 256 threads over `total` elements, at most `cap`
+static inline int grid_for(size_t total, int cap) {
+  return (int)((total + 255) / 256 < (size_t)cap ? (total + 255) / 256 : (size_t)cap);
+}
+
+// The caller's workspace: at least `need` bytes (size_fn tells how many), 128-byte aligned.
+static inline int check_workspace(const char* fn, const char* size_fn, const void* ws, int64_t bytes, int64_t need) {
+  CTR_REQUIRE(ws != nullptr && bytes >= need, "%s: workspace of %lld bytes required (%s), got %lld", fn, (long long)need,
+              size_fn, (long long)bytes);
+  CTR_REQUIRE((reinterpret_cast<uintptr_t>(ws) & 127) == 0, "%s: workspace must be 128-byte aligned", fn);
+  return CTR_OK;
+}
+
+// Tensor map of a float32 tensor at `base`: dims and box innermost first, byte_strides of dimensions 1 .. rank - 1.
+static inline int encode_tmap(const char* fn, CUtensorMap* map, int rank, const void* base, const cuuint64_t* dims,
+                              const cuuint64_t* byte_strides, const cuuint32_t* box, CUtensorMapSwizzle swizzle) {
+  typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
+                                    const cuuint64_t*, const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave,
+                                    CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
+  static EncodeTiledFn enc = nullptr;
+  if (enc == nullptr) {
     void* p = nullptr;
     cudaDriverEntryPointQueryResult q;
     if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &q) == cudaSuccess &&
         q == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<EncodeTiledFn>(p);
+      enc = reinterpret_cast<EncodeTiledFn>(p);
   }
-  return fn;
+  if (enc == nullptr) {
+    set_error("%s: cuTensorMapEncodeTiled is not available from the driver", fn);
+    return CTR_ERR_CUDA;
+  }
+  const cuuint32_t elem_strides[5] = {1, 1, 1, 1, 1};
+  CUresult cr = enc(map, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, rank, const_cast<void*>(base), dims, byte_strides, box,
+                    elem_strides, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (cr != CUDA_SUCCESS) {
+    set_error("%s: cuTensorMapEncodeTiled failed with CUresult %d", fn, (int)cr);
+    return CTR_ERR_CUDA;
+  }
+  return CTR_OK;
+}
+
+// Launches k with `smem` bytes of dynamic shared memory (raising the kernel's limit past the default 48 KB when needed)
+// and checks the launch; `what` names it in the error message.
+template <class... P, class... A>
+int launch(const char* what, void (*k)(P...), dim3 grid, int block, size_t smem, cudaStream_t st, const A&... args) {
+  if (smem > 48 * 1024) CTR_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  k<<<grid, block, smem, st>>>(args...);
+  CTR_CHECK_LAUNCH(what);
+  return CTR_OK;
+}
+
+// Compile-time dispatch: returns f(std::integral_constant<int, V>{}) for the V of Vs equal to v (the kernels take their
+// shape class or method as a template argument).
+template <int... Vs, class F>
+int with_const(int v, F&& f) {
+  int rc = CTR_OK;
+  const bool hit = ((v == Vs && ((rc = f(std::integral_constant<int, Vs>{})), true)) || ...);
+  if (!hit) {
+    set_error("no kernel instantiation for %d", v);
+    return CTR_ERR_INVALID_ARG;
+  }
+  return rc;
 }
 
 }  // namespace tc

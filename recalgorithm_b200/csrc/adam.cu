@@ -369,12 +369,13 @@ extern "C" int ctr_adam_rows(float* var, float* m, float* v, int64_t state_strid
   if (max_n == 0) return CTR_OK;
   cudaStream_t st = as_stream(stream);
   const long long total = (long long)max_n * (D / 4);
-  const int grid = (int)((total + 255) / 256 < (long long)sm_count() * 16 ? (total + 255) / 256 : (long long)sm_count() * 16);
-#define GO(L) adam_rows_kernel<L><<<grid, 256, 0, st>>>(reinterpret_cast<float4*>(var), reinterpret_cast<float4*>(m), reinterpret_cast<float4*>(v), (int)(state_stride / 4), V, reinterpret_cast<const long long*>(rows), reinterpret_cast<const float4*>(grads), reinterpret_cast<const long long*>(count), max_n, lr_t, beta1, beta2, eps, touched_bitmap)
-  switch (D / 4) { case 1: GO(1); break; case 2: GO(2); break; case 4: GO(4); break; case 8: GO(8); break; case 16: GO(16); break; default: GO(32); break; }
-#undef GO
-  CTR_CHECK_LAUNCH("ctr_adam_rows");
-  return CTR_OK;
+  const int grid = capped_grid((total + 255) / 256, (long long)sm_count() * 16);
+  return with_lpr(D, [&](auto L) {
+    return launch("ctr_adam_rows", adam_rows_kernel<L>, grid, 256, 0, st, reinterpret_cast<float4*>(var), reinterpret_cast<float4*>(m),
+                  reinterpret_cast<float4*>(v), (int)(state_stride / 4), V, reinterpret_cast<const long long*>(rows),
+                  reinterpret_cast<const float4*>(grads), reinterpret_cast<const long long*>(count), max_n, lr_t, beta1, beta2, eps,
+                  touched_bitmap);
+  });
 }
 
 extern "C" int ctr_adam_dense_rest(float* var, float* m, float* v, int64_t state_stride, int64_t V, int64_t D, float lr_t, float beta1, float beta2,
@@ -387,38 +388,38 @@ extern "C" int ctr_adam_dense_rest(float* var, float* m, float* v, int64_t state
   if (V == 0) return CTR_OK;
   cudaStream_t st = as_stream(stream);
   const long long total = (long long)V * (D / 4);
-  const int grid = (int)((total + 255) / 256 < (long long)sm_count() * 32 ? (total + 255) / 256 : (long long)sm_count() * 32);
-#define GO(L) adam_dense_rest_kernel<L><<<grid, 256, 0, st>>>(reinterpret_cast<float4*>(var), reinterpret_cast<float4*>(m), reinterpret_cast<float4*>(v), (int)(state_stride / 4), V, lr_t, beta1, beta2, eps, touched_bitmap)
-  switch (D / 4) { case 1: GO(1); break; case 2: GO(2); break; case 4: GO(4); break; case 8: GO(8); break; case 16: GO(16); break; default: GO(32); break; }
-#undef GO
-  CTR_CHECK_LAUNCH("ctr_adam_dense_rest");
-  return CTR_OK;
+  const int grid = capped_grid((total + 255) / 256, (long long)sm_count() * 32);
+  return with_lpr(D, [&](auto L) {
+    return launch("ctr_adam_dense_rest", adam_dense_rest_kernel<L>, grid, 256, 0, st, reinterpret_cast<float4*>(var),
+                  reinterpret_cast<float4*>(m), reinterpret_cast<float4*>(v), (int)(state_stride / 4), V, lr_t, beta1, beta2, eps,
+                  touched_bitmap);
+  });
 }
 
 static int adam_dedup_launch(const char* fn, float* var, float* m, float* v, int64_t state_stride, int64_t D, const EntrySrc& src, long long n,
                              float* vals, int32_t* slot_of_row, int32_t* dup_list, float lr_t, float beta1, float beta2, float eps,
                              uint32_t* touched_bitmap, int64_t* n_unique, cudaStream_t st) {
   const long long total = n * (D / 4);
-  auto cap = [](long long want, long long lim) { return (int)(want < lim ? want : lim); };
-  const int grid_e = cap((n + 255) / 256, (long long)sm_count() * 16), grid_t = cap((total + 255) / 256, (long long)sm_count() * 16);
+  const int grid_e = capped_grid((n + 255) / 256, (long long)sm_count() * 16);
+  const int grid_t = capped_grid((total + 255) / 256, (long long)sm_count() * 16);
   auto* g4 = reinterpret_cast<float4*>(vals);
+  int rc;
   if (dup_list != nullptr) {
     CTR_CUDA(cudaMemsetAsync(dup_list + n, 0, sizeof(int32_t), st));
-    adam_claim_list_kernel<<<grid_e, 256, 0, st>>>(src, n, slot_of_row, dup_list, dup_list + n);
+    rc = launch(fn, adam_claim_list_kernel, grid_e, 256, 0, st, src, n, slot_of_row, dup_list, dup_list + n);
   } else {
-    adam_claim_kernel<<<grid_e, 256, 0, st>>>(src, n, slot_of_row);
+    rc = launch(fn, adam_claim_kernel, grid_e, 256, 0, st, src, n, slot_of_row);
   }
-#define GO(L)                                                                                                               \
-  if (dup_list != nullptr) adam_merge_list_kernel<L><<<sm_count() * 2, 256, 0, st>>>(src, slot_of_row, g4, dup_list, dup_list + n); \
-  else adam_merge_kernel<L><<<grid_t, 256, 0, st>>>(src, n, slot_of_row, g4);                                               \
-  adam_update_kernel<L><<<grid_t, 256, 0, st>>>(reinterpret_cast<float4*>(var), reinterpret_cast<float4*>(m),               \
-                                                reinterpret_cast<float4*>(v), (int)(state_stride / 4), src, n, slot_of_row, g4, lr_t, beta1, beta2,  \
-                                                eps, touched_bitmap, reinterpret_cast<long long*>(n_unique))
-  switch (D / 4) { case 1: GO(1); break; case 2: GO(2); break; case 4: GO(4); break; case 8: GO(8); break; case 16: GO(16); break; default: GO(32); break; }
-#undef GO
-  CTR_CHECK_LAUNCH(fn);
-  count_launch(2);
-  return CTR_OK;
+  if (rc) return rc;
+  return with_lpr(D, [&](auto L) {
+    const int r = dup_list != nullptr ? launch(fn, adam_merge_list_kernel<L>, sm_count() * 2, 256, 0, st, src, slot_of_row, g4, dup_list,
+                                               dup_list + n)
+                                      : launch(fn, adam_merge_kernel<L>, grid_t, 256, 0, st, src, n, slot_of_row, g4);
+    if (r) return r;
+    return launch(fn, adam_update_kernel<L>, grid_t, 256, 0, st, reinterpret_cast<float4*>(var), reinterpret_cast<float4*>(m),
+                  reinterpret_cast<float4*>(v), (int)(state_stride / 4), src, n, slot_of_row, g4, lr_t, beta1, beta2, eps,
+                  touched_bitmap, reinterpret_cast<long long*>(n_unique));
+  });
 }
 
 extern "C" int ctr_adam_indexed_slices(float* var, float* m, float* v, int64_t state_stride, const int64_t* field_row_offset, int64_t F, int64_t D,
@@ -458,24 +459,20 @@ template <int LPR, int HOLD>
 static int launch_bwd_adam(const float* tile, const float* d_tile, const float* d_fm2, const EntrySrc& src, int64_t B, int64_t F,
                            float* var, float* m, float* v, int SS, int32_t* slot, float* dup_grads, int32_t* dup_list, float lr_t, float b1,
                            float b2, float eps, uint32_t* touched, int64_t* n_unique, cudaStream_t st) {
-  auto k = embed_fm2_bwd_adam_kernel<LPR, HOLD>;
-  int per_sm = 1;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, 256, 0) != cudaSuccess || per_sm < 1) per_sm = 1;
-  long long grid = (long long)per_sm * sm_count();
-  if (grid > (B + 7) / 8) grid = (B + 7) / 8;
+  const char* fn = "ctr_embed_fm2_bwd_adam";
   int* n_dup = dup_list + B * F;
-  k<<<(int)grid, 256, 0, st>>>(reinterpret_cast<const float4*>(tile), reinterpret_cast<const float4*>(d_tile), d_fm2, src.off, src.ids,
-                               (int)B, (int)F, reinterpret_cast<float4*>(var), reinterpret_cast<float4*>(m),
-                               reinterpret_cast<float4*>(v), SS, slot, reinterpret_cast<float4*>(dup_grads), dup_list, n_dup, lr_t, b1, b2,
-                               eps, touched, reinterpret_cast<long long*>(n_unique));
+  int rc = launch_resident(fn, embed_fm2_bwd_adam_kernel<LPR, HOLD>, (B + 7) / 8, 256, 0, st, reinterpret_cast<const float4*>(tile),
+                           reinterpret_cast<const float4*>(d_tile), d_fm2, src.off, src.ids, (int)B, (int)F,
+                           reinterpret_cast<float4*>(var), reinterpret_cast<float4*>(m), reinterpret_cast<float4*>(v), SS, slot,
+                           reinterpret_cast<float4*>(dup_grads), dup_list, n_dup, lr_t, b1, b2, eps, touched,
+                           reinterpret_cast<long long*>(n_unique));
+  if (rc) return rc;
   const int g2 = sm_count() * 2;
-  adam_dup_merge_kernel<LPR><<<g2, 256, 0, st>>>(src, slot, reinterpret_cast<float4*>(dup_grads), dup_list, n_dup);
-  adam_dup_update_kernel<LPR><<<g2, 256, 0, st>>>(reinterpret_cast<float4*>(var), reinterpret_cast<float4*>(m),
-                                                  reinterpret_cast<float4*>(v), SS, src, slot, reinterpret_cast<const float4*>(dup_grads),
-                                                  dup_list, n_dup, lr_t, b1, b2, eps, touched, reinterpret_cast<long long*>(n_unique));
-  CTR_CHECK_LAUNCH("ctr_embed_fm2_bwd_adam");
-  count_launch(2);
-  return CTR_OK;
+  rc = launch(fn, adam_dup_merge_kernel<LPR>, g2, 256, 0, st, src, slot, reinterpret_cast<float4*>(dup_grads), dup_list, n_dup);
+  if (rc) return rc;
+  return launch(fn, adam_dup_update_kernel<LPR>, g2, 256, 0, st, reinterpret_cast<float4*>(var), reinterpret_cast<float4*>(m),
+                reinterpret_cast<float4*>(v), SS, src, slot, reinterpret_cast<const float4*>(dup_grads), dup_list, n_dup, lr_t, b1, b2,
+                eps, touched, reinterpret_cast<long long*>(n_unique));
 }
 
 template <int LPR>
@@ -483,14 +480,15 @@ static int dispatch_bwd_adam(const float* tile, const float* d_tile, const float
                              float* var, float* m, float* v, int SS, int32_t* slot, float* dup_grads, int32_t* dup_list, float lr_t, float b1,
                              float b2, float eps, uint32_t* touched, int64_t* n_unique, cudaStream_t st) {
   const int64_t per_lane = (F * LPR + 31) / 32;
-#define GO(H) return launch_bwd_adam<LPR, H>(tile, d_tile, d_fm2, src, B, F, var, m, v, SS, slot, dup_grads, dup_list, lr_t, b1, b2, eps, touched, n_unique, st)
-  if (per_lane <= 4) GO(4);
-  if (per_lane <= 8) GO(8);
-  if (per_lane <= 12) GO(12);
-#undef GO
-  set_error("ctr_embed_fm2_bwd_adam: F*D = %lld exceeds the register-resident limit of 1536 (use ctr_embed_fm2_bwd + ctr_adam_indexed_slices)",
-            (long long)(F * LPR * 4));
-  return CTR_ERR_UNSUPPORTED;
+  if (per_lane > 12) {
+    set_error("ctr_embed_fm2_bwd_adam: F*D = %lld exceeds the register-resident limit of 1536 (use ctr_embed_fm2_bwd + ctr_adam_indexed_slices)",
+              (long long)(F * LPR * 4));
+    return CTR_ERR_UNSUPPORTED;
+  }
+  return with_const<4, 8, 12>(per_lane <= 4 ? 4 : per_lane <= 8 ? 8 : 12, [&](auto H) {
+    return launch_bwd_adam<LPR, H>(tile, d_tile, d_fm2, src, B, F, var, m, v, SS, slot, dup_grads, dup_list, lr_t, b1, b2, eps, touched,
+                                   n_unique, st);
+  });
 }
 
 extern "C" int ctr_embed_fm2_bwd_adam(const float* tile, const float* d_tile, const float* d_fm2, const int64_t* field_row_offset,
@@ -510,13 +508,11 @@ extern "C" int ctr_embed_fm2_bwd_adam(const float* tile, const float* d_tile, co
   EntrySrc src = {reinterpret_cast<const long long*>(ids), reinterpret_cast<const long long*>(field_row_offset), nullptr, 0, 0, (int)F};
   const long long n = (long long)B * F;
   CTR_CUDA(cudaMemsetAsync(dup_list + n, 0, sizeof(int32_t), st));
-  const int grid_e = (int)((n + 255) / 256 < (long long)sm_count() * 16 ? (n + 255) / 256 : (long long)sm_count() * 16);
-  adam_claim_dup_kernel<<<grid_e, 256, 0, st>>>(src, n, slot_of_row);
-  count_launch(1);
-  switch (D / 4) {
-#define GO(L) case L: return dispatch_bwd_adam<L>(tile, d_tile, d_fm2, src, B, F, var, m, v, (int)(state_stride / 4), slot_of_row, dup_grads, dup_list, lr_t, beta1, beta2, eps, touched_bitmap, n_unique, st)
-    GO(1); GO(2); GO(4); GO(8); GO(16);
-    default: return dispatch_bwd_adam<32>(tile, d_tile, d_fm2, src, B, F, var, m, v, (int)(state_stride / 4), slot_of_row, dup_grads, dup_list, lr_t, beta1, beta2, eps, touched_bitmap, n_unique, st);
-#undef GO
-  }
+  rc = launch("ctr_embed_fm2_bwd_adam", adam_claim_dup_kernel, capped_grid((n + 255) / 256, (long long)sm_count() * 16), 256, 0, st, src,
+              n, slot_of_row);
+  if (rc) return rc;
+  return with_lpr(D, [&](auto L) {
+    return dispatch_bwd_adam<L>(tile, d_tile, d_fm2, src, B, F, var, m, v, (int)(state_stride / 4), slot_of_row, dup_grads, dup_list,
+                                lr_t, beta1, beta2, eps, touched_bitmap, n_unique, st);
+  });
 }

@@ -380,34 +380,19 @@ static int bst_launch_d(const char* fn, const float* q, const float* k, const fl
   const size_t smem = bst_smem_floats((int)T, D, (int)H, L.total, BWD) * sizeof(float);
   CTR_UNSUPPORTED(smem > 220 * 1024, "%s: T=%lld d=%d heads=%lld max_length=%lld needs %zu bytes of shared memory per sample (limit 220 KB)",
                   fn, (long long)T, D, (long long)H, (long long)maxlen, smem);
-  auto kern = bst_kernel<D, BWD>;
-  if (smem > 48 * 1024) CTR_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int per_sm = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, BST_NT, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
-  long long grid = (long long)per_sm * sm_count();
-  if (grid > B) grid = B;
-  kern<<<(int)grid, BST_NT, smem, st>>>(q, k, v, reinterpret_cast<const long long*>(len), params, g, (int)B, (int)T, (int)H,
-                                        (int)maxlen, use_pos, out, dq, dk, dv, dparams);
-  CTR_CHECK_LAUNCH(fn);
-  return CTR_OK;
+  return launch_resident(fn, bst_kernel<D, BWD>, B, BST_NT, smem, st, q, k, v, reinterpret_cast<const long long*>(len), params, g,
+                         (int)B, (int)T, (int)H, (int)maxlen, use_pos, out, dq, dk, dv, dparams);
 }
 
 template <bool BWD>
 static int bst_launch(const char* fn, const float* q, const float* k, const float* v, const int64_t* len, const float* params,
                       const float* g, int64_t B, int64_t T, int64_t d, int64_t H, int64_t maxlen, int use_pos, float* out,
                       float* dq, float* dk, float* dv, float* dparams, cudaStream_t st) {
-#define BST_GO(D_) return bst_launch_d<D_, BWD>(fn, q, k, v, len, params, g, B, T, H, maxlen, use_pos, out, dq, dk, dv, dparams, st)
-  switch (d) {
-    case 4: BST_GO(4);
-    case 8: BST_GO(8);
-    case 16: BST_GO(16);
-    case 32: BST_GO(32);
-    case 64: BST_GO(64);
-    default: break;
-  }
-#undef BST_GO
-  CTR_UNSUPPORTED(true, "%s: d=%lld unsupported (d_k in {4, 8, 16, 32, 64})", fn, (long long)d);
-  return CTR_OK;
+  CTR_UNSUPPORTED(d != 4 && d != 8 && d != 16 && d != 32 && d != 64, "%s: d=%lld unsupported (d_k in {4, 8, 16, 32, 64})", fn,
+                  (long long)d);
+  return with_const<4, 8, 16, 32, 64>((int)d, [&](auto D) {
+    return bst_launch_d<D, BWD>(fn, q, k, v, len, params, g, B, T, H, maxlen, use_pos, out, dq, dk, dv, dparams, st);
+  });
 }
 
 extern "C" int ctr_bst_transformer_fwd(const float* queries, const float* keys, const float* values, const int64_t* keys_length,

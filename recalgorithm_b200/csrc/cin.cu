@@ -236,7 +236,7 @@ extern "C" int ctr_cin_fwd(const float* x0, const float* xk, const float* filter
   if (!tensor_path_ok(m, hk, D, H)) {
     const size_t smem = sizeof(float) * (size_t)(m + hk) * D;
     CTR_UNSUPPORTED(smem > 200 * 1024, "ctr_cin_fwd: (m+hk)*D too large for the CUDA-core path");
-    const int grid = (int)(B < (int64_t)sm_count() * 4 ? B : (int64_t)sm_count() * 4);
+    const int grid = capped_grid(B, (int64_t)sm_count() * 4);
     return launch("ctr_cin_fwd(simple)", cin_fwd_simple_kernel, grid, 256, smem, st, x0, xk, filter, out, pooled, (int)B,
                   (int)m, (int)hk, (int)D, (int)H);
   }
@@ -246,7 +246,7 @@ extern "C" int ctr_cin_fwd(const float* x0, const float* xk, const float* filter
   if (rc) return rc;
   float* wt = static_cast<float*>(workspace);
   const int KP = (int)hk * KB;
-  rc = launch("ctr_cin_fwd(split filter)", cin_split_filter_kernel, grid_for((size_t)NP * KP, 4096), 256, 0, st, filter,
+  rc = launch("ctr_cin_fwd(split filter)", cin_split_filter_kernel, capped_grid(((size_t)NP * KP + 255) / 256, 4096), 256, 0, st, filter,
               wt, (int)m, (int)hk, (int)H, NP);
   if (rc) return rc;
   CUtensorMap tmap;
@@ -259,7 +259,7 @@ extern "C" int ctr_cin_fwd(const float* x0, const float* xk, const float* filter
   while ((1 << logD) < D) ++logD;
   const long long rows_total = (long long)B * D;
   const int n_tiles = (int)((rows_total + TILE_M - 1) / TILE_M);
-  const int grid = n_tiles < sm_count() ? n_tiles : sm_count();
+  const int grid = capped_grid(n_tiles, sm_count());
   // 3xTF32: 4 stages, chains of 8 K-blocks = 96 chained MMAs before the registers take the sum.  TF32: 6 stages, 32 blocks.
   return with_const<0, 1>(precision, [&](auto P1) {
     constexpr int PASSES = P1 ? 1 : 3, SB = P1 ? 6 : 4, CHUNK = P1 ? 32 : 8;

@@ -383,7 +383,7 @@ extern "C" int ctr_cin_bwd(const float* x0, const float* xk, const float* filter
   if (!tensor_path_ok(m, hk, D, H)) {
     const size_t smem_dx = sizeof(float) * (size_t)(2 * (m + hk) + H) * D;
     CTR_UNSUPPORTED(smem_dx > 200 * 1024, "ctr_cin_bwd: shared memory need %zu B too large", smem_dx);
-    const int grid = (int)(B < (int64_t)sms * 4 ? B : (int64_t)sms * 4);
+    const int grid = capped_grid(B, (int64_t)sms * 4);
     rc = launch("ctr_cin_bwd(dx)", cin_bwd_dx_kernel, grid, 256, smem_dx, st, x0, xk, filter, g_out, (int)B, (int)m,
                 (int)hk, (int)D, (int)H, dx0, dxk);
     if (rc) return rc;
@@ -403,11 +403,11 @@ extern "C" int ctr_cin_bwd(const float* x0, const float* xk, const float* filter
   const int NP = pad3(H);                                   // wgmma N of the dW kernel
   float* ws_w = static_cast<float*>(workspace);
   float* ws_g = ws_w + (size_t)(2 * KRP + m) * HP;          // + m rows so the i-in-step window of the lo copy stays inside
-  rc = launch("ctr_cin_bwd(split filter)", split_filter_native_kernel, grid_for((size_t)KRP * HP, 2048), 256, 0, st,
+  rc = launch("ctr_cin_bwd(split filter)", split_filter_native_kernel, capped_grid(((size_t)KRP * HP + 255) / 256, 2048), 256, 0, st,
               filter, ws_w, (int)(hk * m), (int)H, KRP, HP);
   if (rc) return rc;
   const size_t tg = (size_t)B * H * D;
-  rc = launch("ctr_cin_bwd(split grad)", split_grad_kernel, grid_for(tg, 4096), 256, 0, st, g_out, ws_g, tg);
+  rc = launch("ctr_cin_bwd(split grad)", split_grad_kernel, capped_grid((tg + 255) / 256, 4096), 256, 0, st, g_out, ws_g, tg);
   if (rc) return rc;
   int logD = 0;
   while ((1 << logD) < D) ++logD;
@@ -425,7 +425,7 @@ extern "C" int ctr_cin_bwd(const float* x0, const float* xk, const float* filter
     const int smem = SB * 2 * nkb * DX_N * 128 + 8 * 2 * SB + 1024;
     const long long rows = (long long)B * D;
     const int tiles = (int)((rows + DX_TILE - 1) / DX_TILE);
-    const int grid = tiles < sms ? tiles : sms;
+    const int grid = capped_grid(tiles, sms);
     rc = with_const<1, 2, 3, 4>(nkb, [&](auto NKB) {
       return launch("ctr_cin_bwd(dx, wgmma)", cin_bwd_dx_tc_kernel<SB, NKB>, grid, NTHREADS, smem, st, tmap, x0, xk, g_out,
                     dx0, dxk, (int)B, (int)m, (int)hk, logD, (int)H, KRP);

@@ -583,21 +583,11 @@ static size_t cross_bwd_smem(int64_t d, int64_t L, bool has_xl, bool prefetch) {
 template <int VEC, int N>
 static int launch_cross_fwd(const float* x0, const float* xl_in, const float* w, const float* b, int64_t B, int64_t d,
                             int64_t L, float* out, cudaStream_t st) {
-  auto k = cross_fwd_kernel<VEC, N>;
-  const size_t smem = sizeof(float) * 2 * (size_t)L * d;
-  if (smem > 48 * 1024) CTR_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int per_sm = 1;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, CROSS_WARPS * 32, smem);
-  if (per_sm < 1) per_sm = 1;
-  long long grid = (long long)per_sm * sm_count();
-  const long long need = (B + CROSS_WARPS - 1) / CROSS_WARPS;
-  if (grid > need) grid = need;
-  k<<<(int)grid, CROSS_WARPS * 32, smem, st>>>(x0, xl_in, w, b, (int)B, (int)d, (int)L, out);
-  CTR_CHECK_LAUNCH("ctr_cross_fwd");
-  return CTR_OK;
+  return launch_resident("ctr_cross_fwd", cross_fwd_kernel<VEC, N>, (B + CROSS_WARPS - 1) / CROSS_WARPS, CROSS_WARPS * 32,
+                         sizeof(float) * 2 * (size_t)L * d, st, x0, xl_in, w, b, (int)B, (int)d, (int)L, out);
 }
 
-template <int VEC, int N, int CPT>
+template <int VEC, int N>
 static int launch_cross_bwd(const float* x0, const float* xl_in, const float* w, const float* b, const float* g,
                             int64_t B, int64_t d, int64_t L, float* dx0, float* dxl, float* dw, float* db,
                             cudaStream_t st) {
@@ -610,73 +600,61 @@ static int launch_cross_bwd(const float* x0, const float* xl_in, const float* w,
       const int rw = wide ? 12 : 8;
       const size_t smem_r = sizeof(float) * ((size_t)2 * L * d + (size_t)rw * ((L + 1) * d + 4));
       if (smem_r <= 200 * 1024) {
-        auto pick = [&](auto tag) {
-          constexpr int RW = decltype(tag)::value;
-          return L <= 1 ? cross_bwd_reg_kernel<N, 1, RW> : L == 2 ? cross_bwd_reg_kernel<N, 2, RW>
-               : L == 3 ? cross_bwd_reg_kernel<N, 3, RW> : cross_bwd_reg_kernel<N, 4, RW>;
-        };
-        auto kr = wide ? pick(std::integral_constant<int, 12>{}) : pick(std::integral_constant<int, 8>{});
-        if (smem_r > 48 * 1024) CTR_CUDA(cudaFuncSetAttribute(kr, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_r));
-        int per_sm = 1;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kr, rw * 32, smem_r);
-        if (per_sm < 1) per_sm = 1;
-        long long grid = (long long)per_sm * sm_count();
-        const long long need = (B + rw - 1) / rw;
-        if (grid > need) grid = need;
         if (db == dw + L * d) {                          // the host API allocates dw | db back to back: one memset node
           CTR_CUDA(cudaMemsetAsync(dw, 0, sizeof(float) * 2 * L * d, st));
         } else {
           CTR_CUDA(cudaMemsetAsync(dw, 0, sizeof(float) * L * d, st));
           CTR_CUDA(cudaMemsetAsync(db, 0, sizeof(float) * L * d, st));
         }
-        kr<<<(int)grid, rw * 32, smem_r, st>>>(x0, w, b, g, (int)B, (int)d, (int)L, dx0, dw, db);
-        CTR_CHECK_LAUNCH("ctr_cross_bwd");
-        return CTR_OK;
+        auto go = [&](auto LL, auto RW) {
+          return launch_resident("ctr_cross_bwd", cross_bwd_reg_kernel<N, LL, RW>, (B + RW - 1) / RW, RW * 32, smem_r, st, x0, w, b,
+                                 g, (int)B, (int)d, (int)L, dx0, dw, db);
+        };
+        return with_const<1, 2, 3, 4>((int)L, [&](auto LL) {
+          if constexpr (N == 4 && LL == 4) return with_const<8>(rw, [&](auto RW) { return go(LL, RW); });
+          else return with_const<8, 12>(rw, [&](auto RW) { return go(LL, RW); });
+        });
       }
     }
   }
-  // double-buffered cp.async staging needs 16-byte rows (VEC == 4) and has to fit next to the parameter tables
-  const bool pf = VEC == 4 && cross_bwd_smem(d, L, xl_in != nullptr, true) <= 160 * 1024;
-  // LM = compile-time bound of the unrolled layer loops (predicated-off iterations still issue): 4 covers the reference's sweeps
-  auto k = L <= 4 ? (pf ? cross_bwd_kernel<VEC, N, CPT, VEC == 4, 4> : cross_bwd_kernel<VEC, N, CPT, false, 4>)
-                  : (pf ? cross_bwd_kernel<VEC, N, CPT, VEC == 4, 8> : cross_bwd_kernel<VEC, N, CPT, false, 8>);
-  const size_t smem = cross_bwd_smem(d, L, xl_in != nullptr, pf);
-  if (smem > 48 * 1024) CTR_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int per_sm = 1;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, CROSS_WARPS * 32, smem);
-  if (per_sm < 1) per_sm = 1;
-  if (per_sm > 2) per_sm = 2;                         // fewer CTAs -> fewer atomic merges of dw/db
-  long long grid = (long long)per_sm * sm_count();
-  const long long need = (B + CROSS_WARPS - 1) / CROSS_WARPS;
-  if (grid > need) grid = need;
+  // chunks per thread of the dw/db reduction, fixed by the largest d of the (VEC, N) class
+  constexpr int CPT = VEC * N * 32 <= 256 ? 1 : VEC * N * 32 <= 512 ? 2 : 4;
   CTR_CUDA(cudaMemsetAsync(dw, 0, sizeof(float) * L * d, st));
   CTR_CUDA(cudaMemsetAsync(db, 0, sizeof(float) * L * d, st));
-  k<<<(int)grid, CROSS_WARPS * 32, smem, st>>>(x0, xl_in, w, b, g, (int)B, (int)d, (int)L, dx0, dxl, dw, db);
-  CTR_CHECK_LAUNCH("ctr_cross_bwd");
-  return CTR_OK;
+  // LM = compile-time bound of the unrolled layer loops (predicated-off iterations still issue): 4 covers the reference's sweeps
+  auto go = [&](auto PF) {
+    auto k = L <= 4 ? cross_bwd_kernel<VEC, N, CPT, PF, 4> : cross_bwd_kernel<VEC, N, CPT, PF, 8>;
+    // fewer CTAs -> fewer atomic merges of dw/db
+    return launch_resident<2>("ctr_cross_bwd", k, (B + CROSS_WARPS - 1) / CROSS_WARPS, CROSS_WARPS * 32,
+                              cross_bwd_smem(d, L, xl_in != nullptr, PF), st, x0, xl_in, w, b, g, (int)B, (int)d, (int)L, dx0, dxl,
+                              dw, db);
+  };
+  // double-buffered cp.async staging needs 16-byte rows (VEC == 4) and has to fit next to the parameter tables, which only
+  // d > 512 (N = 8) can miss: at d = 512 and L = CROSS_LMAX the staged layout is 148 KB
+  if constexpr (VEC == 4 && N == 8) {
+    if (cross_bwd_smem(d, L, xl_in != nullptr, true) <= 160 * 1024) return go(std::true_type{});
+    return go(std::false_type{});
+  } else {
+    return go(std::bool_constant<VEC == 4>{});
+  }
+}
+
+// f(VEC, N): d is served by N element groups of VEC floats per lane, the vector path (VEC = 4) when d % 4 == 0
+template <class Fn>
+static int with_cross_class(int64_t d, Fn&& f) {
+  if (d % 4 == 0) {
+    const int64_t n = (d / 4 + 31) / 32;
+    return with_const<1, 2, 4, 8>(n <= 1 ? 1 : n <= 2 ? 2 : n <= 4 ? 4 : 8,
+                                  [&](auto N) { return f(std::integral_constant<int, 4>{}, N); });
+  }
+  const int64_t n = (d + 31) / 32;
+  return with_const<1, 2, 4, 8, 16, 32>(n <= 1 ? 1 : n <= 2 ? 2 : n <= 4 ? 4 : n <= 8 ? 8 : n <= 16 ? 16 : 32,
+                                        [&](auto N) { return f(std::integral_constant<int, 1>{}, N); });
 }
 
 }  // namespace ctr
 
 using namespace ctr;
-
-// d is served by N element groups per lane: vector path (VEC=4) when d % 4 == 0, scalar path otherwise.
-#define CTR_CROSS_DISPATCH(FN, ...)                                                          \
-  if (d % 4 == 0) {                                                                          \
-    const int64_t n = (d / 4 + 31) / 32;                                                     \
-    if (n <= 1) return FN(4, 1, __VA_ARGS__);                                                \
-    if (n <= 2) return FN(4, 2, __VA_ARGS__);                                                \
-    if (n <= 4) return FN(4, 4, __VA_ARGS__);                                                \
-    return FN(4, 8, __VA_ARGS__);                                                            \
-  } else {                                                                                   \
-    const int64_t n = (d + 31) / 32;                                                         \
-    if (n <= 1) return FN(1, 1, __VA_ARGS__);                                                \
-    if (n <= 2) return FN(1, 2, __VA_ARGS__);                                                \
-    if (n <= 4) return FN(1, 4, __VA_ARGS__);                                                \
-    if (n <= 8) return FN(1, 8, __VA_ARGS__);                                                \
-    if (n <= 16) return FN(1, 16, __VA_ARGS__);                                              \
-    return FN(1, 32, __VA_ARGS__);                                                           \
-  }
 
 static int check_cross(const char* fn, int64_t B, int64_t d, int64_t L) {
   CTR_REQUIRE(B >= 0 && d >= 1 && L >= 1, "%s: bad sizes B=%lld d=%lld L=%lld", fn, (long long)B, (long long)d,
@@ -695,9 +673,7 @@ extern "C" int ctr_cross_fwd(const float* x0, const float* xl_in, const float* w
     CTR_REQUIRE(aligned16(x0) && aligned16(xl_in) && aligned16(out), "ctr_cross_fwd: buffers must be 16-byte aligned");
   if (B == 0) return CTR_OK;
   cudaStream_t st = as_stream(stream);
-#define FWD(V, NN, ...) launch_cross_fwd<V, NN>(__VA_ARGS__)
-  CTR_CROSS_DISPATCH(FWD, x0, xl_in, w, b, B, d, L, out, st)
-#undef FWD
+  return with_cross_class(d, [&](auto VEC, auto N) { return launch_cross_fwd<VEC, N>(x0, xl_in, w, b, B, d, L, out, st); });
 }
 
 extern "C" int ctr_cross_bwd(const float* x0, const float* xl_in, const float* w, const float* b, const float* g_out,
@@ -716,11 +692,9 @@ extern "C" int ctr_cross_bwd(const float* x0, const float* xl_in, const float* w
     CTR_CUDA(cudaMemsetAsync(db, 0, sizeof(float) * L * d, st));
     return CTR_OK;
   }
-#define BWD(V, NN, ...)                                                        \
-  (d <= 256 ? launch_cross_bwd<V, NN, 1>(__VA_ARGS__)                          \
-            : d <= 512 ? launch_cross_bwd<V, NN, 2>(__VA_ARGS__) : launch_cross_bwd<V, NN, 4>(__VA_ARGS__))
-  CTR_CROSS_DISPATCH(BWD, x0, xl_in, w, b, g_out, B, d, L, dx0, dxl_in, dw, db, st)
-#undef BWD
+  return with_cross_class(d, [&](auto VEC, auto N) {
+    return launch_cross_bwd<VEC, N>(x0, xl_in, w, b, g_out, B, d, L, dx0, dxl_in, dw, db, st);
+  });
 }
 
 template <int N, typename IdT>
@@ -728,17 +702,9 @@ static int launch_embed_cross(const float* table, const int64_t* off, const IdT*
                               int64_t F, int64_t D, int64_t L, float* x0, float* out, cudaStream_t st) {
   auto k = L <= 1 ? embed_cross_fwd_kernel<N, 1, IdT> : L == 2 ? embed_cross_fwd_kernel<N, 2, IdT>
          : L == 3 ? embed_cross_fwd_kernel<N, 3, IdT> : embed_cross_fwd_kernel<N, 4, IdT>;
-  const size_t smem = sizeof(float) * ((size_t)L * F * D + F * D + 8);
-  int per_sm = 1;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, CROSS_WARPS * 32, smem);
-  if (per_sm < 1) per_sm = 1;
-  long long grid = (long long)per_sm * sm_count();
-  const long long need = (B + CROSS_WARPS - 1) / CROSS_WARPS;
-  if (grid > need) grid = need;
-  k<<<(int)grid, CROSS_WARPS * 32, smem, st>>>(table, reinterpret_cast<const long long*>(off), ids, w, b, (int)B, (int)F, (int)D,
-                                             (int)L, x0, out);
-  CTR_CHECK_LAUNCH("ctr_embed_cross_fwd");
-  return CTR_OK;
+  return launch_resident("ctr_embed_cross_fwd", k, (B + CROSS_WARPS - 1) / CROSS_WARPS, CROSS_WARPS * 32,
+                         sizeof(float) * ((size_t)L * F * D + F * D + 8), st, table, reinterpret_cast<const long long*>(off), ids, w, b,
+                         (int)B, (int)F, (int)D, (int)L, x0, out);
 }
 
 extern "C" int ctr_embed_cross_fwd(const float* table, const int64_t* field_row_offset, const void* ids, int ids_are_int32,
@@ -755,13 +721,10 @@ extern "C" int ctr_embed_cross_fwd(const float* table, const int64_t* field_row_
   CTR_REQUIRE(B < (1ll << 31), "ctr_embed_cross_fwd: batch too large");
   if (B == 0) return CTR_OK;
   cudaStream_t st = as_stream(stream);
-  const int n = (int)((d + 127) / 128);
-#define EC(NN)                                                                                                              \
-  return ids_are_int32 ? launch_embed_cross<NN, int>(table, field_row_offset, static_cast<const int*>(ids), w, b, B, F, D, L, x0, \
-                                                     out, st)                                                                \
-                       : launch_embed_cross<NN, long long>(table, field_row_offset, static_cast<const long long*>(ids), w, b, B, \
-                                                           F, D, L, x0, out, st);
-  if (n <= 1) { EC(1) } else if (n == 2) { EC(2) } else if (n == 3) { EC(3) } else { EC(4) }
-#undef EC
+  return with_const<1, 2, 3, 4>((int)((d + 127) / 128), [&](auto N) {   // d <= 512
+    return ids_are_int32 ? launch_embed_cross<N>(table, field_row_offset, static_cast<const int*>(ids), w, b, B, F, D, L, x0, out, st)
+                         : launch_embed_cross<N>(table, field_row_offset, static_cast<const long long*>(ids), w, b, B, F, D, L, x0,
+                                                 out, st);
+  });
 }
 

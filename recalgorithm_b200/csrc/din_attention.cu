@@ -670,30 +670,19 @@ static int check_din(const char* fn, int64_t B, int64_t T, int64_t H) {
   return CTR_OK;
 }
 
-template <int WARPS>
 static int din_fwd_launch(const float* query, const float* keys, const int64_t* len, const float* w1, const float* b1,
                           const float* w2, const float* b2, const float* w3, const float* b3, int64_t B, int64_t T,
                           int64_t H, int is_softmax, float* out, float* att_w, int* sched, cudaStream_t st) {
+  constexpr int WARPS = 4;
   const DinSmem L = din_layout((int)H, (int)T, WARPS, false);
   const size_t smem = sizeof(float) * (size_t)L.total;
   CTR_UNSUPPORTED(smem > 220 * 1024, "ctr_din_attention_fwd: T=%lld H=%lld needs %zu B of shared memory", (long long)T,
                   (long long)H, smem);
-  const long long need = (B + WARPS - 1) / WARPS;
-#define GO(HPV)                                                                                                   \
-  {                                                                                                               \
-    auto k = din_attention_fwd_kernel<HPV, WARPS>;                                                                \
-    if (smem > 48 * 1024) CTR_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    int per_sm = 1;                                                                                               \
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, WARPS * 32, smem);                                  \
-    long long grid = (long long)(per_sm < 1 ? 1 : per_sm) * sm_count();                                           \
-    if (grid > need) grid = need;                                                                                 \
-    k<<<(int)grid, WARPS * 32, smem, st>>>(query, keys, reinterpret_cast<const long long*>(len), w1, b1, w2, b2,  \
-                                           w3, b3, (int)B, (int)T, (int)H, is_softmax, out, att_w, sched);        \
-  }
-  if (H <= 4) GO(4) else if (H <= 8) GO(8) else if (H <= 16) GO(16) else GO(32)
-#undef GO
-  CTR_CHECK_LAUNCH("ctr_din_attention_fwd");
-  return CTR_OK;
+  return with_const<4, 8, 16, 32>(H <= 4 ? 4 : H <= 8 ? 8 : H <= 16 ? 16 : 32, [&](auto HPV) {
+    return launch_resident("ctr_din_attention_fwd", din_attention_fwd_kernel<HPV, WARPS>, (B + WARPS - 1) / WARPS, WARPS * 32, smem, st,
+                           query, keys, reinterpret_cast<const long long*>(len), w1, b1, w2, b2, w3, b3, (int)B, (int)T, (int)H,
+                           is_softmax, out, att_w, sched);
+  });
 }
 
 extern "C" int ctr_din_attention_fwd(const float* query, const float* keys, const int64_t* keys_length, const float* w1,
@@ -712,10 +701,11 @@ extern "C" int ctr_din_attention_fwd(const float* query, const float* keys, cons
   }
   if (sched_scratch != nullptr) {
     CTR_UNSUPPORTED(T > 8192, "ctr_din_attention_fwd: T=%lld too long for the schedule pass", (long long)T);
-    din_schedule_kernel<<<1, 1024, sizeof(int) * (T + 2), st>>>(reinterpret_cast<const long long*>(keys_length), (int)B, (int)T, sched_scratch);
-    count_launch();
+    rc = launch("ctr_din_attention_fwd(schedule)", din_schedule_kernel, 1, 1024, sizeof(int) * (T + 2), st,
+                reinterpret_cast<const long long*>(keys_length), (int)B, (int)T, sched_scratch);
+    if (rc) return rc;
   }
-  return din_fwd_launch<4>(query, keys, keys_length, w1, b1, w2, b2, w3, b3, B, T, H, is_softmax, out, att_w, sched_scratch, st);
+  return din_fwd_launch(query, keys, keys_length, w1, b1, w2, b2, w3, b3, B, T, H, is_softmax, out, att_w, sched_scratch, st);
 }
 
 extern "C" int ctr_din_attention_bwd(const float* query, const float* keys, const int64_t* keys_length, const float* w1,
@@ -737,10 +727,10 @@ extern "C" int ctr_din_attention_bwd(const float* query, const float* keys, cons
   }
   if (sched_scratch != nullptr) {
     CTR_UNSUPPORTED(T > 8192, "ctr_din_attention_bwd: T=%lld too long for the schedule pass", (long long)T);
-    din_schedule_kernel<<<1, 1024, sizeof(int) * (T + 2), st>>>(reinterpret_cast<const long long*>(keys_length), (int)B, (int)T, sched_scratch);
-    count_launch();
+    rc = launch("ctr_din_attention_bwd(schedule)", din_schedule_kernel, 1, 1024, sizeof(int) * (T + 2), st,
+                reinterpret_cast<const long long*>(keys_length), (int)B, (int)T, sched_scratch);
+    if (rc) return rc;
   }
-  int* sched = sched_scratch;
   const int HPv = H <= 4 ? 4 : H <= 8 ? 8 : H <= 16 ? 16 : 32;
   // 8 warps per CTA unless their staging areas do not fit the shared memory (long sequences of wide keys): then 4
   const bool w8 = sizeof(float) * (size_t)din_bwd_layout((int)H, HPv, (int)T, 8).total <= 220 * 1024;
@@ -749,23 +739,11 @@ extern "C" int ctr_din_attention_bwd(const float* query, const float* keys, cons
   const size_t smem = sizeof(float) * (size_t)L.total;
   CTR_UNSUPPORTED(smem > 220 * 1024, "ctr_din_attention_bwd: T=%lld H=%lld needs %zu B of shared memory", (long long)T,
                   (long long)H, smem);
-  const long long need = (B + warps - 1) / warps;
-#define GO2(HPV, WARPS)                                                                                           \
-  {                                                                                                               \
-    auto k = din_attention_bwd_kernel<HPV, WARPS>;                                                                \
-    if (smem > 48 * 1024) CTR_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    int per_sm = 1;                                                                                               \
-    cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, WARPS * 32, smem);                                  \
-    long long grid = (long long)(per_sm < 1 ? 1 : per_sm) * sm_count();                                           \
-    if (grid > need) grid = need;                                                                                 \
-    k<<<(int)grid, WARPS * 32, smem, st>>>(query, keys, reinterpret_cast<const long long*>(keys_length), w1, b1,  \
-                                           w2, b2, w3, b3, g_out, att_w, (int)B, (int)T, (int)H, is_softmax,      \
-                                           d_query, d_keys, d_params, sched);                                     \
-  }
-#define GO(HPV) { if (w8) GO2(HPV, 8) else GO2(HPV, 4) }
-  if (H <= 4) GO(4) else if (H <= 8) GO(8) else if (H <= 16) GO(16) else GO(32)
-#undef GO
-#undef GO2
-  CTR_CHECK_LAUNCH("ctr_din_attention_bwd");
-  return CTR_OK;
+  return with_const<4, 8, 16, 32>(HPv, [&](auto HPV) {
+    return with_const<4, 8>(warps, [&](auto WARPS) {
+      return launch_resident("ctr_din_attention_bwd", din_attention_bwd_kernel<HPV, WARPS>, (B + WARPS - 1) / WARPS, WARPS * 32, smem,
+                             st, query, keys, reinterpret_cast<const long long*>(keys_length), w1, b1, w2, b2, w3, b3, g_out, att_w,
+                             (int)B, (int)T, (int)H, is_softmax, d_query, d_keys, d_params, sched_scratch);
+    });
+  });
 }

@@ -389,17 +389,6 @@ first_order_fwd_kernel(const float* __restrict__ w, const long long* __restrict_
   }
 }
 
-template <typename K>
-static int resident_grid(K kernel, int block, size_t smem, long long blocks_needed) {
-  int per_sm = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, block, smem) != cudaSuccess || per_sm < 1)
-    per_sm = 1;
-  long long g = (long long)per_sm * sm_count();
-  if (g > blocks_needed) g = blocks_needed;
-  if (g < 1) g = 1;
-  return (int)g;
-}
-
 template <int LPR, typename IdT>
 static int launch_fwd(const float* table, const PeerTables* peers, const int64_t* off, const IdT* ids, int64_t B,
                       int64_t F, float* tile, float* fm2, int64_t* ids64_out, cudaStream_t st) {
@@ -407,29 +396,20 @@ static int launch_fwd(const float* table, const PeerTables* peers, const int64_t
   // 4 CTAs/SM (64 registers) measured 0.80 of HBM peak vs 0.71-0.80 uncapped; a next-sample id prefetch variant measured
   // neutral-to-negative (it costs spills) and was removed.  The sharded (peer-pull) variant keeps the register budget open.
   const PeerTables& pt = peers ? *peers : none;
-  const float4* tb = reinterpret_cast<const float4*>(table);
-#define EMB_LAUNCH(SH_, MINB_)                                                                                       \
-  {                                                                                                                  \
-    auto k = embed_fm2_fwd_kernel<LPR, SH_, MINB_, false, IdT>;                                                      \
-    const int grid = resident_grid(k, 256, 0, (B + 7) / 8);                                                          \
-    k<<<grid, 256, 0, st>>>(tb, pt, reinterpret_cast<const long long*>(off), ids, (int)B, (int)F,                    \
-                            reinterpret_cast<float4*>(tile), fm2, reinterpret_cast<long long*>(ids64_out), nullptr, nullptr); \
-  }
-  if (peers != nullptr) EMB_LAUNCH(true, 1) else EMB_LAUNCH(false, 4)
-#undef EMB_LAUNCH
-  CTR_CHECK_LAUNCH("ctr_embed_fm2_fwd");
-  return CTR_OK;
+  auto go = [&](auto k) {
+    return launch_resident("ctr_embed_fm2_fwd", k, (B + 7) / 8, 256, 0, st, reinterpret_cast<const float4*>(table), pt,
+                           reinterpret_cast<const long long*>(off), ids, (int)B, (int)F, reinterpret_cast<float4*>(tile), fm2,
+                           reinterpret_cast<long long*>(ids64_out), nullptr, nullptr);
+  };
+  return peers != nullptr ? go(embed_fm2_fwd_kernel<LPR, true, 1, false, IdT>) : go(embed_fm2_fwd_kernel<LPR, false, 4, false, IdT>);
 }
 
 template <int LPR, int HOLD, bool BI = false>
 static int launch_bwd(const float* tile, const float* d_tile, const float* d_fm2, int64_t B, int64_t F,
                       float* row_grads, cudaStream_t st) {
-  auto k = embed_fm2_bwd_kernel<LPR, HOLD, BI>;
-  const int grid = resident_grid(k, 256, 0, (B + 7) / 8);
-  k<<<grid, 256, 0, st>>>(reinterpret_cast<const float4*>(tile), reinterpret_cast<const float4*>(d_tile), d_fm2,
-                          (int)B, (int)F, reinterpret_cast<float4*>(row_grads));
-  CTR_CHECK_LAUNCH("ctr_embed_fm2_bwd");
-  return CTR_OK;
+  return launch_resident("ctr_embed_fm2_bwd", embed_fm2_bwd_kernel<LPR, HOLD, BI>, (B + 7) / 8, 256, 0, st,
+                         reinterpret_cast<const float4*>(tile), reinterpret_cast<const float4*>(d_tile), d_fm2, (int)B, (int)F,
+                         reinterpret_cast<float4*>(row_grads));
 }
 
 template <int LPR, bool BI = false>
@@ -445,12 +425,10 @@ static int dispatch_bwd(const float* tile, const float* d_tile, const float* d_f
 template <int LPR>
 static int launch_fwd_bi(const float* table, const int64_t* off, const int64_t* ids, int64_t B, int64_t F, float* tile,
                          float* bi, cudaStream_t st) {
-  auto k = embed_fm2_fwd_kernel<LPR, false, 4, true>;
-  const int grid = resident_grid(k, 256, 0, (B + 7) / 8);
-  k<<<grid, 256, 0, st>>>(reinterpret_cast<const float4*>(table), PeerTables{}, reinterpret_cast<const long long*>(off),
-                          reinterpret_cast<const long long*>(ids), (int)B, (int)F, reinterpret_cast<float4*>(tile), bi, nullptr, nullptr, nullptr);
-  CTR_CHECK_LAUNCH("ctr_embed_bi_fwd");
-  return CTR_OK;
+  return launch_resident("ctr_embed_bi_fwd", embed_fm2_fwd_kernel<LPR, false, 4, true>, (B + 7) / 8, 256, 0, st,
+                         reinterpret_cast<const float4*>(table), PeerTables{}, reinterpret_cast<const long long*>(off),
+                         reinterpret_cast<const long long*>(ids), (int)B, (int)F, reinterpret_cast<float4*>(tile), bi, nullptr,
+                         nullptr, nullptr);
 }
 
 static int check_bfd(const char* fn, int64_t B, int64_t F, int64_t D) {
@@ -466,14 +444,7 @@ static int check_bfd(const char* fn, int64_t B, int64_t F, int64_t D) {
 template <typename IdT>
 static int dispatch_fwd(const float* table, const PeerTables* peers, const int64_t* off, const IdT* ids, int64_t B,
                         int64_t F, int64_t D, float* tile, float* fm2, int64_t* ids64_out, cudaStream_t st) {
-  switch (D / 4) {
-    case 1: return launch_fwd<1>(table, peers, off, ids, B, F, tile, fm2, ids64_out, st);
-    case 2: return launch_fwd<2>(table, peers, off, ids, B, F, tile, fm2, ids64_out, st);
-    case 4: return launch_fwd<4>(table, peers, off, ids, B, F, tile, fm2, ids64_out, st);
-    case 8: return launch_fwd<8>(table, peers, off, ids, B, F, tile, fm2, ids64_out, st);
-    case 16: return launch_fwd<16>(table, peers, off, ids, B, F, tile, fm2, ids64_out, st);
-    default: return launch_fwd<32>(table, peers, off, ids, B, F, tile, fm2, ids64_out, st);
-  }
+  return with_lpr(D, [&](auto LPR) { return launch_fwd<LPR>(table, peers, off, ids, B, F, tile, fm2, ids64_out, st); });
 }
 
 static int fill_peers(const char* fn, PeerTables& peers, const float* const* shard_ptrs, int64_t G) {
@@ -557,14 +528,7 @@ extern "C" int ctr_embed_fm2_bwd(const float* tile, const float* d_tile, const f
               "ctr_embed_fm2_bwd: tile, d_tile and row_grads must be 16-byte aligned");
   if (B == 0) return CTR_OK;
   cudaStream_t st = as_stream(stream);
-  switch (D / 4) {
-    case 1: return dispatch_bwd<1>(tile, d_tile, d_fm2, B, F, row_grads, st);
-    case 2: return dispatch_bwd<2>(tile, d_tile, d_fm2, B, F, row_grads, st);
-    case 4: return dispatch_bwd<4>(tile, d_tile, d_fm2, B, F, row_grads, st);
-    case 8: return dispatch_bwd<8>(tile, d_tile, d_fm2, B, F, row_grads, st);
-    case 16: return dispatch_bwd<16>(tile, d_tile, d_fm2, B, F, row_grads, st);
-    default: return dispatch_bwd<32>(tile, d_tile, d_fm2, B, F, row_grads, st);
-  }
+  return with_lpr(D, [&](auto LPR) { return dispatch_bwd<LPR>(tile, d_tile, d_fm2, B, F, row_grads, st); });
 }
 
 extern "C" int ctr_embed_scatter_add(float* grad_table, const int64_t* field_row_offset, const int64_t* ids,
@@ -576,21 +540,12 @@ extern "C" int ctr_embed_scatter_add(float* grad_table, const int64_t* field_row
   if (B == 0) return CTR_OK;
   cudaStream_t st = as_stream(stream);
   const long long total = (long long)B * F * (D / 4);
-  const int grid = (int)((total + 255) / 256 < (long long)sm_count() * 16 ? (total + 255) / 256 : (long long)sm_count() * 16);
-  auto* gt = reinterpret_cast<float4*>(grad_table);
-  auto* off = reinterpret_cast<const long long*>(field_row_offset);
-  auto* idp = reinterpret_cast<const long long*>(ids);
-  auto* rg = reinterpret_cast<const float4*>(row_grads);
-  switch (D / 4) {
-    case 1: embed_scatter_add_kernel<1><<<grid, 256, 0, st>>>(gt, off, idp, rg, (int)B, (int)F); break;
-    case 2: embed_scatter_add_kernel<2><<<grid, 256, 0, st>>>(gt, off, idp, rg, (int)B, (int)F); break;
-    case 4: embed_scatter_add_kernel<4><<<grid, 256, 0, st>>>(gt, off, idp, rg, (int)B, (int)F); break;
-    case 8: embed_scatter_add_kernel<8><<<grid, 256, 0, st>>>(gt, off, idp, rg, (int)B, (int)F); break;
-    case 16: embed_scatter_add_kernel<16><<<grid, 256, 0, st>>>(gt, off, idp, rg, (int)B, (int)F); break;
-    default: embed_scatter_add_kernel<32><<<grid, 256, 0, st>>>(gt, off, idp, rg, (int)B, (int)F); break;
-  }
-  CTR_CHECK_LAUNCH("ctr_embed_scatter_add");
-  return CTR_OK;
+  const int grid = capped_grid((total + 255) / 256, (long long)sm_count() * 16);
+  return with_lpr(D, [&](auto LPR) {
+    return launch("ctr_embed_scatter_add", embed_scatter_add_kernel<LPR>, grid, 256, 0, st, reinterpret_cast<float4*>(grad_table),
+                  reinterpret_cast<const long long*>(field_row_offset), reinterpret_cast<const long long*>(ids),
+                  reinterpret_cast<const float4*>(row_grads), (int)B, (int)F);
+  });
 }
 
 static int bag_group(int64_t D) {
@@ -606,13 +561,9 @@ extern "C" int ctr_bag_lookup_fwd(const float* table, int64_t V, int64_t D, cons
   CTR_UNSUPPORTED(D > 256, "ctr_bag_lookup_fwd: D=%lld > 256", (long long)D);
   if (B == 0) return CTR_OK;
   const int G = bag_group(D);
-  const long long blocks = ((long long)B * G + 255) / 256;
-  const int grid = (int)(blocks < (long long)sm_count() * 16 ? blocks : (long long)sm_count() * 16);
-  bag_lookup_fwd_kernel<<<grid, 256, 0, as_stream(stream)>>>(table, V, (int)D, reinterpret_cast<const long long*>(ids),
-                                                             reinterpret_cast<const long long*>(offsets), (int)B, out,
-                                                             out_stride, G);
-  CTR_CHECK_LAUNCH("ctr_bag_lookup_fwd");
-  return CTR_OK;
+  return launch("ctr_bag_lookup_fwd", bag_lookup_fwd_kernel, capped_grid(((long long)B * G + 255) / 256, (long long)sm_count() * 16),
+                256, 0, as_stream(stream), table, V, (int)D, reinterpret_cast<const long long*>(ids),
+                reinterpret_cast<const long long*>(offsets), (int)B, out, out_stride, G);
 }
 
 extern "C" int ctr_bag_lookup_bwd(const float* d_out, int64_t out_stride, int64_t V, int64_t D, const int64_t* ids,
@@ -622,14 +573,9 @@ extern "C" int ctr_bag_lookup_bwd(const float* d_out, int64_t out_stride, int64_
   CTR_UNSUPPORTED(D > 256, "ctr_bag_lookup_bwd: D=%lld > 256", (long long)D);
   if (B == 0) return CTR_OK;
   const int G = bag_group(D);
-  const long long blocks = ((long long)B * G + 255) / 256;
-  const int grid = (int)(blocks < (long long)sm_count() * 16 ? blocks : (long long)sm_count() * 16);
-  bag_lookup_bwd_kernel<<<grid, 256, 0, as_stream(stream)>>>(d_out, out_stride, V, (int)D,
-                                                             reinterpret_cast<const long long*>(ids),
-                                                             reinterpret_cast<const long long*>(offsets), (int)B,
-                                                             row_grads, G);
-  CTR_CHECK_LAUNCH("ctr_bag_lookup_bwd");
-  return CTR_OK;
+  return launch("ctr_bag_lookup_bwd", bag_lookup_bwd_kernel, capped_grid(((long long)B * G + 255) / 256, (long long)sm_count() * 16),
+                256, 0, as_stream(stream), d_out, out_stride, V, (int)D, reinterpret_cast<const long long*>(ids),
+                reinterpret_cast<const long long*>(offsets), (int)B, row_grads, G);
 }
 
 extern "C" int ctr_first_order_fwd(const float* w, const int64_t* field_row_offset, const int64_t* ids, int64_t B,
@@ -637,13 +583,9 @@ extern "C" int ctr_first_order_fwd(const float* w, const int64_t* field_row_offs
   CTR_REQUIRE(w && field_row_offset && ids && out, "ctr_first_order_fwd: null argument");
   CTR_REQUIRE(B >= 0 && F >= 1 && B <= 0x7fffffffLL / 8 && F <= 65536, "ctr_first_order_fwd: bad sizes");
   if (B == 0) return CTR_OK;
-  const long long blocks = (B + 7) / 8;
-  const int grid = (int)(blocks < (long long)sm_count() * 8 ? blocks : (long long)sm_count() * 8);
-  first_order_fwd_kernel<<<grid, 256, 0, as_stream(stream)>>>(w, reinterpret_cast<const long long*>(field_row_offset),
-                                                              reinterpret_cast<const long long*>(ids), (int)B, (int)F,
-                                                              bias, out);
-  CTR_CHECK_LAUNCH("ctr_first_order_fwd");
-  return CTR_OK;
+  return launch("ctr_first_order_fwd", first_order_fwd_kernel, capped_grid((B + 7) / 8, (long long)sm_count() * 8), 256, 0,
+                as_stream(stream), w, reinterpret_cast<const long long*>(field_row_offset), reinterpret_cast<const long long*>(ids),
+                (int)B, (int)F, bias, out);
 }
 
 // ---- NFM bi-interaction pooling (SURVEY 8f.4): the same gather, (B, D) output instead of the FM2 scalar ------------------
@@ -655,14 +597,7 @@ extern "C" int ctr_embed_bi_fwd(const float* table, const int64_t* field_row_off
   CTR_REQUIRE(aligned16(table) && aligned16(tile) && aligned16(bi), "ctr_embed_bi_fwd: table, tile and bi must be 16-byte aligned");
   if (B == 0) return CTR_OK;
   cudaStream_t st = as_stream(stream);
-  switch (D / 4) {
-    case 1: return launch_fwd_bi<1>(table, field_row_offset, ids, B, F, tile, bi, st);
-    case 2: return launch_fwd_bi<2>(table, field_row_offset, ids, B, F, tile, bi, st);
-    case 4: return launch_fwd_bi<4>(table, field_row_offset, ids, B, F, tile, bi, st);
-    case 8: return launch_fwd_bi<8>(table, field_row_offset, ids, B, F, tile, bi, st);
-    case 16: return launch_fwd_bi<16>(table, field_row_offset, ids, B, F, tile, bi, st);
-    default: return launch_fwd_bi<32>(table, field_row_offset, ids, B, F, tile, bi, st);
-  }
+  return with_lpr(D, [&](auto LPR) { return launch_fwd_bi<LPR>(table, field_row_offset, ids, B, F, tile, bi, st); });
 }
 
 extern "C" int ctr_embed_bi_bwd(const float* tile, const float* d_tile, const float* d_bi, int64_t B, int64_t F, int64_t D,
@@ -674,49 +609,27 @@ extern "C" int ctr_embed_bi_bwd(const float* tile, const float* d_tile, const fl
               "ctr_embed_bi_bwd: tile, d_tile, d_bi and row_grads must be 16-byte aligned");
   if (B == 0) return CTR_OK;
   cudaStream_t st = as_stream(stream);
-  switch (D / 4) {
-    case 1: return dispatch_bwd<1, true>(tile, d_tile, d_bi, B, F, row_grads, st);
-    case 2: return dispatch_bwd<2, true>(tile, d_tile, d_bi, B, F, row_grads, st);
-    case 4: return dispatch_bwd<4, true>(tile, d_tile, d_bi, B, F, row_grads, st);
-    case 8: return dispatch_bwd<8, true>(tile, d_tile, d_bi, B, F, row_grads, st);
-    case 16: return dispatch_bwd<16, true>(tile, d_tile, d_bi, B, F, row_grads, st);
-    default: return dispatch_bwd<32, true>(tile, d_tile, d_bi, B, F, row_grads, st);
-  }
+  return with_lpr(D, [&](auto LPR) { return dispatch_bwd<LPR, true>(tile, d_tile, d_bi, B, F, row_grads, st); });
 }
 
 // ---- lookup + FM2 + fused dense(1) head over the flattened tile (e2e form: the consumer does not re-stream the tile) ------
 template <int LPR, typename IdT>
 static int launch_fwd_lin(const float* table, const PeerTables* peers, const int64_t* off, const IdT* ids, int64_t B, int64_t F,
                           float* tile, float* fm2, int64_t* ids64_out, const float* wlin, float* lin, cudaStream_t st) {
-  if (peers != nullptr) {
-    auto k = embed_fm2_fwd_kernel<LPR, true, 1, false, IdT, true>;
-    const int grid = resident_grid(k, 256, 0, (B + 7) / 8);
-    k<<<grid, 256, 0, st>>>(nullptr, *peers, reinterpret_cast<const long long*>(off), ids, (int)B, (int)F,
-                            reinterpret_cast<float4*>(tile), fm2, reinterpret_cast<long long*>(ids64_out),
-                            reinterpret_cast<const float4*>(wlin), lin);
-  } else {
-    // 3 CTAs/SM (85 registers): at the 64 registers of the plain gather this variant spills 88 bytes in its inner loop
-    auto k = embed_fm2_fwd_kernel<LPR, false, 3, false, IdT, true>;
-    const int grid = resident_grid(k, 256, 0, (B + 7) / 8);
-    k<<<grid, 256, 0, st>>>(reinterpret_cast<const float4*>(table), PeerTables{}, reinterpret_cast<const long long*>(off), ids, (int)B,
-                            (int)F, reinterpret_cast<float4*>(tile), fm2, reinterpret_cast<long long*>(ids64_out),
-                            reinterpret_cast<const float4*>(wlin), lin);
-  }
-  CTR_CHECK_LAUNCH("ctr_embed_fm2_lin_fwd");
-  return CTR_OK;
+  auto go = [&](auto k, const float4* tb, const PeerTables& pt) {
+    return launch_resident("ctr_embed_fm2_lin_fwd", k, (B + 7) / 8, 256, 0, st, tb, pt, reinterpret_cast<const long long*>(off),
+                           ids, (int)B, (int)F, reinterpret_cast<float4*>(tile), fm2, reinterpret_cast<long long*>(ids64_out),
+                           reinterpret_cast<const float4*>(wlin), lin);
+  };
+  if (peers != nullptr) return go(embed_fm2_fwd_kernel<LPR, true, 1, false, IdT, true>, nullptr, *peers);
+  // 3 CTAs/SM (85 registers): at the 64 registers of the plain gather this variant spills 88 bytes in its inner loop
+  return go(embed_fm2_fwd_kernel<LPR, false, 3, false, IdT, true>, reinterpret_cast<const float4*>(table), PeerTables{});
 }
 
 template <typename IdT>
 static int dispatch_fwd_lin(const float* table, const PeerTables* peers, const int64_t* off, const IdT* ids, int64_t B, int64_t F,
                             int64_t D, float* tile, float* fm2, int64_t* ids64_out, const float* wlin, float* lin, cudaStream_t st) {
-  switch (D / 4) {
-    case 1: return launch_fwd_lin<1>(table, peers, off, ids, B, F, tile, fm2, ids64_out, wlin, lin, st);
-    case 2: return launch_fwd_lin<2>(table, peers, off, ids, B, F, tile, fm2, ids64_out, wlin, lin, st);
-    case 4: return launch_fwd_lin<4>(table, peers, off, ids, B, F, tile, fm2, ids64_out, wlin, lin, st);
-    case 8: return launch_fwd_lin<8>(table, peers, off, ids, B, F, tile, fm2, ids64_out, wlin, lin, st);
-    case 16: return launch_fwd_lin<16>(table, peers, off, ids, B, F, tile, fm2, ids64_out, wlin, lin, st);
-    default: return launch_fwd_lin<32>(table, peers, off, ids, B, F, tile, fm2, ids64_out, wlin, lin, st);
-  }
+  return with_lpr(D, [&](auto LPR) { return launch_fwd_lin<LPR>(table, peers, off, ids, B, F, tile, fm2, ids64_out, wlin, lin, st); });
 }
 
 extern "C" int ctr_embed_fm2_lin_fwd(const float* table, const int64_t* field_row_offset, const void* ids, int ids_are_int32,
@@ -753,14 +666,10 @@ extern "C" int ctr_embed_fm2_lin_fwd_sharded(const float* const* shard_ptrs, int
 template <int LPR, int HOLD>
 static int launch_lin_bwd(const float* tile, const float* wlin, const float* d_fm2, const float* d_lin, int64_t B, int64_t F,
                           float* row_grads, float* d_wlin, cudaStream_t st) {
-  auto k = embed_fm2_lin_bwd_kernel<LPR, HOLD>;
-  const size_t smem = sizeof(float4) * 2 * (size_t)F * LPR;
-  if (smem > 48 * 1024) CTR_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  const int grid = resident_grid(k, 256, smem, (B + 7) / 8);
-  k<<<grid, 256, smem, st>>>(reinterpret_cast<const float4*>(tile), reinterpret_cast<const float4*>(wlin), d_fm2, d_lin, (int)B,
-                             (int)F, reinterpret_cast<float4*>(row_grads), reinterpret_cast<float4*>(d_wlin));
-  CTR_CHECK_LAUNCH("ctr_embed_fm2_lin_bwd");
-  return CTR_OK;
+  return launch_resident("ctr_embed_fm2_lin_bwd", embed_fm2_lin_bwd_kernel<LPR, HOLD>, (B + 7) / 8, 256,
+                         sizeof(float4) * 2 * (size_t)F * LPR, st, reinterpret_cast<const float4*>(tile),
+                         reinterpret_cast<const float4*>(wlin), d_fm2, d_lin, (int)B, (int)F, reinterpret_cast<float4*>(row_grads),
+                         reinterpret_cast<float4*>(d_wlin));
 }
 
 template <int LPR>
@@ -784,27 +693,17 @@ extern "C" int ctr_embed_fm2_lin_bwd(const float* tile, const float* wlin, const
   cudaStream_t st = as_stream(stream);
   CTR_CUDA(cudaMemsetAsync(d_wlin, 0, sizeof(float) * F * D, st));
   if (B == 0) return CTR_OK;
-  switch (D / 4) {
-    case 1: return dispatch_lin_bwd<1>(tile, wlin, d_fm2, d_lin, B, F, row_grads, d_wlin, st);
-    case 2: return dispatch_lin_bwd<2>(tile, wlin, d_fm2, d_lin, B, F, row_grads, d_wlin, st);
-    case 4: return dispatch_lin_bwd<4>(tile, wlin, d_fm2, d_lin, B, F, row_grads, d_wlin, st);
-    case 8: return dispatch_lin_bwd<8>(tile, wlin, d_fm2, d_lin, B, F, row_grads, d_wlin, st);
-    case 16: return dispatch_lin_bwd<16>(tile, wlin, d_fm2, d_lin, B, F, row_grads, d_wlin, st);
-    default: return dispatch_lin_bwd<32>(tile, wlin, d_fm2, d_lin, B, F, row_grads, d_wlin, st);
-  }
+  return with_lpr(D, [&](auto LPR) { return dispatch_lin_bwd<LPR>(tile, wlin, d_fm2, d_lin, B, F, row_grads, d_wlin, st); });
 }
 
 // ---- sequence lookup: (B, T) ids into ONE table -> (B, T, D), zero rows for id -1 / out of range (the zero padding of
 // tf.contrib.feature_column.sequence_input_layer, DIN/din.py:209-214) -------------------------------------------------------
 template <int LPR>
 static int launch_seq(const float* table, const int64_t* range2, const int64_t* ids, int64_t B, int64_t T, float* out, cudaStream_t st) {
-  auto k = embed_fm2_fwd_kernel<LPR, false, 4, false, long long, false, true>;
-  const int grid = resident_grid(k, 256, 0, (B + 7) / 8);
-  k<<<grid, 256, 0, st>>>(reinterpret_cast<const float4*>(table), PeerTables{}, reinterpret_cast<const long long*>(range2),
-                          reinterpret_cast<const long long*>(ids), (int)B, (int)T, reinterpret_cast<float4*>(out), nullptr, nullptr,
-                          nullptr, nullptr);
-  CTR_CHECK_LAUNCH("ctr_embed_seq_fwd");
-  return CTR_OK;
+  return launch_resident("ctr_embed_seq_fwd", embed_fm2_fwd_kernel<LPR, false, 4, false, long long, false, true>, (B + 7) / 8, 256,
+                         0, st, reinterpret_cast<const float4*>(table), PeerTables{}, reinterpret_cast<const long long*>(range2),
+                         reinterpret_cast<const long long*>(ids), (int)B, (int)T, reinterpret_cast<float4*>(out), nullptr, nullptr,
+                         nullptr, nullptr);
 }
 
 extern "C" int ctr_embed_seq_fwd(const float* table, const int64_t* row_range, const int64_t* ids, int64_t B, int64_t T, int64_t D,
@@ -815,12 +714,5 @@ extern "C" int ctr_embed_seq_fwd(const float* table, const int64_t* row_range, c
   CTR_REQUIRE(aligned16(table) && aligned16(out), "ctr_embed_seq_fwd: table and out must be 16-byte aligned");
   if (B == 0 || T == 0) return CTR_OK;
   cudaStream_t st = as_stream(stream);
-  switch (D / 4) {
-    case 1: return launch_seq<1>(table, row_range, ids, B, T, out, st);
-    case 2: return launch_seq<2>(table, row_range, ids, B, T, out, st);
-    case 4: return launch_seq<4>(table, row_range, ids, B, T, out, st);
-    case 8: return launch_seq<8>(table, row_range, ids, B, T, out, st);
-    case 16: return launch_seq<16>(table, row_range, ids, B, T, out, st);
-    default: return launch_seq<32>(table, row_range, ids, B, T, out, st);
-  }
+  return with_lpr(D, [&](auto LPR) { return launch_seq<LPR>(table, row_range, ids, B, T, out, st); });
 }

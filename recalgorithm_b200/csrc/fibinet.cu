@@ -833,10 +833,14 @@ static int rr_tile(int F, int K, int arrays, size_t fixed, size_t budget) {
   return bs;
 }
 
-static int grid_for(long long need, int per_sm) {
-  long long g = (long long)sm_count() * per_sm;
-  if (g > need) g = need;
-  return (int)(g < 1 ? 1 : g);
+// f(K, KT) for the tournament kernels of K in {8, 16, 32}: kt 1 and 2 as given, any other kt as 4 (K <= 16) or 2 (K = 32)
+template <class Fn>
+static int with_rr(int64_t K, int kt, Fn&& f) {
+  return with_const<8, 16, 32>((int)K, [&](auto KK) {
+    const int KT = kt == 1 || kt == 2 ? kt : KK <= 16 ? 4 : 2;
+    if constexpr (KK <= 16) return with_const<1, 2, 4>(KT, [&](auto T) { return f(KK, T); });
+    else return with_const<1, 2>(KT, [&](auto T) { return f(KK, T); });
+  });
 }
 
 }  // namespace ctr
@@ -859,12 +863,8 @@ extern "C" int ctr_senet_fwd(const float* x, const float* w1, const float* w2, i
   CTR_REQUIRE(x && w1 && w2 && out, "ctr_senet_fwd: null argument");
   if (B == 0) return CTR_OK;
   const size_t smem = sizeof(float) * (2 * F * r + SENET_WARPS * (3 * F + 2 * r));
-  auto k = senet_kernel<false>;
-  if (smem > 48 * 1024) CTR_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k<<<grid_for((B + SENET_WARPS - 1) / SENET_WARPS, 8), SENET_WARPS * 32, smem, as_stream(stream)>>>(
-      x, w1, w2, nullptr, (int)B, (int)F, (int)K, (int)r, out, nullptr, nullptr);
-  CTR_CHECK_LAUNCH("ctr_senet_fwd");
-  return CTR_OK;
+  return launch("ctr_senet_fwd", senet_kernel<false>, capped_grid((B + SENET_WARPS - 1) / SENET_WARPS, (long long)sm_count() * 8),
+                SENET_WARPS * 32, smem, as_stream(stream), x, w1, w2, nullptr, (int)B, (int)F, (int)K, (int)r, out, nullptr, nullptr);
 }
 
 extern "C" int ctr_senet_bwd(const float* x, const float* w1, const float* w2, const float* g_out, int64_t B, int64_t F,
@@ -877,12 +877,8 @@ extern "C" int ctr_senet_bwd(const float* x, const float* w1, const float* w2, c
   CTR_CUDA(cudaMemsetAsync(dw2, 0, sizeof(float) * F * r, st));
   if (B == 0) return CTR_OK;
   const size_t smem = sizeof(float) * (4 * F * r + SENET_WARPS * (3 * F + 2 * r));
-  auto k = senet_kernel<true>;
-  if (smem > 48 * 1024) CTR_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k<<<grid_for((B + SENET_WARPS - 1) / SENET_WARPS, 4), SENET_WARPS * 32, smem, st>>>(
-      x, w1, w2, g_out, (int)B, (int)F, (int)K, (int)r, dx, dw1, dw2);
-  CTR_CHECK_LAUNCH("ctr_senet_bwd");
-  return CTR_OK;
+  return launch("ctr_senet_bwd", senet_kernel<true>, capped_grid((B + SENET_WARPS - 1) / SENET_WARPS, (long long)sm_count() * 4),
+                SENET_WARPS * 32, smem, st, x, w1, w2, g_out, (int)B, (int)F, (int)K, (int)r, dx, dw1, dw2);
 }
 
 
@@ -899,19 +895,6 @@ static bool st_usable(int64_t K, int type, const void* a, const void* b, const v
   if (K != 8 && K != 16 && K != 32) return false;
   return aligned16(a) && aligned16(b) && aligned16(c) && (d == nullptr || aligned16(d));
 }
-#define ST_DISPATCH(K, type, NAME, ...)                                                  \
-  if (K == 8) { if (type == 0) { auto kern = NAME<8, 0>; __VA_ARGS__ } else { auto kern = NAME<8, 1>; __VA_ARGS__ } }        \
-  else if (K == 16) { if (type == 0) { auto kern = NAME<16, 0>; __VA_ARGS__ } else { auto kern = NAME<16, 1>; __VA_ARGS__ } } \
-  else { if (type == 0) { auto kern = NAME<32, 0>; __VA_ARGS__ } else { auto kern = NAME<32, 1>; __VA_ARGS__ } }
-
-#define RR_DISPATCH_KT(KK, kt, NAME, ...)                                  \
-  if (kt == 1) { auto kern = NAME<KK, 1>; __VA_ARGS__ }                   \
-  else if (kt == 2) { auto kern = NAME<KK, 2>; __VA_ARGS__ }              \
-  else { auto kern = NAME<KK, (KK <= 16 ? 4 : 2)>; __VA_ARGS__ }
-#define RR_DISPATCH(K, kt, NAME, ...)                                     \
-  if (K == 8) { RR_DISPATCH_KT(8, kt, NAME, __VA_ARGS__) }                \
-  else if (K == 16) { RR_DISPATCH_KT(16, kt, NAME, __VA_ARGS__) }         \
-  else { RR_DISPATCH_KT(32, kt, NAME, __VA_ARGS__) }
 
 extern "C" int ctr_bilinear_set_rr(int mask) {
   const int prev = g_bilinear_rr | (g_bilinear_old << 3) | (g_bilinear_tile << 4) | (g_bilinear_kt << 10);
@@ -946,44 +929,29 @@ extern "C" int ctr_bilinear_fwd(const float* x, const float* w, int64_t B, int64
     if (bs < 1) bs = rr_tile((int)F, (int)K, 1, fixed, 200 * 1024);
     if (bs >= 1) {
       const size_t smem_rr = fixed + sizeof(float) * bs * F * K;
-      const int kt = rr_kt((int)K);
-      const int threads = 256;
-      RR_DISPATCH(K, kt, bilinear_rr_fwd_kernel, {
-        if (smem_rr > 48 * 1024) CTR_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_rr));
-        int per_sm = 1;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem_rr);
-        kern<<<grid_for((B + bs - 1) / bs, per_sm < 1 ? 1 : per_sm), threads, smem_rr, st>>>(x, w, type, (int)B, (int)F, bs, out);
+      return with_rr(K, rr_kt((int)K), [&](auto KK, auto KT) {
+        return launch_resident("ctr_bilinear_fwd", bilinear_rr_fwd_kernel<KK, KT>, (B + bs - 1) / bs, 256, smem_rr, st, x, w, type,
+                               (int)B, (int)F, bs, out);
       });
-      CTR_CHECK_LAUNCH("ctr_bilinear_fwd");
-      return CTR_OK;
     }
   }
   if (st_usable(K, type, x, w, out, nullptr)) {
     const int64_t nw = type == 0 ? 1 : n;
     const size_t smem_st = sizeof(float) * (nw * K * K + 2 * F * K + n * K) + sizeof(int) * P;
     if (smem_st <= 200 * 1024) {
-      ST_DISPATCH(K, type, bilinear_st_fwd_kernel, {
-        if (smem_st > 48 * 1024) CTR_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_st));
-        int per_sm = 1;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, BST_THREADS, smem_st);
-        kern<<<grid_for(B, per_sm < 1 ? 1 : per_sm), BST_THREADS, smem_st, st>>>(x, w, (int)B, (int)F, out);
+      return with_const<8, 16, 32>((int)K, [&](auto KK) {
+        return with_const<0, 1>(type, [&](auto T) {
+          return launch_resident("ctr_bilinear_fwd", bilinear_st_fwd_kernel<KK, T>, B, BST_THREADS, smem_st, st, x, w, (int)B, (int)F,
+                                 out);
+        });
       });
-      CTR_CHECK_LAUNCH("ctr_bilinear_fwd");
-      return CTR_OK;
     }
   }
   const size_t smem = sizeof(float) * (F * K + n * K) + sizeof(int) * P;
-  const int grid = grid_for(B, 8);
-#define LAUNCH(T)                                                                                            \
-  {                                                                                                          \
-    auto k = bilinear_fwd_kernel<T>;                                                                         \
-    if (smem > 48 * 1024) CTR_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    k<<<grid, BIL_THREADS, smem, st>>>(x, w, (int)B, (int)F, (int)K, out);                                   \
-  }
-  if (type == 0) LAUNCH(0) else if (type == 1) LAUNCH(1) else LAUNCH(2)
-#undef LAUNCH
-  CTR_CHECK_LAUNCH("ctr_bilinear_fwd");
-  return CTR_OK;
+  return with_const<0, 1, 2>(type, [&](auto T) {
+    return launch("ctr_bilinear_fwd", bilinear_fwd_kernel<T>, capped_grid(B, (long long)sm_count() * 8), BIL_THREADS, smem, st, x, w,
+                  (int)B, (int)F, (int)K, out);
+  });
 }
 
 extern "C" int ctr_bilinear_bwd(const float* x, const float* w, const float* g_out, int64_t B, int64_t F, int64_t K,
@@ -1011,13 +979,11 @@ extern "C" int ctr_bilinear_bwd(const float* x, const float* w, const float* g_o
     if (bs > RR_GP) bs = RR_GP;                                  // the dX kernel keeps the tile's g values in registers
     if (bs >= 1) {
       const size_t smem_rr = fixed + sizeof(float) * 2 * bs * F * K;
-      RR_DISPATCH(K, kt, bilinear_rr_bwd_dx_kernel, {
-        if (smem_rr > 48 * 1024) CTR_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_rr));
-        int per_sm = 1;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem_rr);
-        kern<<<grid_for((B + bs - 1) / bs, per_sm < 1 ? 1 : per_sm), threads, smem_rr, st>>>(x, w, g_out, type, (int)B, (int)F, bs, dx);
+      rc = with_rr(K, kt, [&](auto KK, auto KT) {
+        return launch_resident("ctr_bilinear_bwd(dx)", bilinear_rr_bwd_dx_kernel<KK, KT>, (B + bs - 1) / bs, threads, smem_rr, st, x, w,
+                               g_out, type, (int)B, (int)F, bs, dx);
       });
-      CTR_CHECK_LAUNCH("ctr_bilinear_bwd(dx)");
+      if (rc) return rc;
       // weight gradient: one CTA per (block of adjacent pairs, batch chunk); ~8 CTAs per SM (the loads are latency-bound: ncu
       // long-scoreboard 12.6 per issue at 4), at least 32 samples per chunk
       const int dw_threads = 256, dw_groups = dw_threads / lp;
@@ -1027,55 +993,42 @@ extern "C" int ctr_bilinear_bwd(const float* x, const float* w, const float* g_o
       if (chunks > max_chunks) chunks = max_chunks;
       if (chunks < 1) chunks = 1;
       const size_t smem_dw = sizeof(float) * dw_groups * 2 * K;
-      RR_DISPATCH(K, kt, bilinear_rr_bwd_dw_kernel, {
-        kern<<<dim3((unsigned)pair_blocks, (unsigned)chunks), dw_threads, smem_dw, st>>>(x, g_out, type, (int)B, (int)F, dw);
+      return with_rr(K, kt, [&](auto KK, auto KT) {
+        return launch("ctr_bilinear_bwd(dw)", bilinear_rr_bwd_dw_kernel<KK, KT>, dim3((unsigned)pair_blocks, (unsigned)chunks), dw_threads,
+                      smem_dw, st, x, g_out, type, (int)B, (int)F, dw);
       });
-      CTR_CHECK_LAUNCH("ctr_bilinear_bwd(dw)");
-      return CTR_OK;
     }
   }
   if (type == 2) {
     const size_t smem = sizeof(float) * (2 * F * K + P * K) + sizeof(int) * P;
     CTR_UNSUPPORTED(smem > 200 * 1024, "ctr_bilinear_bwd: F=%lld K=%lld needs %zu B of shared memory", (long long)F,
                     (long long)K, smem);
-    auto k = bilinear_bwd_interaction_dx_kernel;
-    if (smem > 48 * 1024) CTR_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    k<<<grid_for(B, 8), BIL_THREADS, smem, st>>>(x, w, g_out, (int)B, (int)F, (int)K, dx);
-    CTR_CHECK_LAUNCH("ctr_bilinear_bwd(dx)");
+    rc = launch("ctr_bilinear_bwd(dx)", bilinear_bwd_interaction_dx_kernel, capped_grid(B, (long long)sm_count() * 8), BIL_THREADS, smem, st,
+                x, w, g_out, (int)B, (int)F, (int)K, dx);
+    if (rc) return rc;
     int nsplit = (int)((B + 255) / 256);
     if (nsplit > 16) nsplit = 16;
     const int threads = (int)(K * K < 1024 ? ((K * K + 31) / 32) * 32 : 1024);
-    bilinear_bwd_interaction_dw_kernel<<<dim3((unsigned)P, (unsigned)nsplit), threads, 0, st>>>(x, g_out, (int)B, (int)F,
-                                                                                               (int)K, dw);
-    CTR_CHECK_LAUNCH("ctr_bilinear_bwd(dw)");
-    return CTR_OK;
+    return launch("ctr_bilinear_bwd(dw)", bilinear_bwd_interaction_dw_kernel, dim3((unsigned)P, (unsigned)nsplit), threads, 0, st, x, g_out,
+                  (int)B, (int)F, (int)K, dw);
   }
   if (st_usable(K, type, x, w, dx, dw) && aligned16(g_out)) {
     const int64_t nw = type == 0 ? 1 : n;
     const size_t smem_st = sizeof(float) * (2 * nw * K * K + 2 * F * K + 2 * P * K + 2 * n * K);
     if (smem_st <= 200 * 1024) {
-      ST_DISPATCH(K, type, bilinear_st_bwd_kernel, {
-        if (smem_st > 48 * 1024) CTR_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_st));
-        int per_sm = 1;
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, BST_THREADS, smem_st);
-        kern<<<grid_for(B, per_sm < 1 ? 1 : per_sm), BST_THREADS, smem_st, st>>>(x, w, g_out, (int)B, (int)F, dx, dw);
+      return with_const<8, 16, 32>((int)K, [&](auto KK) {
+        return with_const<0, 1>(type, [&](auto T) {
+          return launch_resident("ctr_bilinear_bwd", bilinear_st_bwd_kernel<KK, T>, B, BST_THREADS, smem_st, st, x, w, g_out, (int)B,
+                                 (int)F, dx, dw);
+        });
       });
-      CTR_CHECK_LAUNCH("ctr_bilinear_bwd");
-      return CTR_OK;
     }
   }
   const size_t smem = sizeof(float) * (F * K + 2 * n * K + (type == 0 ? 1 : n) * K * K);
   CTR_UNSUPPORTED(smem > 200 * 1024, "ctr_bilinear_bwd: F=%lld K=%lld needs %zu B of shared memory", (long long)F,
                   (long long)K, smem);
-  const int grid = grid_for(B, 2);
-#define LAUNCH(T)                                                                                            \
-  {                                                                                                          \
-    auto k = bilinear_bwd_kernel<T>;                                                                         \
-    if (smem > 48 * 1024) CTR_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem)); \
-    k<<<grid, BIL_THREADS, smem, st>>>(x, w, g_out, (int)B, (int)F, (int)K, dx, dw);                         \
-  }
-  if (type == 0) LAUNCH(0) else LAUNCH(1)
-#undef LAUNCH
-  CTR_CHECK_LAUNCH("ctr_bilinear_bwd");
-  return CTR_OK;
+  return with_const<0, 1>(type, [&](auto T) {     // type 2 took the interaction path above
+    return launch("ctr_bilinear_bwd", bilinear_bwd_kernel<T>, capped_grid(B, (long long)sm_count() * 2), BIL_THREADS, smem, st, x, w,
+                  g_out, (int)B, (int)F, (int)K, dx, dw);
+  });
 }

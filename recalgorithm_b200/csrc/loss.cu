@@ -42,8 +42,6 @@ extern "C" int ctr_sigmoid_ce(const float* logit_a, const float* logit_b, const 
   cudaStream_t st = as_stream(stream);
   CTR_CUDA(cudaMemsetAsync(loss, 0, sizeof(float), st));
   if (B == 0) return CTR_OK;
-  const int grid = (int)((B + 255) / 256 < (int64_t)sm_count() * 2 ? (B + 255) / 256 : (int64_t)sm_count() * 2);
-  sigmoid_ce_kernel<<<grid, 256, 0, st>>>(logit_a, logit_b, labels, (int)B, 1.f / (float)B, loss, d_logit);
-  CTR_CHECK_LAUNCH("ctr_sigmoid_ce");
-  return CTR_OK;
+  return launch("ctr_sigmoid_ce", sigmoid_ce_kernel, capped_grid((B + 255) / 256, (int64_t)sm_count() * 2), 256, 0, st, logit_a,
+                logit_b, labels, (int)B, 1.f / (float)B, loss, d_logit);
 }

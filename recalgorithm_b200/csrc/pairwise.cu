@@ -315,42 +315,31 @@ ffm_kernel(const float* __restrict__ tile, const float* __restrict__ g, int B, i
   }
 }
 
-template <typename Kern>
-static int pw_grid(Kern k, size_t smem, int64_t B) {
-  int per_sm = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, PW_WARPS * 32, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
-  long long g = (long long)per_sm * sm_count(), need = (B + PW_WARPS - 1) / PW_WARPS;
-  return (int)(g < need ? g : (need < 1 ? 1 : need));
-}
-
 template <int K, int TU, bool BWD>
 static int afm_launch(const float* tile, const float* w, const float* b, const float* h, const float* g, int64_t B, int64_t F,
                       int64_t T, float* pooled, float* score, float* d_tile, float* d_w, float* d_b, float* d_h, cudaStream_t st) {
   const int64_t PP = (F * (F - 1) / 2 + 3) & ~3LL;
   const size_t smem = (size_t)PW_WARPS * (F * K + PP + (BWD ? PP + F * K : 0)) * sizeof(float);
-  auto k = afm_kernel<K, TU, BWD>;
   CTR_UNSUPPORTED(smem > 200 * 1024, "ctr_afm: F=%lld K=%d needs %zu bytes of shared memory", (long long)F, K, smem);
-  if (smem > 48 * 1024) CTR_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k<<<pw_grid(k, smem, B), PW_WARPS * 32, smem, st>>>(tile, w, b, h, g, (int)B, (int)F, (int)T, pooled, score, d_tile, d_w, d_b, d_h);
-  CTR_CHECK_LAUNCH(BWD ? "ctr_afm_bwd" : "ctr_afm_fwd");
-  return CTR_OK;
+  return launch_resident(BWD ? "ctr_afm_bwd" : "ctr_afm_fwd", afm_kernel<K, TU, BWD>, (B + PW_WARPS - 1) / PW_WARPS, PW_WARPS * 32,
+                         smem, st, tile, w, b, h, g, (int)B, (int)F, (int)T, pooled, score, d_tile, d_w, d_b, d_h);
 }
 
 template <bool BWD>
 static int afm_dispatch(const float* tile, const float* w, const float* b, const float* h, const float* g, int64_t B, int64_t F,
                         int64_t K, int64_t T, float* pooled, float* score, float* d_tile, float* d_w, float* d_b, float* d_h,
                         cudaStream_t st) {
-  const int tu = (int)((T + 31) / 32);
-#define AFM_GO(K_, TU_) return afm_launch<K_, TU_, BWD>(tile, w, b, h, g, B, F, T, pooled, score, d_tile, d_w, d_b, d_h, st)
+  const int64_t tu = (T + 31) / 32;
   // register budget: W (and dW in the backward) columns live in registers, K * TU <= 64 floats each
-  if (K == 4)  { if (tu <= 1) AFM_GO(4, 1);  if (tu <= 2) AFM_GO(4, 2);  if (tu <= 4) AFM_GO(4, 4);  if (tu <= 8) AFM_GO(4, 8); }
-  if (K == 8)  { if (tu <= 1) AFM_GO(8, 1);  if (tu <= 2) AFM_GO(8, 2);  if (tu <= 4) AFM_GO(8, 4);  if (tu <= 8) AFM_GO(8, 8); }
-  if (K == 16) { if (tu <= 1) AFM_GO(16, 1); if (tu <= 2) AFM_GO(16, 2); if (tu <= 4) AFM_GO(16, 4); }
-  if (K == 32) { if (tu <= 1) AFM_GO(32, 1); if (tu <= 2) AFM_GO(32, 2); }
-#undef AFM_GO
-  CTR_UNSUPPORTED(true, "ctr_afm: K=%lld, attention_factor=%lld unsupported (K in {4,8,16,32}, K*ceil(t/32) <= 64)",
-                  (long long)K, (long long)T);
-  return CTR_OK;
+  CTR_UNSUPPORTED((K != 4 && K != 8 && K != 16 && K != 32) || tu > 8 || K * tu > 64,
+                  "ctr_afm: K=%lld, attention_factor=%lld unsupported (K in {4,8,16,32}, K*ceil(t/32) <= 64)", (long long)K,
+                  (long long)T);
+  return with_const<4, 8, 16, 32>((int)K, [&](auto KK) {
+    return with_const<1, 2, 4, 8>(tu <= 1 ? 1 : tu <= 2 ? 2 : tu <= 4 ? 4 : 8, [&](auto TU) {
+      if constexpr (KK * TU <= 64) return afm_launch<KK, TU, BWD>(tile, w, b, h, g, B, F, T, pooled, score, d_tile, d_w, d_b, d_h, st);
+      else return (int)CTR_ERR_UNSUPPORTED;   // refused above
+    });
+  });
 }
 
 }  // namespace ctr
@@ -369,11 +358,8 @@ static int fwfm_launch(const char* fn, const float* tile, const float* r, const 
   const int64_t P = F * (F - 1) / 2, PP = (P + 3) & ~3LL, FF = (F * F + 3) & ~3LL, KP = VEC ? K + 4 : K + 1;
   const size_t smem = (size_t)(FF + (BWD ? PP : 0) + PW_WARPS * F * KP) * sizeof(float);
   CTR_UNSUPPORTED(smem > 200 * 1024, "%s: F=%lld K=%lld needs %zu bytes of shared memory", fn, (long long)F, (long long)K, smem);
-  auto k = fwfm_kernel<BWD, VEC>;
-  if (smem > 48 * 1024) CTR_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k<<<pw_grid(k, smem, B), PW_WARPS * 32, smem, st>>>(tile, r, g, (int)B, (int)F, (int)K, out, d_tile, d_r);
-  CTR_CHECK_LAUNCH(fn);
-  return CTR_OK;
+  return launch_resident(fn, fwfm_kernel<BWD, VEC>, (B + PW_WARPS - 1) / PW_WARPS, PW_WARPS * 32, smem, st, tile, r, g, (int)B, (int)F,
+                         (int)K, out, d_tile, d_r);
 }
 
 static int fwfm_run(bool bwd, const float* tile, const float* r, const float* g, int64_t B, int64_t F, int64_t K, float* out,
@@ -433,12 +419,9 @@ static int ffm_run(bool bwd, const float* tile, const float* g, int64_t B, int64
   if (rc) return rc;
   CTR_REQUIRE(F * (F - 1) * K < (1LL << 30), "%s: F=%lld K=%lld too large", fn, (long long)F, (long long)K);
   if (B == 0) return CTR_OK;
-  const long long need = (B + 7) / 8;
-  const int grid = (int)(need < (long long)sm_count() * 8 ? need : (long long)sm_count() * 8);
-  if (bwd) ffm_kernel<true><<<grid, 256, 0, as_stream(stream)>>>(tile, g, (int)B, (int)F, (int)K, nullptr, d_tile);
-  else ffm_kernel<false><<<grid, 256, 0, as_stream(stream)>>>(tile, nullptr, (int)B, (int)F, (int)K, out, nullptr);
-  CTR_CHECK_LAUNCH(fn);
-  return CTR_OK;
+  const int grid = capped_grid((B + 7) / 8, (long long)sm_count() * 8);
+  if (bwd) return launch(fn, ffm_kernel<true>, grid, 256, 0, as_stream(stream), tile, g, (int)B, (int)F, (int)K, nullptr, d_tile);
+  return launch(fn, ffm_kernel<false>, grid, 256, 0, as_stream(stream), tile, nullptr, (int)B, (int)F, (int)K, out, nullptr);
 }
 
 extern "C" int ctr_ffm_fwd(const float* tile, int64_t B, int64_t F, int64_t K, float* out, void* stream) {

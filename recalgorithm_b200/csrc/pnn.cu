@@ -710,7 +710,7 @@ extern "C" int ctr_pnn_fwd(const float* e, const float* wlin, const float* wprod
   float* ws = static_cast<float*>(workspace);
   const int sms = sm_count();
   if (s.tc) {
-    rc = launch("ctr_pnn_fwd(prep)", pnn_prep_kernel, grid_for((size_t)s.NP * s.WP, 2048), 256, 0, st, wlin, wprod, bias, ws,
+    rc = launch("ctr_pnn_fwd(prep)", pnn_prep_kernel, capped_grid(((size_t)s.NP * s.WP + 255) / 256, 2048), 256, 0, st, wlin, wprod, bias, ws,
                 (int)F, (int)K, (int)N, method, (int)s.WX, (int)s.NP, s.WP, 0, 1);
     if (rc) return rc;
     CUtensorMap tmap;
@@ -721,7 +721,7 @@ extern "C" int ctr_pnn_fwd(const float* e, const float* wlin, const float* wprod
     if (nsplit < 1) nsplit = 1;
     if (nsplit > NT) nsplit = NT;
     const long long items = (long long)n_btiles * nsplit;
-    const int grid = (int)(items < sms ? items : sms);
+    const int grid = capped_grid(items, sms);
     return with_const<0, 1>(method, [&](auto M) {
       return with_const<32, 64, 128>(s.WP, [&](auto WP) {
         constexpr int SB = WP == 32 ? 4 : WP == 64 ? 3 : 2;
@@ -733,11 +733,11 @@ extern "C" int ctr_pnn_fwd(const float* e, const float* wlin, const float* wprod
   }
   const size_t smem = sizeof(float) * (size_t)(SIMPLE_SPB * s.WX + s.FK + s.K);
   CTR_UNSUPPORTED(smem > SMEM_CAP, "ctr_pnn_fwd: F*K=%lld too large for the CUDA-core path", (long long)s.FK);
-  rc = launch("ctr_pnn_fwd(prep)", pnn_prep_kernel, grid_for((size_t)s.WX * N, 4096), 256, 0, st, wlin, wprod, bias, ws,
+  rc = launch("ctr_pnn_fwd(prep)", pnn_prep_kernel, capped_grid(((size_t)s.WX * N + 255) / 256, 4096), 256, 0, st, wlin, wprod, bias, ws,
               (int)F, (int)K, (int)N, method, (int)s.WX, (int)s.WX, (int)N, 1, 0);
   if (rc) return rc;
   const int64_t groups = (B + SIMPLE_SPB - 1) / SIMPLE_SPB;
-  const int grid = (int)(groups < (int64_t)sms * 4 ? groups : (int64_t)sms * 4);
+  const int grid = capped_grid(groups, (int64_t)sms * 4);
   return with_const<0, 1>(method, [&](auto M) {
     return launch("ctr_pnn_fwd(simple)", pnn_fwd_simple_kernel<M>, grid, 256, smem, st, e, ws, out, (int)B,
                   (int)F, (int)K, (int)N, (int)s.WX);
@@ -761,7 +761,7 @@ extern "C" int ctr_pnn_bwd(const float* e, const float* wlin, const float* wprod
   CTR_CUDA(cudaMemsetAsync(dwt, 0, sizeof(float) * (size_t)N * s.WX, st));
   if (B > 0 && s.tc) {
     CTR_REQUIRE(aligned16(out) && aligned16(g_out), "ctr_pnn_bwd: out and g_out must be 16-byte aligned");
-    rc = launch("ctr_pnn_bwd(prep)", pnn_prep_kernel, grid_for((size_t)s.WP * s.NPK, 2048), 256, 0, st, wlin, wprod,
+    rc = launch("ctr_pnn_bwd(prep)", pnn_prep_kernel, capped_grid(((size_t)s.WP * s.NPK + 255) / 256, 2048), 256, 0, st, wlin, wprod,
                 nullptr, ws, (int)F, (int)K, (int)N, method, (int)s.WX, s.WP, (int)s.NPK, 1, 1);
     if (rc) return rc;
     // ---- d_e: Wm (hi | lo) as [2 WP rows x NPK], one [WP x 32] swizzled box per K-block
@@ -786,7 +786,7 @@ extern "C" int ctr_pnn_bwd(const float* e, const float* wlin, const float* wprod
     if (sb > 4) sb = 4;
     rc = with_const<0, 1>(method, [&](auto M) {
       return with_const<32, 64, 128>(s.WP, [&](auto WP) {
-        if (int r = launch("ctr_pnn_bwd(dx, wgmma)", pnn_bwd_dx_tc_kernel<WP, 4, M>, tiles < sms ? tiles : sms, NTHREADS,
+        if (int r = launch("ctr_pnn_bwd(dx, wgmma)", pnn_bwd_dx_tc_kernel<WP, 4, M>, capped_grid(tiles, sms), NTHREADS,
                            dx_smem_bytes(WP, 4) + 1024, st, tw, e, out, g_out, d_e, (int)B, (int)F, (int)K, (int)N, (int)s.NPK))
           return r;
         return launch("ctr_pnn_bwd(dw, wgmma)", pnn_bwd_dw_tc_kernel<WP, M>, ngroups * nslices, NTHREADS, fixed + sb * stage,
@@ -798,10 +798,10 @@ extern "C" int ctr_pnn_bwd(const float* e, const float* wlin, const float* wprod
     const size_t smem_dx = sizeof(float) * (size_t)(N + s.FK + s.K + s.WX);
     const size_t smem_dw = sizeof(float) * (size_t)(s.FK + s.K + SIMPLE_PC);
     CTR_UNSUPPORTED(smem_dx > SMEM_CAP, "ctr_pnn_bwd: N + F*K too large for the CUDA-core path");
-    rc = launch("ctr_pnn_bwd(prep)", pnn_prep_kernel, grid_for((size_t)s.WX * N, 4096), 256, 0, st, wlin, wprod,
+    rc = launch("ctr_pnn_bwd(prep)", pnn_prep_kernel, capped_grid(((size_t)s.WX * N + 255) / 256, 4096), 256, 0, st, wlin, wprod,
                 nullptr, ws, (int)F, (int)K, (int)N, method, (int)s.WX, (int)N, (int)s.WX, 0, 0);
     if (rc) return rc;
-    const int gdx = (int)(B < (int64_t)sms * 4 ? B : (int64_t)sms * 4);
+    const int gdx = capped_grid(B, (int64_t)sms * 4);
     const int gx = (int)((s.WX + SIMPLE_PC - 1) / SIMPLE_PC), gy = (int)((N + 255) / 256);
     int gz = (int)((int64_t)sms * 4 / ((int64_t)gx * gy));
     if (gz < 1) gz = 1;
@@ -816,6 +816,6 @@ extern "C" int ctr_pnn_bwd(const float* e, const float* wlin, const float* wprod
     if (rc) return rc;
   }
   const size_t total = (size_t)s.FK * N + N + (method == 0 ? (size_t)N * F : (size_t)N * K * K);
-  return launch("ctr_pnn_bwd(fold)", pnn_fold_kernel, grid_for(total, 4096), 256, 0, st, dwt, wprod, d_wlin,
+  return launch("ctr_pnn_bwd(fold)", pnn_fold_kernel, capped_grid((total + 255) / 256, 4096), 256, 0, st, dwt, wprod, d_wlin,
                 d_wprod, d_bias, (int)F, (int)K, (int)N, method, (int)s.WX);
 }

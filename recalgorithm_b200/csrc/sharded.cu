@@ -259,15 +259,6 @@ rows_scatter_add_kernel(float4* __restrict__ dst, long long V, const long long* 
   }
 }
 
-template <typename K>
-static int resident_grid_sh(K kernel, int block, long long blocks_needed) {
-  int per_sm = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, block, 0) != cudaSuccess || per_sm < 1) per_sm = 1;
-  long long g = (long long)per_sm * sm_count();
-  if (g > blocks_needed) g = blocks_needed;
-  return (int)(g < 1 ? 1 : g);
-}
-
 static int check_g(const char* fn, int64_t G, int64_t rank) {
   CTR_REQUIRE(G >= 1 && G <= 8 && (G & (G - 1)) == 0, "%s: G=%lld must be a power of two <= 8", fn, (long long)G);
   CTR_REQUIRE(rank >= 0 && rank < G, "%s: rank %lld out of range", fn, (long long)rank);
@@ -301,28 +292,18 @@ static int fill_queues(const char* fn, PeerQueues& q, int64_t G, int64_t my_rank
 template <int LPR, int HOLD>
 static int launch_bwd_push(const float* tile, const float* d_tile, const float* d_fm2, const int32_t* plan, int64_t B, int64_t F,
                            const PeerQueues& q, float* row_grads, cudaStream_t st) {
-  auto k = embed_fm2_bwd_push_kernel<LPR, HOLD, false>;
-  const int grid = resident_grid_sh(k, 256, (B + 7) / 8);
-  k<<<grid, 256, 0, st>>>(reinterpret_cast<const float4*>(tile), reinterpret_cast<const float4*>(d_tile), d_fm2, plan, (int)B,
-                          (int)F, q, reinterpret_cast<float4*>(row_grads), nullptr, nullptr);
-  CTR_CHECK_LAUNCH("ctr_embed_fm2_bwd_push");
-  return CTR_OK;
+  return launch_resident("ctr_embed_fm2_bwd_push", embed_fm2_bwd_push_kernel<LPR, HOLD, false>, (B + 7) / 8, 256, 0, st,
+                         reinterpret_cast<const float4*>(tile), reinterpret_cast<const float4*>(d_tile), d_fm2, plan, (int)B, (int)F, q,
+                         reinterpret_cast<float4*>(row_grads), nullptr, nullptr);
 }
 
 template <int LPR, int HOLD>
 static int launch_lin_bwd_push(const float* tile, const float* wlin, const float* d_fm2, const float* d_lin, const int32_t* plan,
                                int64_t B, int64_t F, const PeerQueues& q, float* row_grads, float* d_wlin, cudaStream_t st) {
-  auto k = embed_fm2_bwd_push_kernel<LPR, HOLD, true>;
-  const size_t smem = sizeof(float4) * 2 * (size_t)F * LPR;
-  if (smem > 48 * 1024) CTR_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  int per_sm = 0;
-  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k, 256, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
-  long long grid = (long long)per_sm * sm_count();
-  if (grid > (B + 7) / 8) grid = (B + 7) / 8;
-  k<<<(int)grid, 256, smem, st>>>(reinterpret_cast<const float4*>(tile), reinterpret_cast<const float4*>(wlin), d_fm2, plan, (int)B,
-                                  (int)F, q, reinterpret_cast<float4*>(row_grads), d_lin, reinterpret_cast<float4*>(d_wlin));
-  CTR_CHECK_LAUNCH("ctr_embed_fm2_lin_bwd_push");
-  return CTR_OK;
+  return launch_resident("ctr_embed_fm2_lin_bwd_push", embed_fm2_bwd_push_kernel<LPR, HOLD, true>, (B + 7) / 8, 256,
+                         sizeof(float4) * 2 * (size_t)F * LPR, st, reinterpret_cast<const float4*>(tile),
+                         reinterpret_cast<const float4*>(wlin), d_fm2, plan, (int)B, (int)F, q, reinterpret_cast<float4*>(row_grads),
+                         d_lin, reinterpret_cast<float4*>(d_wlin));
 }
 
 template <int LPR>
@@ -364,17 +345,13 @@ extern "C" int ctr_sharded_plan(const int64_t* field_row_offset, const void* ids
   const long long n = (long long)B * F;
   const long long chunks = (n + PLAN_CHUNK - 1) / PLAN_CHUNK;
   // B == 0 still runs one CTA: it publishes the zero counts
-  const int grid = (int)(chunks < 1 ? 1 : (chunks < (long long)sm_count() * 4 ? chunks : (long long)sm_count() * 4));
-  if (ids_are_int32)
-    sharded_plan_kernel<int><<<grid, PLAN_THREADS, 0, st>>>(reinterpret_cast<const long long*>(field_row_offset),
-                                                            reinterpret_cast<const int*>(ids), n, (int)F, q,
-                                                            reinterpret_cast<unsigned long long*>(counters), overflow, plan);
-  else
-    sharded_plan_kernel<long long><<<grid, PLAN_THREADS, 0, st>>>(reinterpret_cast<const long long*>(field_row_offset),
-                                                                  reinterpret_cast<const long long*>(ids), n, (int)F, q,
-                                                                  reinterpret_cast<unsigned long long*>(counters), overflow, plan);
-  CTR_CHECK_LAUNCH("ctr_sharded_plan");
-  return CTR_OK;
+  const int grid = capped_grid(chunks < 1 ? 1 : chunks, (long long)sm_count() * 4);
+  auto go = [&](auto k, auto typed_ids) {
+    return launch("ctr_sharded_plan", k, grid, PLAN_THREADS, 0, st, reinterpret_cast<const long long*>(field_row_offset), typed_ids, n,
+                  (int)F, q, reinterpret_cast<unsigned long long*>(counters), overflow, plan);
+  };
+  return ids_are_int32 ? go(sharded_plan_kernel<int>, static_cast<const int*>(ids))
+                       : go(sharded_plan_kernel<long long>, static_cast<const long long*>(ids));
 }
 
 extern "C" int ctr_embed_fm2_bwd_push(const float* tile, const float* d_tile, const float* d_fm2, const int32_t* plan, int64_t B,
@@ -390,14 +367,7 @@ extern "C" int ctr_embed_fm2_bwd_push(const float* tile, const float* d_tile, co
               "ctr_embed_fm2_bwd_push: tile, d_tile and row_grads must be 16-byte aligned");
   if (B == 0) return CTR_OK;
   cudaStream_t st = as_stream(stream);
-  switch (D / 4) {
-    case 1: return dispatch_bwd_push<1>(tile, d_tile, d_fm2, plan, B, F, q, row_grads, st);
-    case 2: return dispatch_bwd_push<2>(tile, d_tile, d_fm2, plan, B, F, q, row_grads, st);
-    case 4: return dispatch_bwd_push<4>(tile, d_tile, d_fm2, plan, B, F, q, row_grads, st);
-    case 8: return dispatch_bwd_push<8>(tile, d_tile, d_fm2, plan, B, F, q, row_grads, st);
-    case 16: return dispatch_bwd_push<16>(tile, d_tile, d_fm2, plan, B, F, q, row_grads, st);
-    default: return dispatch_bwd_push<32>(tile, d_tile, d_fm2, plan, B, F, q, row_grads, st);
-  }
+  return with_lpr(D, [&](auto LPR) { return dispatch_bwd_push<LPR>(tile, d_tile, d_fm2, plan, B, F, q, row_grads, st); });
 }
 
 extern "C" int ctr_embed_fm2_lin_bwd_push(const float* tile, const float* wlin, const float* d_fm2, const float* d_lin,
@@ -415,14 +385,9 @@ extern "C" int ctr_embed_fm2_lin_bwd_push(const float* tile, const float* wlin, 
   cudaStream_t st = as_stream(stream);
   CTR_CUDA(cudaMemsetAsync(d_wlin, 0, sizeof(float) * F * D, st));
   if (B == 0) return CTR_OK;
-  switch (D / 4) {
-    case 1: return dispatch_lin_bwd_push<1>(tile, wlin, d_fm2, d_lin, plan, B, F, q, row_grads, d_wlin, st);
-    case 2: return dispatch_lin_bwd_push<2>(tile, wlin, d_fm2, d_lin, plan, B, F, q, row_grads, d_wlin, st);
-    case 4: return dispatch_lin_bwd_push<4>(tile, wlin, d_fm2, d_lin, plan, B, F, q, row_grads, d_wlin, st);
-    case 8: return dispatch_lin_bwd_push<8>(tile, wlin, d_fm2, d_lin, plan, B, F, q, row_grads, d_wlin, st);
-    case 16: return dispatch_lin_bwd_push<16>(tile, wlin, d_fm2, d_lin, plan, B, F, q, row_grads, d_wlin, st);
-    default: return dispatch_lin_bwd_push<32>(tile, wlin, d_fm2, d_lin, plan, B, F, q, row_grads, d_wlin, st);
-  }
+  return with_lpr(D, [&](auto LPR) {
+    return dispatch_lin_bwd_push<LPR>(tile, wlin, d_fm2, d_lin, plan, B, F, q, row_grads, d_wlin, st);
+  });
 }
 
 extern "C" int ctr_sharded_grad_push(const float* row_grads, const int32_t* plan, int64_t B, int64_t F, int64_t D, int64_t G,
@@ -437,18 +402,11 @@ extern "C" int ctr_sharded_grad_push(const float* row_grads, const int32_t* plan
   if (B == 0) return CTR_OK;
   cudaStream_t st = as_stream(stream);
   const long long n_rows = (long long)B * F, total = n_rows * (D / 4);
-  const int grid = (int)((total + 255) / 256 < (long long)sm_count() * 8 ? (total + 255) / 256 : (long long)sm_count() * 8);
-  auto* rg = reinterpret_cast<const float4*>(row_grads);
-  switch (D / 4) {
-    case 1: sharded_push_rows_kernel<1><<<grid, 256, 0, st>>>(rg, plan, n_rows, q); break;
-    case 2: sharded_push_rows_kernel<2><<<grid, 256, 0, st>>>(rg, plan, n_rows, q); break;
-    case 4: sharded_push_rows_kernel<4><<<grid, 256, 0, st>>>(rg, plan, n_rows, q); break;
-    case 8: sharded_push_rows_kernel<8><<<grid, 256, 0, st>>>(rg, plan, n_rows, q); break;
-    case 16: sharded_push_rows_kernel<16><<<grid, 256, 0, st>>>(rg, plan, n_rows, q); break;
-    default: sharded_push_rows_kernel<32><<<grid, 256, 0, st>>>(rg, plan, n_rows, q); break;
-  }
-  CTR_CHECK_LAUNCH("ctr_sharded_grad_push");
-  return CTR_OK;
+  const int grid = capped_grid((total + 255) / 256, (long long)sm_count() * 8);
+  return with_lpr(D, [&](auto LPR) {
+    return launch("ctr_sharded_grad_push", sharded_push_rows_kernel<LPR>, grid, 256, 0, st, reinterpret_cast<const float4*>(row_grads),
+                  plan, n_rows, q);
+  });
 }
 
 extern "C" int ctr_rows_scatter_add(float* dst, int64_t V, int64_t D, const int64_t* rows, const float* vals,
@@ -460,19 +418,10 @@ extern "C" int ctr_rows_scatter_add(float* dst, int64_t V, int64_t D, const int6
   if (max_n == 0) return CTR_OK;
   cudaStream_t st = as_stream(stream);
   const long long total = (long long)max_n * (D / 4);
-  const int grid = (int)((total + 255) / 256 < (long long)sm_count() * 16 ? (total + 255) / 256 : (long long)sm_count() * 16);
-  auto* d4 = reinterpret_cast<float4*>(dst);
-  auto* r = reinterpret_cast<const long long*>(rows);
-  auto* v4 = reinterpret_cast<const float4*>(vals);
-  auto* cn = reinterpret_cast<const long long*>(count);
-  switch (D / 4) {
-    case 1: rows_scatter_add_kernel<1><<<grid, 256, 0, st>>>(d4, V, r, v4, cn, max_n); break;
-    case 2: rows_scatter_add_kernel<2><<<grid, 256, 0, st>>>(d4, V, r, v4, cn, max_n); break;
-    case 4: rows_scatter_add_kernel<4><<<grid, 256, 0, st>>>(d4, V, r, v4, cn, max_n); break;
-    case 8: rows_scatter_add_kernel<8><<<grid, 256, 0, st>>>(d4, V, r, v4, cn, max_n); break;
-    case 16: rows_scatter_add_kernel<16><<<grid, 256, 0, st>>>(d4, V, r, v4, cn, max_n); break;
-    default: rows_scatter_add_kernel<32><<<grid, 256, 0, st>>>(d4, V, r, v4, cn, max_n); break;
-  }
-  CTR_CHECK_LAUNCH("ctr_rows_scatter_add");
-  return CTR_OK;
+  const int grid = capped_grid((total + 255) / 256, (long long)sm_count() * 16);
+  return with_lpr(D, [&](auto LPR) {
+    return launch("ctr_rows_scatter_add", rows_scatter_add_kernel<LPR>, grid, 256, 0, st, reinterpret_cast<float4*>(dst), V,
+                  reinterpret_cast<const long long*>(rows), reinterpret_cast<const float4*>(vals),
+                  reinterpret_cast<const long long*>(count), max_n);
+  });
 }

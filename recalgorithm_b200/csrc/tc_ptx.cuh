@@ -1,10 +1,8 @@
 // wgmma / TMA / mbarrier PTX wrappers shared by the tensor-core kernels (sm_90a), the pipeline mechanics built on them
 // (shared-memory alignment, the mbarrier ring, the producer / consumer role split, the 3xTF32 k-step, accumulation chains)
-// and the host side of a launch (tensor-map encoding, shared-memory attribute, compile-time shape dispatch).
+// and the host side of a tensor-core launch (workspace check, tensor-map encoding).
 #pragma once
 #include <cuda.h>
-
-#include <type_traits>
 
 #include "ctr_common.cuh"
 
@@ -245,11 +243,6 @@ __device__ __forceinline__ bool producer_role(int warp, int lane, Producer&& pro
 static inline int64_t pad_to(int64_t v, int64_t q) { return (v + q - 1) / q * q; }
 // wgmma N (or K) class of a width v <= 128: 32, 64 or 128
 static inline int pad3(int64_t v) { return v <= 32 ? 32 : v <= 64 ? 64 : 128; }
-// CTAs of 256 threads over `total` elements, at most `cap`
-static inline int grid_for(size_t total, int cap) {
-  return (int)((total + 255) / 256 < (size_t)cap ? (total + 255) / 256 : (size_t)cap);
-}
-
 // The caller's workspace: at least `need` bytes (size_fn tells how many), 128-byte aligned.
 static inline int check_workspace(const char* fn, const char* size_fn, const void* ws, int64_t bytes, int64_t need) {
   CTR_REQUIRE(ws != nullptr && bytes >= need, "%s: workspace of %lld bytes required (%s), got %lld", fn, (long long)need,
@@ -285,29 +278,6 @@ static inline int encode_tmap(const char* fn, CUtensorMap* map, int rank, const 
     return CTR_ERR_CUDA;
   }
   return CTR_OK;
-}
-
-// Launches k with `smem` bytes of dynamic shared memory (raising the kernel's limit past the default 48 KB when needed)
-// and checks the launch; `what` names it in the error message.
-template <class... P, class... A>
-int launch(const char* what, void (*k)(P...), dim3 grid, int block, size_t smem, cudaStream_t st, const A&... args) {
-  if (smem > 48 * 1024) CTR_CUDA(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-  k<<<grid, block, smem, st>>>(args...);
-  CTR_CHECK_LAUNCH(what);
-  return CTR_OK;
-}
-
-// Compile-time dispatch: returns f(std::integral_constant<int, V>{}) for the V of Vs equal to v (the kernels take their
-// shape class or method as a template argument).
-template <int... Vs, class F>
-int with_const(int v, F&& f) {
-  int rc = CTR_OK;
-  const bool hit = ((v == Vs && ((rc = f(std::integral_constant<int, Vs>{})), true)) || ...);
-  if (!hit) {
-    set_error("no kernel instantiation for %d", v);
-    return CTR_ERR_INVALID_ARG;
-  }
-  return rc;
 }
 
 }  // namespace tc

@@ -118,7 +118,11 @@ def test_backward_fused_with_adam_equals_unfused(lazy, B, F, D, rows):
     ctr_embed_fm2_bwd + ctr_adam_indexed_slices and the float64 oracle, three steps, duplicates / OOV / out-of-range ids."""
     from recalgorithm_b200 import autograd, optim
     rng = np.random.default_rng(B + F + D + int(lazy))
-    tf = autograd.EmbeddingTables([rows] * F, D, device="cuda")
+    # seeded weights as well as ids and gradients: a summed duplicate gradient within ~1e-6 of zero (a few in 10^3 draws
+    # of the (300, 40, 32, 1000) shape) makes m / (sqrt(v) + eps) ill-conditioned, and the float32 summation order of the
+    # duplicates, which the atomics leave open, then decides whether the weight meets the 2e-6 bar
+    tf = autograd.EmbeddingTables([rows] * F, D, device="cuda",
+                                  generator=torch.Generator(device="cuda").manual_seed(B + F + D + int(lazy)))
     tu = autograd.EmbeddingTables([rows] * F, D, device="cuda", init=None)
     tu.weight.copy_(tf.weight)
     of = optim.TableAdam(tf, lr=0.01, lazy=lazy, fused_backward=True)

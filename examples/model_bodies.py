@@ -123,3 +123,20 @@ def pnn_logit(fields_embeddings, num_fields: int, embedding_dim: int, output_dim
         for name in ("linear_part/linear_w", prod):
             reg = reg + weight_regularizer * 0.5 * store.vars[store.full_name(name)].pow(2).sum()
     return logit, reg
+
+
+def dien_logit(dense_input, category_input, target_input, sequnence_input, sequnence_length, gru_output_units=8,
+               custom_gru_type: str = "AGRU", hidden_units=(64, 32)):
+    """DIEN/dien.py:179-254 (the auxiliary loss :261-300, Dice / PReLU / batch-norm of the fcn tail left out, as for DIN).
+    Returns (logit, attention_scores (B, T, 1))."""
+    with L.variable_scope("seq_encoder"):                                                 # :199-229, one kernel each way
+        final_state, attention_scores = L.dien_interest_evolution(sequnence_input, sequnence_length, target_input,
+                                                                  gru_output_units, custom_gru_type=custom_gru_type,
+                                                                  return_attention_scores=True)
+        concat_all = torch.cat([dense_input, category_input, target_input, final_state], dim=-1)   # :237
+        with L.variable_scope("fcn"):                                                     # :240-254 (TF names dense, dense_1, ...)
+            net = concat_all
+            for i, unit in enumerate(hidden_units):
+                net = dense(net, unit, name=f"dense_{i}" if i else "dense")
+            logit = dense(net, 1, name=f"dense_{len(hidden_units)}" if hidden_units else "dense")
+    return logit, attention_scores

@@ -312,6 +312,30 @@ int ctr_din_attention_bwd(const float* query, const float* keys, const int64_t* 
                           int64_t B, int64_t T, int64_t H, int is_softmax,
                           float* d_query, float* d_keys, float* d_params, int32_t* sched_scratch, void* stream);
 
+/* ---- Row DIEN: interest extractor, attention and interest evolution ----------------------------------------
+ * Replaces the seq_encoder block of dien_model_fn (DIEN/dien.py:198-229) with the cells of DIEN/custom_grucell.py:19-167 and
+ * the loop of DIEN/rnn.py:443-798 (_rnn_step with skip_conditionals, :143-216):
+ *   h_t  = GRUCell(nh) over seq_input (B,T,na) from a zero state, every position (dien.py:202-204);
+ *   a    = softmax_t(h_t . (W_att e)), scores at t >= seq_length replaced by -2^32 + 1 (dien.py:206-218), e = target_input (B,na);
+ *   s    = AGRU (cell_type 0, dien.py:223: any custom_gru_type other than "AUGRU") or AUGRU (cell_type 1) over h with the
+ *          weights a, state copied through for t >= seq_length (dien.py:225-229);  final_state (B,nh) = s after step len-1
+ *          (zero for len <= 0; len > T acts as T).  att_scores (B,T) = a, or NULL.
+ * params: the nine variables packed in this order (floats):
+ *   rnn/gru_cell/gates/kernel (na+nh, 2nh) | rnn/gru_cell/gates/bias (2nh) | rnn/gru_cell/candidate/kernel (na+nh, nh) |
+ *   rnn/gru_cell/candidate/bias (nh) | attention_project_matrix (nh, na) | rnn/gates/kernel (2nh, 2nh) | rnn/gates/bias (2nh) |
+ *   rnn/candidate/kernel (2nh, nh) | rnn/candidate/bias (nh)       (kernels: input rows first, then state rows).
+ * workspace: ctr_dien_workspace_bytes() bytes; the forward keeps the states and weights the backward reads there, so the pair
+ * must share one workspace.  The backward overwrites d_seq_input (B,T,na; exactly 0 at t >= len), d_target_input (B,na) and
+ * d_params (packed like params; for AGRU the u half of rnn/gates/kernel and rnn/gates/bias gets exactly 0).
+ * na <= 64, nh <= 64, T <= 128 (CTR_ERR_UNSUPPORTED otherwise). */
+int ctr_dien_workspace_bytes(int64_t B, int64_t T, int64_t na, int64_t nh, int64_t* bytes);
+int ctr_dien_fwd(const float* seq_input, const int64_t* seq_length, const float* target_input, const float* params, int64_t B,
+                 int64_t T, int64_t na, int64_t nh, int cell_type, float* final_state, float* att_scores, void* workspace,
+                 int64_t workspace_bytes, void* stream);
+int ctr_dien_bwd(const float* seq_input, const int64_t* seq_length, const float* target_input, const float* params,
+                 const float* g_final_state, int64_t B, int64_t T, int64_t na, int64_t nh, int cell_type, float* d_seq_input,
+                 float* d_target_input, float* d_params, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ---- Rows SENET / BILINEAR: FiBiNET ---------------------------------------------------------------------
  * senet(input, embedding_dim, reduction_ratio) (FiBiNET/senet.py:26-34): x (B,F,K); w1 (F,r); w2 (r,F). */
 int ctr_senet_fwd(const float* x, const float* w1, const float* w2, int64_t B, int64_t F, int64_t K, int64_t r,

@@ -410,3 +410,29 @@ class _PNN(torch.autograd.Function):
 def pnn(e: torch.Tensor, wlin: torch.Tensor, wprod: torch.Tensor, bias: torch.Tensor, method: int) -> torch.Tensor:
     """PNN product layer: (B,F,K) field embeddings -> relu(lz + lp + bias) (B,N); method 0 = IPNN, 1 = OPNN."""
     return _PNN.apply(e, wlin, wprod, bias, method)
+
+
+class _DIEN(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, seq, seq_len, target, nh, cell, *params):
+        na = seq.shape[-1]
+        packed = ops.dien_pack_params(params, na, nh)
+        seq, target = seq.contiguous(), target.contiguous()
+        final, scores, ws = ops.dien_fwd(seq, seq_len, target, packed, nh, cell)
+        ctx.save_for_backward(seq, seq_len, target, packed, ws)     # ws: the forward's states and attention weights
+        ctx.cfg = (nh, cell)
+        ctx.mark_non_differentiable(scores)
+        return final, scores
+
+    @staticmethod
+    def backward(ctx, g, _g_scores):
+        seq, seq_len, target, packed, ws = ctx.saved_tensors
+        nh, cell = ctx.cfg
+        d_seq, d_tgt, d_p = ops.dien_bwd(seq, seq_len, target, packed, g.contiguous(), nh, cell, ws)
+        return (d_seq, None, d_tgt, None, None) + tuple(ops.dien_unpack_params(d_p, seq.shape[-1], nh))
+
+
+def dien(seq, seq_len, target, params, nh: int, cell: int):
+    """DIEN seq_encoder (DIEN/dien.py:198-229): (final_state (B,nh), attention scores (B,T), forward only); params in
+    ops.DIEN_PARAM_ORDER; cell 0 = AGRU, 1 = AUGRU."""
+    return _DIEN.apply(seq, seq_len, target, nh, cell, *params)

@@ -271,6 +271,42 @@ def pnn_product_layer(fields_embeddings: torch.Tensor, num_fields: int, embeddin
     return autograd.pnn(e, linear_w, wprod, bias, method)
 
 
+# --------------------------------------------------------------------------------------------------- DIEN
+def dien_interest_evolution(sequnence_input: torch.Tensor, sequnence_length: torch.Tensor, target_input: torch.Tensor,
+                            gru_output_units, custom_gru_type: str = "AGRU", return_attention_scores: bool = False):
+    """The seq_encoder block of DIEN/dien.py:198-229 in one kernel each way: the GRU interest extractor over every position,
+    the attention ``softmax_t(h_t . (W e_a))`` with positions t >= length masked, and the AGRU / AUGRU interest evolution over
+    the first ``length`` positions.  Returns ``final_state`` (B, nh), and also the attention scores (B, T, 1) (forward only,
+    what the reference logs) when ``return_attention_scores``.
+
+    Creates, in the caller's scope (``seq_encoder`` in the reference), the variables TF gives them:
+    ``rnn/gru_cell/{gates,candidate}/{kernel,bias}`` (tf.nn.rnn_cell.GRUCell: gate bias ones, candidate bias zeros),
+    ``attention_project_matrix`` (nh, na), and the custom cell's ``rnn/{gates,candidate}/{kernel,bias}`` (gate bias ones,
+    custom_grucell.py:66-68).  Kernels are glorot-uniform.  ``custom_gru_type == "AUGRU"`` selects AUGRU; ANY other value
+    selects AGRU (dien.py:220-223).  ``gru_output_units`` may arrive as a string."""
+    nh = int(gru_output_units)
+    na = int(sequnence_input.shape[-1])
+    cell = 1 if custom_gru_type == "AUGRU" else 0
+    ones, zeros = (lambda s: torch.ones(s)), (lambda s: torch.zeros(s))
+    with variable_scope("rnn"):
+        with variable_scope("gru_cell"):
+            with variable_scope("gates"):
+                gk = get_variable("kernel", (na + nh, 2 * nh)); gb = get_variable("bias", (2 * nh,), initializer=ones)
+            with variable_scope("candidate"):
+                ck = get_variable("kernel", (na + nh, nh)); cb = get_variable("bias", (nh,), initializer=zeros)
+    att = get_variable("attention_project_matrix", (nh, na))
+    with variable_scope("rnn"):
+        with variable_scope("gates"):
+            egk = get_variable("kernel", (2 * nh, 2 * nh)); egb = get_variable("bias", (2 * nh,), initializer=ones)
+        with variable_scope("candidate"):
+            eck = get_variable("kernel", (2 * nh, nh)); ecb = get_variable("bias", (nh,), initializer=zeros)
+    final_state, scores = autograd.dien(sequnence_input, sequnence_length.to(torch.int64), target_input,
+                                        (gk, gb, ck, cb, att, egk, egb, eck, ecb), nh, cell)
+    if return_attention_scores:
+        return final_state, scores.unsqueeze(-1)
+    return final_state
+
+
 # --------------------------------------------------------------------------------------------------- DIN loss-side term
 def mini_batch_aware_regularization(embedding_tensors, l2_lambda: float) -> torch.Tensor:
     """DIN/din.py:254-257 (SURVEY parity note 7): ``l2_lambda * tf.nn.l2_loss(concat(tensors, -1)) / batch`` -- an L2 on the

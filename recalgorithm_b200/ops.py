@@ -6,6 +6,7 @@ into libctr_b200.so.  Functions validate devices/dtypes and raise instead of fal
 from __future__ import annotations
 
 import ctypes
+import math
 from typing import Optional, Tuple
 
 import torch
@@ -644,3 +645,73 @@ def pnn_bwd(e, wlin, wprod, out, g_out, method: int):
     _lib.check(_lib.lib().ctr_pnn_bwd(_ptr(e), _ptr(wlin), _ptr(wprod), _ptr(out), _ptr(g_out), B, F, K, N, method, _ptr(d_e),
                                       _ptr(d_wlin), _ptr(d_wprod), _ptr(d_bias), _ptr(ws), nbytes, _stream()))
     return d_e, d_wlin, d_wprod, d_bias
+
+
+# ------------------------------------------------------------------------------------ DIEN interest extractor + evolution
+DIEN_CELLS = {"AGRU": 0, "AUGRU": 1}
+# the nine variables in the packed order of include/ctr_b200.h (names relative to the caller's seq_encoder scope)
+DIEN_PARAM_ORDER = ("rnn/gru_cell/gates/kernel", "rnn/gru_cell/gates/bias", "rnn/gru_cell/candidate/kernel",
+                    "rnn/gru_cell/candidate/bias", "attention_project_matrix", "rnn/gates/kernel", "rnn/gates/bias",
+                    "rnn/candidate/kernel", "rnn/candidate/bias")
+
+
+def dien_param_shapes(na: int, nh: int):
+    """Shapes of DIEN_PARAM_ORDER for input width na and gru_output_units nh."""
+    return ((na + nh, 2 * nh), (2 * nh,), (na + nh, nh), (nh,), (nh, na), (2 * nh, 2 * nh), (2 * nh,), (2 * nh, nh), (nh,))
+
+
+def dien_pack_params(params, na: int, nh: int) -> torch.Tensor:
+    """The nine variables (DIEN_PARAM_ORDER) -> one packed fp32 buffer."""
+    for p, s, n in zip(params, dien_param_shapes(na, nh), DIEN_PARAM_ORDER):
+        if tuple(p.shape) != s:
+            raise ValueError(f"{n}: expected shape {s}, got {tuple(p.shape)}")
+    return torch.cat([p.reshape(-1) for p in params]).contiguous()
+
+
+def dien_unpack_params(packed: torch.Tensor, na: int, nh: int):
+    out, o = [], 0
+    for s in dien_param_shapes(na, nh):
+        n = 1
+        for d in s:
+            n *= d
+        out.append(packed[o:o + n].view(s))
+        o += n
+    return out
+
+
+def _dien_args(seq, seq_len, target, packed, nh, cell):
+    if cell not in (0, 1):
+        raise ValueError(f"cell must be 0 (AGRU) or 1 (AUGRU), got {cell!r}")
+    B, T, na = seq.shape
+    _chk(seq, F32, "sequnence_input"); _chk(seq_len, I64, "sequnence_length", (B,)); _chk(target, F32, "target_input", (B, na))
+    _chk(packed, F32, "params", (sum(math.prod(s) for s in dien_param_shapes(na, nh)),))
+    return B, T, na
+
+
+def dien_workspace(B: int, T: int, na: int, nh: int, device) -> torch.Tensor:
+    """The caller-owned workspace of one forward / backward pair (the forward's states and attention weights live there)."""
+    nbytes = ctypes.c_int64(0)
+    _lib.check(_lib.lib().ctr_dien_workspace_bytes(B, T, na, nh, ctypes.byref(nbytes)))
+    return torch.empty((int(nbytes.value),), dtype=torch.uint8, device=device)
+
+
+def dien_fwd(seq, seq_len, target, packed, nh: int, cell: int):
+    """DIEN/dien.py:198-229: (final_state (B,nh), attention scores (B,T), workspace for dien_bwd)."""
+    B, T, na = _dien_args(seq, seq_len, target, packed, nh, cell)
+    final = torch.empty((B, nh), dtype=F32, device=seq.device)
+    scores = torch.empty((B, T), dtype=F32, device=seq.device)
+    ws = dien_workspace(B, T, na, nh, seq.device)
+    _lib.check(_lib.lib().ctr_dien_fwd(_ptr(seq), _ptr(seq_len), _ptr(target), _ptr(packed), B, T, na, nh, cell, _ptr(final),
+                                       _ptr(scores), _ptr(ws), ws.numel(), _stream()))
+    return final, scores, ws
+
+
+def dien_bwd(seq, seq_len, target, packed, g_final, nh: int, cell: int, ws):
+    """Gradients of dien_fwd given d final_state (B,nh) and the forward's workspace: (d_seq (B,T,na), d_target (B,na),
+    d_packed)."""
+    B, T, na = _dien_args(seq, seq_len, target, packed, nh, cell)
+    _chk(g_final, F32, "g_final_state", (B, nh))
+    d_seq, d_tgt, d_p = torch.empty_like(seq), torch.empty_like(target), torch.empty_like(packed)
+    _lib.check(_lib.lib().ctr_dien_bwd(_ptr(seq), _ptr(seq_len), _ptr(target), _ptr(packed), _ptr(g_final), B, T, na, nh, cell,
+                                       _ptr(d_seq), _ptr(d_tgt), _ptr(d_p), _ptr(ws), ws.numel(), _stream()))
+    return d_seq, d_tgt, d_p

@@ -4,7 +4,7 @@
 Each kernel is timed alone with CUDA events; an L2 flush (a 256 MB write) runs between timed iterations because these
 working sets are flushed from the 50 MB L2.  Prints one JSON line per measurement.
 
-    python tools/bench_layers.py [--iters 20] [--only cin,dcn,din,fibinet]     (also: pairwise, bst, adam, pnn)
+    python tools/bench_layers.py [--iters 20] [--only cin,dcn,din,fibinet]     (also: pairwise, bst, adam, pnn, dien)
 """
 import argparse
 import json
@@ -105,6 +105,103 @@ def pnn_rows(iters, flush, rn, hbm):
                 kg = ops.pnn_bwd(e, wlin, wprod, out, g, method)
                 gdiff = max(float((a - b).abs().max() / b.abs().max()) for a, b in zip(kg, grads))
                 m, bst = timeit(torch_bwd, iters, flush)
+                print(json.dumps({"kernel": f"torch_fp32_bwd_{tag}", "config": cfg, "ms_median": m, "ms_best": bst,
+                                  "max_rel_diff_vs_kernel": gdiff, "within_1e-5": gdiff <= 1e-5,
+                                  "note": "autograd of the same torch form (backward only), fp32, TF32 disabled"}), flush=True)
+    finally:
+        torch.backends.cuda.matmul.allow_tf32 = prev_tf32
+
+
+def card():
+    """Name and power limit of the GPU the rows are measured on, read in the same run."""
+    import subprocess
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                       capture_output=True, text=True)
+    return {"device": torch.cuda.get_device_name(0), "nvidia_smi": q.stdout.strip() or q.stderr.strip()}
+
+
+def dien_rows(iters, flush, hbm):
+    """DIEN seq_encoder (ctr_dien_fwd / ctr_dien_bwd) at T = 50, na = 16, nh = 8, lengths uniform in {0..50}, B = 4096 and
+    65 536, both cells, next to plain torch running the reference form (a Python loop over T, fp32, TF32 off, autograd
+    backward).  Floors: HBM bytes over 3.35 TB/s and FLOPs over the 67 TFLOP/s FP32 data-sheet rate of the H100 SXM (700 W).
+    The kernels are bound by the dependent chain of 2*T cell steps per sample, so each row also reports time / (2*T)."""
+    T, na, nh = 50, 16, 8
+    fp32_peak = 67.0
+    print(json.dumps({"dien_card": card()}), flush=True)
+
+    def torch_form(seq, L, tgt, params, cell):
+        gk, gb, ck, cb, W, egk, egb, eck, ecb = params
+
+        def gru(x, h, gk, gb, ck, cb):
+            v = torch.sigmoid(torch.cat([x, h], 1) @ gk + gb)
+            r, u = v[:, :nh], v[:, nh:]
+            return u, torch.tanh(torch.cat([x, r * h], 1) @ ck + cb)
+        h = seq.new_zeros(seq.shape[0], nh)
+        hs = []
+        for t in range(T):
+            u, c = gru(seq[:, t], h, gk, gb, ck, cb)
+            h = u * h + (1 - u) * c
+            hs.append(h)
+        H = torch.stack(hs, 1)
+        mask = torch.arange(T, device=seq.device)[None, :] < L[:, None]
+        att = torch.softmax(torch.where(mask, (H @ (tgt @ W.t())[:, :, None])[..., 0], -4294967296.0), dim=1)
+        s = seq.new_zeros(seq.shape[0], nh)
+        for t in range(T):
+            a = att[:, t, None]
+            u, c = gru(H[:, t], s, egk, egb, eck, ecb)
+            sn = ((1 - a) * u) * s + (1 - (1 - a) * u) * c if cell == 1 else (1 - a) * s + a * c
+            s = torch.where(mask[:, t, None], sn, s)
+        return s, att
+
+    prev_tf32 = torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cuda.matmul.allow_tf32 = False
+    gen = torch.Generator(device="cuda").manual_seed(50)
+    try:
+        for B in (4096, 65536):
+            L = torch.randint(0, T + 1, (B,), device="cuda", generator=gen)
+            seq = torch.randn((B, T, na), device="cuda", generator=gen) * 0.7
+            seq[torch.arange(T, device="cuda")[None, :] >= L[:, None]] = 0
+            tgt = torch.randn((B, na), device="cuda", generator=gen) * 0.7
+            g = torch.randn((B, nh), device="cuda", generator=gen)
+            params = [(torch.rand(s, device="cuda", generator=gen) * 2 - 1) * (0.5 if len(s) == 1 else (6.0 / sum(s)) ** 0.5)
+                      for s in ops.dien_param_shapes(na, nh)]
+            packed = ops.dien_pack_params(params, na, nh)
+            steps = int(L.sum())                                    # processed positions (each runs both cells)
+            flop_pos = 2 * (3 * nh * (na + nh) + 3 * nh * 2 * nh) + 2 * nh + 30 * nh   # projections + score + gates
+            fwd_flops, bwd_flops = steps * flop_pos, 3 * steps * flop_pos            # backward: recompute + two transposes
+            fwd_bytes = 4 * (steps * (na + 2 * nh) + B * (T + na + nh) + B * 2)
+            bwd_bytes = 4 * (B * T * na + steps * (na + 2 * nh + 1 + 2 * (nh + 1)) + B * (T + 2 * na + nh) + B * 2)
+            for cell, tag in ((0, "agru"), (1, "augru")):
+                cfg = {"cell": tag.upper(), "B": B, "T": T, "na": na, "nh": nh, "lengths": "uniform 0..50", "mean_len": steps / B}
+                fs, att, ws = ops.dien_fwd(seq, L, tgt, packed, nh, cell)
+                for kind, fn, flops, nbytes in (
+                        ("fwd", lambda: ops.dien_fwd(seq, L, tgt, packed, nh, cell), fwd_flops, fwd_bytes),
+                        ("bwd", lambda: ops.dien_bwd(seq, L, tgt, packed, g, nh, cell, ws), bwd_flops, bwd_bytes)):
+                    m, bst = timeit(fn, iters, flush)
+                    print(json.dumps({"kernel": f"dien_{kind}_{tag}", "config": cfg, "ms_median": m, "ms_best": bst,
+                                      "l2": "flushed between iterations", "us_per_dependent_step": m * 1e3 / (2 * T),
+                                      "hbm_floor_ms": nbytes / (hbm * 1e9) * 1e3, "fp32_floor_ms": flops / (fp32_peak * 1e12) * 1e3,
+                                      "algorithmic_bytes": nbytes, "flops": flops,
+                                      "note": "floors: algorithmic bytes / measured-or-datasheet HBM rate, FLOPs / 67 TFLOP/s FP32"}),
+                          flush=True)
+                ps = [p.clone().requires_grad_() for p in params]
+                xs = seq.clone().requires_grad_()
+                ts = tgt.clone().requires_grad_()
+                ref_s, ref_att = torch_form(xs, L, ts, ps, cell)
+                diff = max(float((ref_s.detach() - fs).abs().max() / ref_s.detach().abs().max()),
+                           float((ref_att.detach() - att).abs().max() / ref_att.detach().abs().max()))
+                m, bst = timeit(lambda: torch_form(seq, L, tgt, params, cell), max(3, iters // 4), flush)
+                print(json.dumps({"kernel": f"torch_fp32_fwd_{tag}", "config": cfg, "ms_median": m, "ms_best": bst,
+                                  "max_rel_diff_vs_kernel": diff, "within_1e-5": diff <= 1e-5,
+                                  "note": "reference form in torch (Python loop over T), fp32, TF32 disabled"}), flush=True)
+
+                def torch_bwd():
+                    return torch.autograd.grad(ref_s, [xs, ts] + ps, g, retain_graph=True)
+                grads = torch_bwd()
+                d_seq, d_tgt, d_p = ops.dien_bwd(seq, L, tgt, packed, g, nh, cell, ws)
+                kg = [d_seq, d_tgt] + list(ops.dien_unpack_params(d_p, na, nh))
+                gdiff = max(float((a - b).abs().max() / max(float(b.abs().max()), 1e-30)) for a, b in zip(kg, grads))
+                m, bst = timeit(torch_bwd, max(3, iters // 4), flush)
                 print(json.dumps({"kernel": f"torch_fp32_bwd_{tag}", "config": cfg, "ms_median": m, "ms_best": bst,
                                   "max_rel_diff_vs_kernel": gdiff, "within_1e-5": gdiff <= 1e-5,
                                   "note": "autograd of the same torch form (backward only), fp32, TF32 disabled"}), flush=True)
@@ -286,6 +383,8 @@ def main():
 
     if "pnn" in only:   # PNN product layer at the reference defaults (F = 8 fields, K = 8, output_dimension 1024); not in the default list
         pnn_rows(args.iters, flush, rn, hbm)
+    if "dien" in only:  # DIEN seq_encoder at the reference shape (na = 16, nh = 8) with config 4's T and lengths; not in the default list
+        dien_rows(args.iters, flush, hbm)
 
 
 if __name__ == "__main__" and "--configs" not in sys.argv:

@@ -140,3 +140,14 @@ def dien_logit(dense_input, category_input, target_input, sequnence_input, sequn
                 net = dense(net, unit, name=f"dense_{i}" if i else "dense")
             logit = dense(net, 1, name=f"dense_{len(hidden_units)}" if hidden_units else "dense")
     return logit, attention_scores
+
+
+def deepcrossing_logit(dense_input, category_input, residual_internal_dim=256, residual_network_num=2):
+    """DeepCrossing/deepcrossing.py:152-159: the residual units over concat_all in scope residual_module, then dense(net, 1)
+    outside it.  The reference's best result.md row is residual_internal_dim 256 with 2 units."""
+    concat_all = torch.cat([dense_input, category_input], dim=-1)                         # :152
+    with L.variable_scope("residual_module"):                                             # :154-157, one kernel each way per unit
+        net = concat_all
+        for i in range(residual_network_num):
+            net = L.residual_unit(net, residual_internal_dim, index=i)
+    return dense(net, 1)                                                                  # :159

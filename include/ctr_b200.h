@@ -292,6 +292,24 @@ int ctr_pnn_bwd(const float* e, const float* wlin, const float* wprod, const flo
                 int64_t F, int64_t K, int64_t N, int method, float* d_e, float* d_wlin, float* d_wprod, float* d_bias,
                 void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- DeepCrossing residual unit -------------------------------------------------------------------------
+ * Replaces residual_unit(input, internal_dim, index) (DeepCrossing/residual_unit.py:4-21, looped at
+ * DeepCrossing/deepcrossing.py:149-153):
+ *   out = relu(x + relu(x . w0 + b0) . w1 + b1)   x (B,d); w0 = dense_{index}_0/kernel (d,H), b0 (H);
+ *                                                  w1 = dense_{index}_1/kernel (H,d), b1 (d); out (B,d).
+ * fp32-class accuracy (3xTF32 on the tensor cores); the (B,H) hidden activation of the forward stays on chip.
+ * d <= 128 and 1 <= H <= 1024 (CTR_ERR_UNSUPPORTED otherwise); B = 0 launches nothing.
+ * workspace: 128-byte aligned, at least ctr_residual_unit_workspace_bytes(0, d, H) bytes for the forward (the prepped
+ * weights) and ctr_residual_unit_workspace_bytes(B, d, H) for the backward (also h and its gradient, (B,H) each).
+ * The backward takes the forward's out (its relu mask) and g_out (B,d), and overwrites d_x (B,d), d_w0 (d,H), d_b0 (H),
+ * d_w1 (H,d) and d_b1 (d) (zeros at B = 0).  b1 is not read by the backward. */
+int ctr_residual_unit_workspace_bytes(int64_t B, int64_t d, int64_t H, int64_t* bytes);
+int ctr_residual_unit_fwd(const float* x, const float* w0, const float* b0, const float* w1, const float* b1, int64_t B,
+                          int64_t d, int64_t H, float* out, void* workspace, int64_t workspace_bytes, void* stream);
+int ctr_residual_unit_bwd(const float* x, const float* w0, const float* b0, const float* w1, const float* b1,
+                          const float* out, const float* g_out, int64_t B, int64_t d, int64_t H, float* d_x, float* d_w0,
+                          float* d_b0, float* d_w1, float* d_b1, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ---- Row DIN-ATT: DIN attention unit -----------------------------------------------------------------
  * Replaces din_attention(query, keys, keys_length, is_softmax) (DIN/din_attention.py:17-43).
  * query (B,H); keys (B,T,H); keys_length int64 (B); dense layers f1_att (4H->64, relu), f2_att (64->32,

@@ -93,6 +93,9 @@ SIGNATURES = {
     "ctr_dien_workspace_bytes": (c_int, [_I, _I, _I, _I, POINTER(c_int64)]),
     "ctr_dien_fwd": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, c_int, _P, _P, _P, _I, _P]),
     "ctr_dien_bwd": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, c_int, _P, _P, _P, _P, _I, _P]),
+    "ctr_residual_unit_workspace_bytes": (c_int, [_I, _I, _I, POINTER(c_int64)]),
+    "ctr_residual_unit_fwd": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _I, _P]),
+    "ctr_residual_unit_bwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _I, _P]),
 }
 
 

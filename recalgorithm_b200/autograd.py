@@ -436,3 +436,21 @@ def dien(seq, seq_len, target, params, nh: int, cell: int):
     """DIEN seq_encoder (DIEN/dien.py:198-229): (final_state (B,nh), attention scores (B,T), forward only); params in
     ops.DIEN_PARAM_ORDER; cell 0 = AGRU, 1 = AUGRU."""
     return _DIEN.apply(seq, seq_len, target, nh, cell, *params)
+
+
+class _ResidualUnit(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, w0, b0, w1, b1):
+        x, w0, b0, w1, b1 = (t.contiguous() for t in (x, w0, b0, w1, b1))
+        out = ops.residual_unit_fwd(x, w0, b0, w1, b1)
+        ctx.save_for_backward(x, w0, b0, w1, b1, out)        # out carries the outer relu mask; h is recomputed from x
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        return ops.residual_unit_bwd(*ctx.saved_tensors, g.contiguous())
+
+
+def residual_unit(x: torch.Tensor, w0: torch.Tensor, b0: torch.Tensor, w1: torch.Tensor, b1: torch.Tensor) -> torch.Tensor:
+    """DeepCrossing residual unit: relu(x + relu(x . w0 + b0) . w1 + b1), (B,d) -> (B,d)."""
+    return _ResidualUnit.apply(x, w0, b0, w1, b1)

@@ -307,6 +307,26 @@ def dien_interest_evolution(sequnence_input: torch.Tensor, sequnence_length: tor
     return final_state
 
 
+# --------------------------------------------------------------------------------------------------- DeepCrossing
+def residual_unit(input: torch.Tensor, internal_dim=None, index=None) -> torch.Tensor:
+    """DeepCrossing residual unit -- same signature as DeepCrossing/residual_unit.py:4, one kernel each way:
+    ``relu(input + dense(relu(dense(input, internal_dim)), output_dim))`` with ``output_dim`` the input's last dimension.
+
+    Creates, in the caller's scope (``residual_module`` in the reference), the variables of the two ``tf.layers.dense``
+    calls: ``dense_{index}_0/kernel`` (d, internal_dim), ``dense_{index}_0/bias`` (internal_dim,), ``dense_{index}_1/kernel``
+    (internal_dim, d), ``dense_{index}_1/bias`` (d,).  Kernels are glorot-uniform and both biases start at zero.  As in the
+    reference, ``internal_dim`` goes through ``int()`` (a string width works, None raises) and ``index=None`` names the
+    variables ``dense_None_0`` / ``dense_None_1``."""
+    output_dim = int(input.shape[-1])
+    internal_dim = int(internal_dim)
+    zeros = lambda s: torch.zeros(s)
+    with variable_scope(f"dense_{index}_0"):
+        w0 = get_variable("kernel", (output_dim, internal_dim)); b0 = get_variable("bias", (internal_dim,), initializer=zeros)
+    with variable_scope(f"dense_{index}_1"):
+        w1 = get_variable("kernel", (internal_dim, output_dim)); b1 = get_variable("bias", (output_dim,), initializer=zeros)
+    return autograd.residual_unit(input, w0, b0, w1, b1)
+
+
 # --------------------------------------------------------------------------------------------------- DIN loss-side term
 def mini_batch_aware_regularization(embedding_tensors, l2_lambda: float) -> torch.Tensor:
     """DIN/din.py:254-257 (SURVEY parity note 7): ``l2_lambda * tf.nn.l2_loss(concat(tensors, -1)) / batch`` -- an L2 on the

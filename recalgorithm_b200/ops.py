@@ -715,3 +715,42 @@ def dien_bwd(seq, seq_len, target, packed, g_final, nh: int, cell: int, ws):
     _lib.check(_lib.lib().ctr_dien_bwd(_ptr(seq), _ptr(seq_len), _ptr(target), _ptr(packed), _ptr(g_final), B, T, na, nh, cell,
                                        _ptr(d_seq), _ptr(d_tgt), _ptr(d_p), _ptr(ws), ws.numel(), _stream()))
     return d_seq, d_tgt, d_p
+
+
+# ------------------------------------------------------------------------------------ DeepCrossing residual unit
+def residual_unit_workspace(B: int, d: int, H: int, device) -> torch.Tensor:
+    """Caller-owned workspace: the prepped weights (B = 0, what the forward needs) plus, for the backward, h and its gradient."""
+    nbytes = ctypes.c_int64(0)
+    _lib.check(_lib.lib().ctr_residual_unit_workspace_bytes(B, d, H, ctypes.byref(nbytes)))
+    return torch.empty((int(nbytes.value),), dtype=torch.uint8, device=device)
+
+
+def _residual_unit_args(x, w0, b0, w1, b1):
+    B, d = x.shape
+    H = w0.shape[1]
+    _chk(x, F32, "input"); _chk(w0, F32, "w0", (d, H)); _chk(b0, F32, "b0", (H,)); _chk(w1, F32, "w1", (H, d))
+    _chk(b1, F32, "b1", (d,))
+    return B, d, H
+
+
+def residual_unit_fwd(x, w0, b0, w1, b1) -> torch.Tensor:
+    """DeepCrossing/residual_unit.py:4-21: relu(x + relu(x . w0 + b0) . w1 + b1), x (B,d), w0 (d,H), w1 (H,d) -> (B,d)."""
+    B, d, H = _residual_unit_args(x, w0, b0, w1, b1)
+    out = torch.empty((B, d), dtype=F32, device=x.device)
+    ws = residual_unit_workspace(0, d, H, x.device)
+    _lib.check(_lib.lib().ctr_residual_unit_fwd(_ptr(x), _ptr(w0), _ptr(b0), _ptr(w1), _ptr(b1), B, d, H, _ptr(out), _ptr(ws),
+                                                ws.numel(), _stream()))
+    return out
+
+
+def residual_unit_bwd(x, w0, b0, w1, b1, out, g_out):
+    """Gradients of residual_unit_fwd given its output `out` (the relu mask) and g_out (B,d): (d_x, d_w0, d_b0, d_w1, d_b1).
+    The hidden activation is recomputed from x."""
+    B, d, H = _residual_unit_args(x, w0, b0, w1, b1)
+    _chk(out, F32, "out", (B, d)); _chk(g_out, F32, "g_out", (B, d))
+    d_x, d_w0, d_b0, d_w1, d_b1 = (torch.empty_like(t) for t in (x, w0, b0, w1, b1))
+    ws = residual_unit_workspace(B, d, H, x.device)
+    _lib.check(_lib.lib().ctr_residual_unit_bwd(_ptr(x), _ptr(w0), _ptr(b0), _ptr(w1), _ptr(b1), _ptr(out), _ptr(g_out), B, d,
+                                                H, _ptr(d_x), _ptr(d_w0), _ptr(d_b0), _ptr(d_w1), _ptr(d_b1), _ptr(ws),
+                                                ws.numel(), _stream()))
+    return d_x, d_w0, d_b0, d_w1, d_b1

@@ -4,7 +4,7 @@
 Each kernel is timed alone with CUDA events; an L2 flush (a 256 MB write) runs between timed iterations because these
 working sets are flushed from the 50 MB L2.  Prints one JSON line per measurement.
 
-    python tools/bench_layers.py [--iters 20] [--only cin,dcn,din,fibinet]     (also: pairwise, bst, adam, pnn, dien)
+    python tools/bench_layers.py [--iters 20] [--only cin,dcn,din,fibinet]     (also: pairwise, bst, adam, pnn, dien, deepcrossing)
 """
 import argparse
 import json
@@ -209,6 +209,57 @@ def dien_rows(iters, flush, hbm):
         torch.backends.cuda.matmul.allow_tf32 = prev_tf32
 
 
+def deepcrossing_rows(iters, flush, rn):
+    """DeepCrossing residual unit (ctr_residual_unit_fwd / _bwd) at the reference width d = 82, H = 128 and 256, B = 1024 (the
+    reference batch) and 65 536, next to plain torch running the same unit (fp32 matmul, TF32 disabled, autograd backward).
+    Floors from data-sheet rates of the H100 SXM (700 W), not measured: FLOPs over the 67 TFLOP/s FP32 rate, the executed
+    3xTF32 FLOPs (3 passes over DP = 96 inputs, the kernels' padded width) over the 495 TFLOP/s TF32 rate, and x + out
+    (forward) or x, out, g, d_x (backward) over 3.35 TB/s of HBM."""
+    d, DP = 82, 96
+    print(json.dumps({"deepcrossing_card": card()}), flush=True)
+
+    def torch_form(x, w0, b0, w1, b1):
+        return torch.relu(x + torch.relu(x @ w0 + b0) @ w1 + b1)
+
+    prev_tf32 = torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cuda.matmul.allow_tf32 = False
+    try:
+        for H in (128, 256):
+            lim = (6.0 / (d + H)) ** 0.5
+            w0, w1 = (torch.rand(d, H, device="cuda") * 2 - 1) * lim, (torch.rand(H, d, device="cuda") * 2 - 1) * lim
+            b0, b1 = rn(H, std=0.1), rn(d, std=0.1)
+            for B in (1024, 65536):
+                x, g = rn(B, d, std=0.7), rn(B, d)
+                cfg = {"B": B, "d": d, "H": H}
+                flops = {"fwd": 4.0 * B * d * H, "bwd": 10.0 * B * d * H}       # bwd: gh, dx, dW1, dW0 + the recomputed a
+                tc = {"fwd": 3 * 4.0 * B * DP * H, "bwd": 3 * 10.0 * B * DP * H}
+                hbm = {"fwd": 2 * B * d * 4, "bwd": 4 * B * d * 4}
+                out = ops.residual_unit_fwd(x, w0, b0, w1, b1)
+                grads = ops.residual_unit_bwd(x, w0, b0, w1, b1, out, g)
+                ps = [t.clone().requires_grad_() for t in (x, w0, b0, w1, b1)]
+                ref_out = torch_form(*ps)
+                ref_grads = torch.autograd.grad(ref_out, ps, g, retain_graph=True)
+                diff = {"fwd": float((ref_out.detach() - out).abs().max() / ref_out.detach().abs().max()),
+                        "bwd": max(float((a - b).abs().max() / b.abs().max()) for a, b in zip(grads, ref_grads))}
+                runs = {"fwd": (lambda: ops.residual_unit_fwd(x, w0, b0, w1, b1),
+                                lambda: torch_form(x, w0, b0, w1, b1)),
+                        "bwd": (lambda: ops.residual_unit_bwd(x, w0, b0, w1, b1, out, g),
+                                lambda: torch.autograd.grad(ref_out, ps, g, retain_graph=True))}
+                for way in ("fwd", "bwd"):
+                    m, bst = timeit(runs[way][0], iters, flush)
+                    tm, tbst = timeit(runs[way][1], iters, flush)
+                    print(json.dumps({
+                        "kernel": f"residual_unit_{way}", "config": cfg, "ms_median": m, "ms_best": bst,
+                        "torch_fp32_ms_median": tm, "torch_fp32_ms_best": tbst, "speedup_vs_torch": tm / m,
+                        "max_norm_rel_diff_vs_torch": diff[way], "l2": "flushed between iterations",
+                        "floor_fp32_us": flops[way] / 67e12 * 1e6, "floor_3xtf32_us": tc[way] / 495e12 * 1e6,
+                        "floor_hbm_us": hbm[way] / 3.35e12 * 1e6,
+                        "note": "floors are data-sheet rates (H100 SXM, 700 W), not measured; torch: same unit, fp32, TF32 off"}),
+                        flush=True)
+    finally:
+        torch.backends.cuda.matmul.allow_tf32 = prev_tf32
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=20)
@@ -385,6 +436,8 @@ def main():
         pnn_rows(args.iters, flush, rn, hbm)
     if "dien" in only:  # DIEN seq_encoder at the reference shape (na = 16, nh = 8) with config 4's T and lengths; not in the default list
         dien_rows(args.iters, flush, hbm)
+    if "deepcrossing" in only:  # DeepCrossing residual unit at the reference width (d = 82) and both result.md H; not in the default list
+        deepcrossing_rows(args.iters, flush, rn)
 
 
 if __name__ == "__main__" and "--configs" not in sys.argv:

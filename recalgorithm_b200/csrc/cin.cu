@@ -250,10 +250,7 @@ extern "C" int ctr_cin_fwd(const float* x0, const float* xk, const float* filter
               wt, (int)m, (int)hk, (int)H, NP);
   if (rc) return rc;
   CUtensorMap tmap;
-  const cuuint64_t gdim[2] = {(cuuint64_t)KP, (cuuint64_t)(2 * NP)};
-  const cuuint64_t gstride[1] = {(cuuint64_t)KP * sizeof(float)};
-  const cuuint32_t box[2] = {(cuuint32_t)KB, (cuuint32_t)NP};
-  rc = encode_tmap("ctr_cin_fwd", &tmap, 2, wt, gdim, gstride, box, CU_TENSOR_MAP_SWIZZLE_128B);
+  rc = encode_2d("ctr_cin_fwd", &tmap, wt, KP, 2 * NP, KB, NP, CU_TENSOR_MAP_SWIZZLE_128B);
   if (rc) return rc;
   int logD = 0;
   while ((1 << logD) < D) ++logD;

@@ -195,9 +195,9 @@ cin_bwd_dw_tc_kernel(const __grid_constant__ CUtensorMap tmap_g, const float* __
   Ring ring(sbase + SB * stage_bytes, SB);
 
   const int warp = warp_uniform(threadIdx.x >> 5), lane = threadIdx.x & 31;
-  const int group = blockIdx.x % ngroups, slice = blockIdx.x / ngroups;
-  const int per_slice = (B + nslices - 1) / nslices;
-  const int b_beg = min(B, slice * per_slice), b_end = min(B, b_beg + per_slice);
+  const int group = blockIdx.x % ngroups;
+  int b_beg, b_end;
+  batch_slice(blockIdx.x / ngroups, nslices, B, b_beg, b_end);
 
   ring.init();
   // ============================ TMA: g[b] as [N rows x D] tiles (hi and lo) ============================
@@ -447,9 +447,7 @@ extern "C" int ctr_cin_bwd(const float* x0, const float* xk, const float* filter
   if (sb > 8) sb = 8;
   const int smem = sb * stage_bytes + 8 * 2 * sb + 1024;
   const int ngroups = (int)((hk + DW_IPC - 1) / DW_IPC);
-  int nslices = sms / ngroups;
-  if (nslices < 1) nslices = 1;
-  if (nslices > B) nslices = (int)B;
+  const int nslices = batch_slices(sms, ngroups, B);
   const int grid = ngroups * nslices;
   const int chunk = (int)(256 / D);                          // 96 chained MMAs per accumulator before a drain
   return with_const<32, 64, 128>(NP, [&](auto N) {

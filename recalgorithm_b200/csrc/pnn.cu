@@ -23,7 +23,8 @@
 //                         B = Wm [WP x 32 n] tiles (TMA).  Epilogue: dxt -> shared memory -> chain rule -> d_e.
 //   pnn_bwd_dw_tc_kernel  A = G^T (rows = n, K = samples) from TMA-staged g_out / out chunks of 32 samples;
 //                         B = xt^T [WP x 32 samples], generated on chip into 128B-swizzled shared memory.
-//                         A CTA owns 128 n and a batch slice; one atomic add per element at the end.
+//                         A CTA owns 128 n and a batch slice; one atomic add per element at the end.  The consumer
+//                         loop is tc_ptx.cuh's batch_reduce, shared with the residual unit's weight gradients.
 // Tensor path: WX = FK + Q + 1 <= 128 (WP = WX padded to 32 / 64 / 128) and N % 4 == 0 (the TMA row pitch of g_out / out).
 // That holds the reference defaults (F = K = 8: WX = 101, N = 1024) for both methods.  Other shapes run the CUDA-core
 // kernels below (chosen by shape only).
@@ -37,17 +38,12 @@ using namespace ctr::tc;
 
 constexpr int TILE = NWG * WG_M;             // samples per CTA tile (forward, dx)
 constexpr int FWD_NT = 64;                   // n per forward B tile (wgmma N)
-constexpr int DW_BC = 32;                    // samples per dW chunk
-constexpr int DW_NC = NWG * WG_M;            // n per dW CTA
 constexpr int CHUNK_KS = 32;                 // k-steps per accumulation chain: 32 x 3 = 96 MMAs
 
 __host__ __device__ inline int pair_index(int i, int j, int n) { return i * n - i * (i - 1) / 2 + (j - i); }   // i <= j
 __host__ __device__ inline int64_t num_pairs(int64_t F, int64_t K, int method) {
   return method == 0 ? F * (F + 1) / 2 : K * (K + 1) / 2;
 }
-
-__device__ __forceinline__ void consumers_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // (i, j) of upper-triangle pair q of an n x n matrix
 __device__ __forceinline__ void pair_of(int q, int n, int& i, int& j) {
@@ -396,10 +392,9 @@ pnn_bwd_dw_tc_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_co
   Ring ring(smem_u32(cinfo + WP), SB);
 
   const int warp = warp_uniform(threadIdx.x >> 5), lane = threadIdx.x & 31;
-  const int group = blockIdx.x % ngroups, slice = blockIdx.x / ngroups;
-  const int n_chunks = (B + DW_BC - 1) / DW_BC;
-  const int per_slice = (n_chunks + nslices - 1) / nslices;
-  const int c_beg = min(n_chunks, slice * per_slice), c_end = min(n_chunks, c_beg + per_slice);
+  const int group = blockIdx.x % ngroups;
+  int c_beg, c_end;
+  batch_slice(blockIdx.x / ngroups, nslices, (B + DW_BC - 1) / DW_BC, c_beg, c_end);
   const int n0 = group * DW_NC;
 
   for (int c = threadIdx.x; c < WP; c += blockDim.x) cinfo[c] = column_info(c, FK, Q, METHOD == 0 ? F : K);
@@ -415,65 +410,34 @@ pnn_bwd_dw_tc_kernel(const __grid_constant__ CUtensorMap tmap_g, const __grid_co
       }))
     return;
 
-  // ============================ consumers ============================
+  // ============================ consumers: B = xt^T generated from the staged e rows, A = G^T ============================
   const int wg = warp >> 2, w = warp & 3, g = lane >> 2, t = lane & 3, ct = threadIdx.x;   // ct: 0..255
-  float acc[WP / 2], dacc[WP / 2];
-#pragma unroll
-  for (int q = 0; q < WP / 2; ++q) { acc[q] = 0.f; dacc[q] = 0.f; }
   const int nl0 = wg * WG_M + w * 16 + g;                     // this thread's A rows: n0 + nl0 (+8)
-  for (int c = c_beg; c < c_end; ++c) {
-    const int b0 = c * DW_BC;
-    // 1. stage the chunk's e rows (+ field sums) -- all 256 consumer threads
-    for (int idx = ct; idx < DW_BC * FK; idx += 256) {
-      const int row = idx / FK, col = idx % FK;
-      esm[row * FKP + col] = b0 + row < B ? __ldg(e + (size_t)b0 * FK + idx) : 0.f;
-    }
-    consumers_bar();
-    if (METHOD == 1) {
-      for (int idx = ct; idx < DW_BC * K; idx += 256) {
-        const int row = idx / K, l = idx % K;
-        float v = 0.f;
-        for (int f = 0; f < F; ++f) v += esm[row * FKP + f * K + l];
-        ssm[row * (K + 1) + l] = v;
-      }
-      consumers_bar();
-    }
-    const int s = ring.wait();
-    // 2. xt^T (tf32 hi | lo) into the stage's swizzled B tiles: element (k, b) at byte k*128 + 4b, 16-byte chunk XOR (k & 7)
-    uint8_t* xt = xts + s * xt_bytes;
-    for (int idx = ct; idx < WP * DW_BC; idx += 256) {
-      const int k = idx / DW_BC, b = idx % DW_BC;
-      const float v = b0 + b < B ? feature<METHOD>(cinfo[k], esm + b * FKP, ssm + b * (K + 1), K) : 0.f;
-      const uint32_t o = (uint32_t)(k * 128 + b * 4);
-      store_split(reinterpret_cast<float*>(xt), WP * 32, (o ^ (((o >> 7) & 7u) << 4)) / 4, v);
-    }
-    fence_proxy_async();                                      // generic-proxy writes -> visible to wgmma
-    consumers_bar();
-    // 3. A fragments of G^T: a[q] = G[b = 8ks + t + 4(q>>1)][n = nl0 + 8(q&1)]
-    const float* gs = gos + (size_t)s * 2 * DW_BC * DW_NC;
-    const float* os = gs + DW_BC * DW_NC;
-    uint32_t ah[4][4], al[4][4];
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {
-      float a[4];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const int b = 8 * ks + t + 4 * (q >> 1), nl = nl0 + 8 * (q & 1);
-        a[q] = os[b * DW_NC + nl] > 0.f ? gs[b * DW_NC + nl] : 0.f;
-      }
-      tf32_split(a, ah[ks], al[ks]);
-    }
-    const bool chain_start = chain_first(c - c_beg, CHUNK_KS / 4);
-    const uint64_t bhi = gmma_desc_kmajor(smem_u32(xt), 128);
-    const uint64_t blo = gmma_desc_kmajor(smem_u32(xt + WP * 128), 128);
-    wgmma_fence();
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) mma_3xtf32<WP>(dacc, ah[ks], al[ks], bhi, blo, 2 * ks, (chain_start && ks == 0) ? 0 : 1);
-    wgmma_commit();
-    wgmma_wait_keep(ah, al);
-    ring.release(lane);
-    if (chain_last(c - c_beg, c_end - c_beg, CHUNK_KS / 4)) chain_drain(acc, dacc);
-  }
+  float acc[WP / 2];
+  batch_reduce<WP>(
+      acc, ring, xts, c_beg, c_end, B, lane, nl0,
+      [&](int b0) {                                           // the chunk's e rows (+ field sums)
+        for (int idx = ct; idx < DW_BC * FK; idx += 256) {
+          const int row = idx / FK, col = idx % FK;
+          esm[row * FKP + col] = b0 + row < B ? __ldg(e + (size_t)b0 * FK + idx) : 0.f;
+        }
+        consumers_bar();
+        if (METHOD == 1) {
+          for (int idx = ct; idx < DW_BC * K; idx += 256) {
+            const int row = idx / K, l = idx % K;
+            float v = 0.f;
+            for (int f = 0; f < F; ++f) v += esm[row * FKP + f * K + l];
+            ssm[row * (K + 1) + l] = v;
+          }
+          consumers_bar();
+        }
+      },
+      [&](int k, int, int b) { return feature<METHOD>(cinfo[k], esm + b * FKP, ssm + b * (K + 1), K); },
+      [&](int s, int b, int nl) {                             // G = g_out [out > 0]
+        const float* gs = gos + (size_t)s * 2 * DW_BC * DW_NC;
+        const float* os = gs + DW_BC * DW_NC;
+        return os[b * DW_NC + nl] > 0.f ? gs[b * DW_NC + nl] : 0.f;
+      });
   if (c_end > c_beg) {
 #pragma unroll
     for (int cc = 0; cc < WP / 8; ++cc) {
@@ -674,17 +638,6 @@ int check_pnn(const char* fn, int64_t B, int64_t F, int64_t K, int64_t N, int me
   return CTR_OK;
 }
 
-// a row-major [outer x inner] float matrix, one box of [box_outer x box_inner]
-int encode_2d(const char* fn, CUtensorMap* map, const void* base, uint64_t inner, uint64_t outer, uint32_t box_inner,
-              uint32_t box_outer, CUtensorMapSwizzle sw) {
-  const cuuint64_t gdim[2] = {(cuuint64_t)inner, (cuuint64_t)outer};
-  const cuuint64_t gstr[1] = {(cuuint64_t)inner * sizeof(float)};
-  const cuuint32_t box[2] = {box_inner, box_outer};
-  return encode_tmap(fn, map, 2, base, gdim, gstr, box, sw);
-}
-
-constexpr size_t SMEM_CAP = 226 * 1024;     // dynamic shared memory per CTA on sm_90 (227 KB) less slack
-
 }  // namespace
 
 extern "C" int ctr_pnn_workspace_bytes(int64_t F, int64_t K, int64_t N, int method, int64_t* bytes) {
@@ -776,14 +729,10 @@ extern "C" int ctr_pnn_bwd(const float* e, const float* wlin, const float* wprod
     rc = encode_2d(fn, &to, out, N, B, DW_NC, DW_BC, CU_TENSOR_MAP_SWIZZLE_NONE);
     if (rc) return rc;
     const int ngroups = (int)((N + DW_NC - 1) / DW_NC);
-    const int64_t chunks = (B + DW_BC - 1) / DW_BC;
-    int nslices = sms / ngroups;
-    if (nslices < 1) nslices = 1;
-    if (nslices > chunks) nslices = (int)chunks;
+    const int nslices = batch_slices(sms, ngroups, (B + DW_BC - 1) / DW_BC);
     const size_t fixed = dw_smem_bytes(s.WP, 0, (int)s.FK, (int)s.K) + 1024;
     const size_t stage = (size_t)dw_smem_bytes(s.WP, 1, (int)s.FK, (int)s.K) + 1024 - fixed;
-    int sb = (int)((SMEM_CAP - fixed) / stage);
-    if (sb > 4) sb = 4;
+    const int sb = stages_that_fit(fixed, stage);
     rc = with_const<0, 1>(method, [&](auto M) {
       return with_const<32, 64, 128>(s.WP, [&](auto WP) {
         if (int r = launch("ctr_pnn_bwd(dx, wgmma)", pnn_bwd_dx_tc_kernel<WP, 4, M>, capped_grid(tiles, sms), NTHREADS,

@@ -20,7 +20,8 @@
 //   resunit_bwd_dw_wgmma_kernel  dW1 = h^T . gy and dW0^T = gh^T . x, with sum_b gh = db0 alongside: A = h^T or gh^T (rows =
 //                                hidden units, K = samples) from TMA-staged [32 samples x 128 units] chunks, B = gy^T or x^T
 //                                [DP x 32 samples] generated on chip into 128B-swizzled shared memory.  A CTA owns 128 hidden
-//                                units and a batch slice, and issues one atomic add per element at the end.
+//                                units and a batch slice, and issues one atomic add per element at the end.  The
+//                                consumer loop is tc_ptx.cuh's batch_reduce, shared with the PNN weight gradients.
 // The rows of x, out and g are d floats (328 B at the reference d = 82), not a multiple of 16 bytes, so they are staged with
 // ordinary loads; only the prepped weights and the workspace's h / gh (pitch HP) are TMA tensors.
 //
@@ -41,11 +42,6 @@ using namespace ctr::tc;
 constexpr int TILE = NWG * WG_M;             // samples per CTA tile (forward, dx)
 constexpr int HC = 32;                       // hidden units per chunk: N of the row GEMMs, K of the hidden GEMMs
 constexpr int CHAIN = 32 / (HC / 8);         // chunks per accumulation chain: 32 k-steps x 3 = 96 MMAs
-constexpr int DW_BC = 32;                    // samples per dW chunk
-constexpr int DW_NC = NWG * WG_M;            // hidden units per dW CTA
-
-__device__ __forceinline__ void consumers_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // hidden unit held at k position `k` of a permuted operand: within each group of 8, k = m < 4 holds 2m and k = m >= 4 holds
 // 2(m - 4) + 1 (the accumulator column order, see the file header)
@@ -363,10 +359,9 @@ resunit_bwd_dw_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_p, const fl
   Ring ring(smem_u32(ps + SB * p_floats), SB);
 
   const int warp = warp_uniform(threadIdx.x >> 5), lane = threadIdx.x & 31;
-  const int group = blockIdx.x % ngroups, slice = blockIdx.x / ngroups;
-  const int n_chunks = (B + DW_BC - 1) / DW_BC;
-  const int per_slice = (n_chunks + nslices - 1) / nslices;
-  const int c_beg = min(n_chunks, slice * per_slice), c_end = min(n_chunks, c_beg + per_slice);
+  const int group = blockIdx.x % ngroups;
+  int c_beg, c_end;
+  batch_slice(blockIdx.x / ngroups, nslices, (B + DW_BC - 1) / DW_BC, c_beg, c_end);
   const int n0 = group * DW_NC;
 
   ring.init();
@@ -379,54 +374,23 @@ resunit_bwd_dw_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_p, const fl
       }))
     return;
 
-  // ============================ consumers ============================
-  const int wg = warp >> 2, w = warp & 3, g = lane >> 2, t = lane & 3, ct = threadIdx.x;   // ct: 0..255
-  float acc[DP / 2], dacc[DP / 2];
-#pragma unroll
-  for (int i = 0; i < DP / 2; ++i) { acc[i] = 0.f; dacc[i] = 0.f; }
+  // ============================ consumers: B = Q^T generated from q, A = P^T ============================
+  const int wg = warp >> 2, w = warp & 3, g = lane >> 2, t = lane & 3;
   float rsum[2] = {0.f, 0.f};                               // MODE 1: sum_b gh of this thread's two units
   const int nl0 = wg * WG_M + w * 16 + g;                   // this thread's A rows: units n0 + nl0 (+8)
-  for (int c = c_beg; c < c_end; ++c) {
-    const int b0 = c * DW_BC;
-    const int s = ring.wait();
-    // Q^T (tf32 hi | lo) into the stage's swizzled B tiles: element (k, b) at byte k*128 + 4b, 16-byte chunk XOR (k & 7)
-    uint8_t* qt = qts + s * qt_bytes;
-    for (int idx = ct; idx < DP * DW_BC; idx += 256) {
-      const int k = idx / DW_BC, b = idx % DW_BC;
-      float v = 0.f;
-      if (k < d && b0 + b < B) {
+  float acc[DP / 2];
+  batch_reduce<DP>(
+      acc, ring, qts, c_beg, c_end, B, lane, nl0, [](int) {},
+      [&](int k, int b0, int b) {
+        if (k >= d) return 0.f;
         const size_t o = (size_t)(b0 + b) * d + k;
-        v = (MODE == 1 || __ldg(qmask + o) > 0.f) ? __ldg(q + o) : 0.f;
-      }
-      const uint32_t off = (uint32_t)(k * 128 + b * 4);
-      store_split(reinterpret_cast<float*>(qt), DP * 32, (off ^ (((off >> 7) & 7u) << 4)) / 4, v);
-    }
-    fence_proxy_async();                                    // generic-proxy writes -> visible to wgmma
-    consumers_bar();
-    // A fragments of P^T: a[r] = P[b = 8ks + t + 4(r>>1)][unit nl0 + 8(r&1)]
-    const float* pc = ps + (size_t)s * p_floats;
-    uint32_t ah[4][4], al[4][4];
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {
-      float a[4];
-#pragma unroll
-      for (int r = 0; r < 4; ++r) {
-        a[r] = pc[(8 * ks + t + 4 * (r >> 1)) * DW_NC + nl0 + 8 * (r & 1)];
-        if (MODE == 1) rsum[r & 1] += a[r];
-      }
-      tf32_split(a, ah[ks], al[ks]);
-    }
-    const bool chain_start = chain_first(c - c_beg, CHAIN);
-    const uint64_t bhi = gmma_desc_kmajor(smem_u32(qt), 128);
-    const uint64_t blo = gmma_desc_kmajor(smem_u32(qt + DP * 128), 128);
-    wgmma_fence();
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) mma_3xtf32<DP>(dacc, ah[ks], al[ks], bhi, blo, 2 * ks, (chain_start && ks == 0) ? 0 : 1);
-    wgmma_commit();
-    wgmma_wait_keep(ah, al);
-    ring.release(lane);
-    if (chain_last(c - c_beg, c_end - c_beg, CHAIN)) chain_drain(acc, dacc);
-  }
+        return (MODE == 1 || __ldg(qmask + o) > 0.f) ? __ldg(q + o) : 0.f;
+      },
+      [&](int s, int b, int nl) {
+        const float v = ps[(size_t)s * p_floats + b * DW_NC + nl];
+        if (MODE == 1) rsum[nl == nl0 ? 0 : 1] += v;
+        return v;
+      });
   if (c_end <= c_beg) return;
 #pragma unroll
   for (int cc = 0; cc < DP / 8; ++cc) {
@@ -489,15 +453,6 @@ int check_shape(const char* fn, int64_t B, int64_t d, int64_t H) {
   return CTR_OK;
 }
 
-// a row-major [outer x inner] float matrix, one box of [box_outer x box_inner]
-int encode_2d(const char* fn, CUtensorMap* map, const void* base, uint64_t inner, uint64_t outer, uint32_t box_inner,
-              uint32_t box_outer, CUtensorMapSwizzle sw) {
-  const cuuint64_t gdim[2] = {(cuuint64_t)inner, (cuuint64_t)outer};
-  const cuuint64_t gstr[1] = {(cuuint64_t)inner * sizeof(float)};
-  const cuuint32_t box[2] = {box_inner, box_outer};
-  return encode_tmap(fn, map, 2, base, gdim, gstr, box, sw);
-}
-
 // prepped layout in workspace slot `slot`, as a rows operand ([2 HP][DP], boxes of [HC x 32]) or a hidden operand
 // ([2 DP][HP], boxes of [DP x 32])
 int encode_weights(const char* fn, CUtensorMap* map, float* ws, const RuShape& s, int slot, bool rows) {
@@ -511,8 +466,6 @@ int prep(const char* what, const float* w0, const float* w1, float* ws, int64_t 
   return launch(what, resunit_prep_kernel, dim3(capped_grid((s.HP * s.DP + 255) / 256, 1024), nslots), 256, 0, st, w0, w1,
                 ws, (int)d, (int)H, s.DP, (int)s.HP, layouts);
 }
-
-constexpr size_t SMEM_CAP = 226 * 1024;     // dynamic shared memory per CTA on sm_90 (227 KB) less slack
 
 }  // namespace
 
@@ -582,10 +535,7 @@ extern "C" int ctr_residual_unit_bwd(const float* x, const float* w0, const floa
   const int sms = sm_count();
   const int grid = capped_grid((B + TILE - 1) / TILE, sms);
   const int ngroups = (int)((s.HP + DW_NC - 1) / DW_NC);
-  const int64_t chunks = (B + DW_BC - 1) / DW_BC;
-  int nslices = sms / ngroups;
-  if (nslices < 1) nslices = 1;
-  if (nslices > chunks) nslices = (int)chunks;
+  const int nslices = batch_slices(sms, ngroups, (B + DW_BC - 1) / DW_BC);
   return with_const<32, 64, 96, 128>(s.DP, [&](auto DP) {
     constexpr int SB = DP == 128 ? 2 : 4;
     static_assert(dx_smem_bytes(DP, SB) + 1024 <= SMEM_CAP, "dx shared memory");
@@ -593,8 +543,7 @@ extern "C" int ctr_residual_unit_bwd(const float* x, const float* w0, const floa
                        dx_smem_bytes(DP, SB) + 1024, st, m0, m2, m3, x, b0, out, g_out, d_x, hbuf, ghbuf, d_b1, (int)B,
                        (int)d, (int)H, (int)s.HP))
       return r;
-    int sb = (int)((SMEM_CAP - 1024) / dw_smem_bytes(DP, 1));
-    if (sb > 4) sb = 4;
+    const int sb = stages_that_fit(1024, dw_smem_bytes(DP, 1));
     const size_t smem = dw_smem_bytes(DP, sb) + 1024;
     if (int r = launch("ctr_residual_unit_bwd(dw1, wgmma)", resunit_bwd_dw_wgmma_kernel<DP, 0>, ngroups * nslices, NTHREADS,
                        smem, st, mh, g_out, out, d_w1, nullptr, (int)B, (int)d, (int)H, ngroups, nslices, sb))

@@ -1,6 +1,7 @@
 // wgmma / TMA / mbarrier PTX wrappers shared by the tensor-core kernels (sm_90a), the pipeline mechanics built on them
-// (shared-memory alignment, the mbarrier ring, the producer / consumer role split, the 3xTF32 k-step, accumulation chains)
-// and the host side of a tensor-core launch (workspace check, tensor-map encoding).
+// (shared-memory alignment, the mbarrier ring, the producer / consumer role split, the 3xTF32 k-step, accumulation chains,
+// the consumer loop of the batch-reduction weight-gradient GEMMs) and the host side of a tensor-core launch (workspace
+// check, tensor-map encoding, batch slices and ring depth of the weight-gradient kernels).
 #pragma once
 #include <cuda.h>
 
@@ -47,6 +48,10 @@ template <int R>
 __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R)); }
 // barrier over the 128 threads of one warpgroup (ids 1.. ; 0 is __syncthreads)
 __device__ __forceinline__ void wg_bar_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+// barrier over the 256 threads of both consumer warpgroups (id 1: kernels that use it do not use wg_bar_sync)
+__device__ __forceinline__ void consumers_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+// makes this thread's generic-proxy shared-memory writes visible to the async proxy (wgmma operand reads)
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint32_t bar) {
   asm volatile(
@@ -178,6 +183,13 @@ __device__ __forceinline__ void store_split(float* dst, size_t total, size_t idx
   dst[idx] = hi;
   dst[total + idx] = v - hi;
 }
+// store_split into a K-major SWIZZLE_128B B-operand tile written by threads instead of TMA: `rows` 128-byte rows of 32 tf32
+// (hi tile, then the lo tile rows * 128 bytes on), 1024-byte aligned.  Element (k, b) sits at byte k * 128 + 4 b with its
+// 16-byte chunk index XORed with k & 7, the placement TMA's SWIZZLE_128B gives and gmma_desc_kmajor(.., 128) reads.
+__device__ __forceinline__ void store_split_sw128(float* tile, int rows, int k, int b, float v) {
+  const uint32_t o = (uint32_t)(k * 128 + b * 4);
+  store_split(tile, rows * 32, (o ^ (((o >> 7) & 7u) << 4)) / 4, v);
+}
 
 // SWIZZLE_128B tiles must be 1024-byte aligned: the kernels align their dynamic shared memory here, and every launch
 // asks for 1 KB of slack on top of the layout.
@@ -247,7 +259,71 @@ __device__ __forceinline__ bool producer_role(int warp, int lane, Producer&& pro
   return false;
 }
 
+// Batch slice `slice` of `nslices` over n_units (chunks or samples) of a batch-reduction grid: [beg, end), up to
+// ceil(n_units / nslices) units; empty for the slices past the end.
+__device__ __forceinline__ void batch_slice(int slice, int nslices, int n_units, int& beg, int& end) {
+  const int per_slice = (n_units + nslices - 1) / nslices;
+  beg = min(n_units, slice * per_slice);
+  end = min(n_units, beg + per_slice);
+}
+
+// Batch-reduction GEMM of the weight-gradient kernels: acc[DW_NC rows][N] = sum_b P[b, row] Q[b, k] over the chunks
+// [c_beg, c_end) of DW_BC samples, b < B.  A = P^T (rows x samples) from a TMA-staged P chunk, B = Q^T (N x samples)
+// generated on chip.
+constexpr int DW_BC = KB;                    // samples per chunk: the K of 4 k-steps, one 128-byte swizzle row of Q^T
+constexpr int DW_NC = NWG * WG_M;            // rows (P columns) per CTA
+
+// The consumer side, run by all 256 consumer threads, one ring stage per chunk.  The stage's Q^T tiles sit at
+// qts + stage * 2 N 128 (written here); its P chunk is wherever the producer put it.  Per chunk b0 = c DW_BC:
+//   stage_chunk(b0)   the caller's per-chunk staging for q_of (it may use consumers_bar), or nothing;
+//   Q^T (hi | lo) into the stage's swizzled tiles, element (k, b) = q_of(k, b0, b) for b0 + b < B, else 0;
+//   A fragments of P^T, element (row, b) = p_of(stage, b, row): row = this thread's nl0 or nl0 + 8, b < DW_BC;
+//   4 3xTF32 k-steps, then the stage is released; chains of 8 chunks (32 k-steps, 96 MMAs) drained into acc.
+// The caller owns the shared-memory layout, the producer and the epilogue (acc: the D fragment of rows nl0, nl0 + 8).
+template <int N, class Stage, class QOf, class POf>
+__device__ __forceinline__ void batch_reduce(float (&acc)[N / 2], Ring& ring, uint8_t* qts, int c_beg, int c_end, int B,
+                                             int lane, int nl0, Stage&& stage_chunk, QOf&& q_of, POf&& p_of) {
+  constexpr int qt_bytes = 2 * N * 128;
+  constexpr int CHAIN = 8;                   // chunks per accumulation chain
+  const int t = lane & 3;
+  float dacc[N / 2];
+#pragma unroll
+  for (int q = 0; q < N / 2; ++q) { acc[q] = 0.f; dacc[q] = 0.f; }
+  for (int c = c_beg; c < c_end; ++c) {
+    const int b0 = c * DW_BC;
+    stage_chunk(b0);
+    const int s = ring.wait();
+    float* qt = reinterpret_cast<float*>(qts + s * qt_bytes);
+    for (int idx = threadIdx.x; idx < N * DW_BC; idx += NWG * 128) {
+      const int k = idx / DW_BC, b = idx % DW_BC;
+      store_split_sw128(qt, N, k, b, b0 + b < B ? q_of(k, b0, b) : 0.f);
+    }
+    fence_proxy_async();
+    consumers_bar();
+    uint32_t ah[4][4], al[4][4];
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) {
+      float a[4];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) a[q] = p_of(s, 8 * ks + t + 4 * (q >> 1), nl0 + 8 * (q & 1));
+      tf32_split(a, ah[ks], al[ks]);
+    }
+    const bool chain_start = chain_first(c - c_beg, CHAIN);
+    const uint64_t bhi = gmma_desc_kmajor(smem_u32(qt), 128);
+    const uint64_t blo = gmma_desc_kmajor(smem_u32(qt + N * 32), 128);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) mma_3xtf32<N>(dacc, ah[ks], al[ks], bhi, blo, 2 * ks, (chain_start && ks == 0) ? 0 : 1);
+    wgmma_commit();
+    wgmma_wait_keep(ah, al);
+    ring.release(lane);
+    if (chain_last(c - c_beg, c_end - c_beg, CHAIN)) chain_drain(acc, dacc);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ host
+constexpr size_t SMEM_CAP = 226 * 1024;     // dynamic shared memory per CTA on sm_90 (227 KB) less slack
+
 static inline int64_t pad_to(int64_t v, int64_t q) { return (v + q - 1) / q * q; }
 // wgmma N (or K) class of a width v <= 128: 32, 64 or 128
 static inline int pad3(int64_t v) { return v <= 32 ? 32 : v <= 64 ? 64 : 128; }
@@ -286,6 +362,27 @@ static inline int encode_tmap(const char* fn, CUtensorMap* map, int rank, const 
     return CTR_ERR_CUDA;
   }
   return CTR_OK;
+}
+
+// a row-major [outer x inner] float matrix, one box of [box_outer x box_inner]
+static inline int encode_2d(const char* fn, CUtensorMap* map, const void* base, uint64_t inner, uint64_t outer,
+                            uint32_t box_inner, uint32_t box_outer, CUtensorMapSwizzle sw) {
+  const cuuint64_t gdim[2] = {(cuuint64_t)inner, (cuuint64_t)outer};
+  const cuuint64_t gstr[1] = {(cuuint64_t)inner * sizeof(float)};
+  const cuuint32_t box[2] = {box_inner, box_outer};
+  return encode_tmap(fn, map, 2, base, gdim, gstr, box, sw);
+}
+
+// Slices per group of a batch-reduction grid of ngroups x nslices CTAs: one wave over the SMs, at most one per unit.
+static inline int batch_slices(int sms, int64_t ngroups, int64_t n_units) {
+  int64_t n = sms / ngroups;
+  if (n < 1) n = 1;
+  return (int)(n < n_units ? n : n_units);
+}
+// Ring stages of a batch-reduction kernel: as many as fit in SMEM_CAP next to `fixed` bytes (slack included), at most 4.
+static inline int stages_that_fit(size_t fixed, size_t stage) {
+  const size_t sb = (SMEM_CAP - fixed) / stage;
+  return (int)(sb < 4 ? sb : 4);
 }
 
 }  // namespace tc

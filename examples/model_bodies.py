@@ -151,3 +151,23 @@ def deepcrossing_logit(dense_input, category_input, residual_internal_dim=256, r
         for i in range(residual_network_num):
             net = L.residual_unit(net, residual_internal_dim, index=i)
     return dense(net, 1)                                                                  # :159
+
+
+def mmoe_logits(dense_input, category_input, labels, task_names=("read_comment", "like", "click_avatar"), num_experts=3,
+                expert_hidden_units=512, hidden_units=(512, 256, 128)):
+    """MMOE/mmoe.py:205-263: experts, gates and gated sums in one kernel each way, then one tower_layer per task
+    (MMOE/tower_layer.py: relu dense stack, tower_{task}_logit; its batch norm and dropout left out) in scope tower, and the
+    sum of the per-task mean sigmoid cross-entropies.  labels maps task name -> (B, 1).  Returns (logits, total_loss)."""
+    concat_all_input = torch.cat([dense_input, category_input], dim=-1)                   # :205
+    towers = L.mmoe_experts_gates(concat_all_input, num_experts, expert_hidden_units, len(task_names))   # :208-236
+    logits, n_dense = [], 0
+    with L.variable_scope("tower"):
+        for x, task_name in zip(towers, task_names):                                      # :241-246
+            net = x
+            for unit in hidden_units:                                                     # TF uniquifies dense, dense_1, ...
+                net = dense(net, unit, activation=torch.relu, name=f"dense_{n_dense}" if n_dense else "dense")
+                n_dense += 1
+            logits.append(dense(net, 1, name=f"tower_{task_name}_logit"))
+    losses = [torch.nn.functional.binary_cross_entropy_with_logits(logit, labels[task_name])          # :261-263
+              for logit, task_name in zip(logits, task_names)]
+    return logits, sum(losses[1:], losses[0])

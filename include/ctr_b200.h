@@ -310,6 +310,27 @@ int ctr_residual_unit_bwd(const float* x, const float* w0, const float* b0, cons
                           const float* out, const float* g_out, int64_t B, int64_t d, int64_t H, float* d_x, float* d_w0,
                           float* d_b0, float* d_w1, float* d_b1, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- MMoE expert-gate layer ------------------------------------------------------------------------------
+ * Replaces the experts / gates / tower blocks of mmoe_model_fn (MMOE/mmoe.py:207-236) up to the task towers:
+ *   h_e     = relu(x . w_e + b_e)        x (B,d) = concat_all_input; w_experts (E,d,H): w_e = experts/expert_{e}/kernel,
+ *                                        b_experts (E,H): b_e = experts/expert_{e}/bias, e < E = num_experts;
+ *   p_t     = softmax_e(x . g_t)         w_gates (T,d,E): g_t = gates/gate_{t}/kernel (no bias), t < T = num_tasks;
+ *   tower_t = sum_e p_t[e] h_e           towers (T,B,H), gates (T,B,E) (the reference's gate_log, :298).
+ * fp32-class accuracy (3xTF32 on the tensor cores); the (B,E,H) expert outputs stay on chip.  1 <= d <= 128, 1 <= E <= 8,
+ * 1 <= H <= 1024 and 1 <= T <= 4 (CTR_ERR_UNSUPPORTED otherwise); B = 0 launches nothing.
+ * workspace: 128-byte aligned, at least ctr_mmoe_workspace_bytes(0, d, E, H, T) bytes for the forward (the prepped
+ * weights) and ctr_mmoe_workspace_bytes(B, d, E, H, T) for the backward (also the expert and gate-logit gradients,
+ * (B, E*HP + 32) floats with HP = H rounded up to 32).  The backward takes the forward's gates and g_towers (T,B,H), and overwrites d_x (B,d),
+ * d_w_experts (E,d,H), d_b_experts (E,H) and d_w_gates (T,d,E) (zeros at B = 0). */
+int ctr_mmoe_workspace_bytes(int64_t B, int64_t d, int64_t E, int64_t H, int64_t T, int64_t* bytes);
+int ctr_mmoe_fwd(const float* x, const float* w_experts, const float* b_experts, const float* w_gates, int64_t B, int64_t d,
+                 int64_t E, int64_t H, int64_t T, float* towers, float* gates, void* workspace, int64_t workspace_bytes,
+                 void* stream);
+int ctr_mmoe_bwd(const float* x, const float* w_experts, const float* b_experts, const float* w_gates, const float* gates,
+                 const float* g_towers, int64_t B, int64_t d, int64_t E, int64_t H, int64_t T, float* d_x,
+                 float* d_w_experts, float* d_b_experts, float* d_w_gates, void* workspace, int64_t workspace_bytes,
+                 void* stream);
+
 /* ---- Row DIN-ATT: DIN attention unit -----------------------------------------------------------------
  * Replaces din_attention(query, keys, keys_length, is_softmax) (DIN/din_attention.py:17-43).
  * query (B,H); keys (B,T,H); keys_length int64 (B); dense layers f1_att (4H->64, relu), f2_att (64->32,

@@ -96,6 +96,9 @@ SIGNATURES = {
     "ctr_residual_unit_workspace_bytes": (c_int, [_I, _I, _I, POINTER(c_int64)]),
     "ctr_residual_unit_fwd": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _I, _P]),
     "ctr_residual_unit_bwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _I, _P]),
+    "ctr_mmoe_workspace_bytes": (c_int, [_I, _I, _I, _I, _I, POINTER(c_int64)]),
+    "ctr_mmoe_fwd": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _I, _P]),
+    "ctr_mmoe_bwd": (c_int, [_P] * 6 + [_I] * 5 + [_P] * 5 + [_I, _P]),
 }
 
 

@@ -454,3 +454,23 @@ class _ResidualUnit(torch.autograd.Function):
 def residual_unit(x: torch.Tensor, w0: torch.Tensor, b0: torch.Tensor, w1: torch.Tensor, b1: torch.Tensor) -> torch.Tensor:
     """DeepCrossing residual unit: relu(x + relu(x . w0 + b0) . w1 + b1), (B,d) -> (B,d)."""
     return _ResidualUnit.apply(x, w0, b0, w1, b1)
+
+
+class _MMoE(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, w_experts, b_experts, w_gates):
+        x, w_experts, b_experts, w_gates = (t.contiguous() for t in (x, w_experts, b_experts, w_gates))
+        towers, gates = ops.mmoe_fwd(x, w_experts, b_experts, w_gates)
+        ctx.save_for_backward(x, w_experts, b_experts, w_gates, gates)   # the expert outputs are recomputed from x
+        ctx.mark_non_differentiable(gates)
+        return towers, gates
+
+    @staticmethod
+    def backward(ctx, g_towers, _g_gates):
+        return ops.mmoe_bwd(*ctx.saved_tensors, g_towers.contiguous())
+
+
+def mmoe(x: torch.Tensor, w_experts: torch.Tensor, b_experts: torch.Tensor, w_gates: torch.Tensor):
+    """MMoE expert-gate layer: (towers (T,B,H), gates (T,B,E), forward only) from x (B,d), w_experts (E,d,H), b_experts (E,H)
+    and w_gates (T,d,E)."""
+    return _MMoE.apply(x, w_experts, b_experts, w_gates)

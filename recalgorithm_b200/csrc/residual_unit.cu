@@ -25,12 +25,10 @@
 // The rows of x, out and g are d floats (328 B at the reference d = 82), not a multiple of 16 bytes, so they are staged with
 // ordinary loads; only the prepped weights and the workspace's h / gh (pitch HP) are TMA tensors.
 //
-// h feeds the second GEMM straight from the accumulator registers of the first.  The wgmma accumulator gives thread (g, t)
-// columns 8c + 2t and 8c + 2t + 1 of each 8-column group c, and the A fragment of k-step c wants columns 8c + t and
-// 8c + t + 4.  Since a sum over k does not depend on its order, the fragment takes the accumulator's two columns as its
-// k = t and k = t + 4, and the prep kernel permutes the hidden rows of W1 (and of W0 for the backward's gh . W0^T) within each
-// group of 8 to match (perm8).  The alternative, a round trip of h through shared memory, would cost a store, a warpgroup
-// barrier and a load per chunk for nothing.
+// h feeds the second GEMM straight from the accumulator registers of the first: the prep kernel permutes the hidden rows of
+// W1 (and of W0 for the backward's gh . W0^T) within each group of 8 to match the accumulator's column order (perm8 and the
+// row-chunk GEMMs live in tc_ptx.cuh, shared with csrc/mmoe.cu).  The alternative, a round trip of h through shared memory,
+// would cost a store, a warpgroup barrier and a load per chunk for nothing.
 //
 // Tensor path (the only path): d <= 128, 1 <= H <= 1024, any B >= 0.  Other shapes return CTR_ERR_UNSUPPORTED.
 #include "tc_ptx.cuh"
@@ -38,17 +36,9 @@
 namespace ctr {
 namespace resunit {
 using namespace ctr::tc;
+using namespace ctr::tc::rows;
 
 constexpr int TILE = NWG * WG_M;             // samples per CTA tile (forward, dx)
-constexpr int HC = 32;                       // hidden units per chunk: N of the row GEMMs, K of the hidden GEMMs
-constexpr int CHAIN = 32 / (HC / 8);         // chunks per accumulation chain: 32 k-steps x 3 = 96 MMAs
-
-// hidden unit held at k position `k` of a permuted operand: within each group of 8, k = m < 4 holds 2m and k = m >= 4 holds
-// 2(m - 4) + 1 (the accumulator column order, see the file header)
-__host__ __device__ __forceinline__ int perm8(int k) {
-  const int m = k & 7;
-  return (k & ~7) | (m < 4 ? 2 * m : 2 * m - 7);
-}
 
 // Writes the tf32 hi | lo copies of the weights, zero padded, one layout per blockIdx.y slot (2 HP DP floats each):
 //   0: W0^T [HP][DP]    1: W1^T [DP][HP] hidden order perm8    2: W1 [HP][DP]    3: W0 [DP][HP] hidden order perm8
@@ -65,93 +55,6 @@ __global__ void resunit_prep_kernel(const float* __restrict__ w0, const float* _
     float v = 0.f;
     if (i < d && j < H) v = (L == 0 || L == 3) ? __ldg(w0 + (size_t)i * H + j) : __ldg(w1 + (size_t)j * d + i);
     store_split(o, total, idx, v);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------ shared device pieces
-__host__ __device__ constexpr int row_pitch(int DP) { return DP + 4; }   // staged rows: conflict-free A-fragment reads
-__host__ __device__ constexpr int stage_bytes(int DP) { return 2 * HC * DP * 4; }
-
-// TMA loads of one weight chunk j into a stage (hi tile, then lo tile):
-// rows operand: [HC units x DP] K-major from a [2 HP][DP] map, DP / 32 boxes of [HC x 32] per copy;
-// hidden operand: [DP x HC units] K-major from a [2 DP][HP] map, one box of [DP x 32] per copy.
-template <int DP>
-__device__ __forceinline__ void load_rows_operand(uint32_t dst, const CUtensorMap* map, int j, int HP, uint32_t bar) {
-#pragma unroll
-  for (int kb = 0; kb < DP / KB; ++kb) {
-    tma_load_2d(dst + kb * HC * 128, map, kb * KB, j * HC, bar);
-    tma_load_2d(dst + HC * DP * 4 + kb * HC * 128, map, kb * KB, HP + j * HC, bar);
-  }
-}
-template <int DP>
-__device__ __forceinline__ void load_hidden_operand(uint32_t dst, const CUtensorMap* map, int j, uint32_t bar) {
-  tma_load_2d(dst, map, j * HC, 0, bar);
-  tma_load_2d(dst + DP * 128, map, j * HC, DP, bar);
-}
-
-// D[64 x HC] = R[64 x DP] . B: R = this warpgroup's 64 staged rows (pitch row_pitch(DP)), B = a rows-operand stage.
-// Issued one 32-column block (4 k-steps) at a time, so that only 32 fragment registers are live.
-template <int DP>
-__device__ __forceinline__ void gemm_rows(float (&d)[HC / 2], const float* rows, int r0, int t, uint32_t stage) {
-  constexpr int LD = row_pitch(DP);
-  const uint64_t bhi = gmma_desc_kmajor(stage, 128);
-  const uint64_t blo = gmma_desc_kmajor(stage + HC * DP * 4, 128);
-#pragma unroll
-  for (int kb = 0; kb < DP / KB; ++kb) {
-    uint32_t ah[4][4], al[4][4];
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {
-      float a[4];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) a[q] = rows[(r0 + 8 * (q & 1)) * LD + kb * KB + 8 * ks + t + 4 * (q >> 1)];
-      tf32_split(a, ah[ks], al[ks]);
-    }
-    wgmma_fence();
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks)
-      mma_3xtf32<HC>(d, ah[ks], al[ks], bhi, blo, (uint64_t)(kb * (HC * 128 / 16) + 2 * ks), (kb | ks) ? 1 : 0);
-    wgmma_commit();
-    wgmma_wait_keep(ah, al);
-  }
-}
-
-// A fragments of a hidden chunk held in accumulator layout: k-step c takes the thread's columns 8c + 2t (as k = t) and
-// 8c + 2t + 1 (as k = t + 4) of rows g and g + 8 -- the order perm8 gives the B operand.
-__device__ __forceinline__ void acc_to_a(const float (&v)[HC / 2], uint32_t (&hh)[HC / 8][4], uint32_t (&hl)[HC / 8][4]) {
-#pragma unroll
-  for (int c = 0; c < HC / 8; ++c) {
-    const float a[4] = {v[4 * c], v[4 * c + 2], v[4 * c + 1], v[4 * c + 3]};
-    tf32_split(a, hh[c], hl[c]);
-  }
-}
-
-// D[64 x DP] (+)= Hc[64 x HC] . B: Hc from acc_to_a, B = a hidden-operand stage; `start` begins a new chain.
-template <int DP>
-__device__ __forceinline__ void gemm_hidden(float (&d)[DP / 2], uint32_t (&hh)[HC / 8][4], uint32_t (&hl)[HC / 8][4],
-                                            uint32_t stage, bool start) {
-  const uint64_t bhi = gmma_desc_kmajor(stage, 128);
-  const uint64_t blo = gmma_desc_kmajor(stage + DP * 128, 128);
-  wgmma_fence();
-#pragma unroll
-  for (int c = 0; c < HC / 8; ++c) mma_3xtf32<DP>(d, hh[c], hl[c], bhi, blo, (uint64_t)(2 * c), (start && c == 0) ? 0 : 1);
-  wgmma_commit();
-  wgmma_wait_keep(hh, hl);
-}
-
-// Stages this warpgroup's 64 rows of a (B, d) tensor, zero padded to DP columns and past B; with `mask`, the rows of
-// g [mask > 0] instead (gy of the backward).
-template <int DP>
-__device__ __forceinline__ void stage_rows(float* dst, const float* __restrict__ src, const float* __restrict__ mask,
-                                           long long base, int B, int d, int tw) {
-  constexpr int LD = row_pitch(DP);
-  for (int idx = tw; idx < WG_M * DP; idx += 128) {
-    const int r = idx / DP, c = idx % DP;
-    float v = 0.f;
-    if (c < d && base + r < B) {
-      const size_t o = (size_t)(base + r) * d + c;
-      v = (mask == nullptr || __ldg(mask + o) > 0.f) ? __ldg(src + o) : 0.f;
-    }
-    dst[r * LD + c] = v;
   }
 }
 
@@ -435,7 +338,7 @@ struct RuShape {
 
 RuShape shape_of(int64_t B, int64_t d, int64_t H) {
   RuShape s;
-  s.DP = d <= 32 ? 32 : d <= 64 ? 64 : d <= 96 ? 96 : 128;
+  s.DP = dp_class(d);
   s.HP = pad_to(H, HC);
   s.slot_floats = 2 * s.HP * s.DP;
   s.fwd_bytes = pad_to(2 * s.slot_floats * (int64_t)sizeof(float), 128);
@@ -457,8 +360,7 @@ int check_shape(const char* fn, int64_t B, int64_t d, int64_t H) {
 // ([2 DP][HP], boxes of [DP x 32])
 int encode_weights(const char* fn, CUtensorMap* map, float* ws, const RuShape& s, int slot, bool rows) {
   const float* base = ws + s.slot_floats * slot;
-  if (rows) return encode_2d(fn, map, base, s.DP, 2 * s.HP, KB, HC, CU_TENSOR_MAP_SWIZZLE_128B);
-  return encode_2d(fn, map, base, s.HP, 2 * s.DP, KB, s.DP, CU_TENSOR_MAP_SWIZZLE_128B);
+  return rows ? encode_rows_operand(fn, map, base, s.DP, s.HP) : encode_hidden_operand(fn, map, base, s.DP, s.HP);
 }
 
 int prep(const char* what, const float* w0, const float* w1, float* ws, int64_t d, int64_t H, const RuShape& s, int nslots,

@@ -1,7 +1,8 @@
 // wgmma / TMA / mbarrier PTX wrappers shared by the tensor-core kernels (sm_90a), the pipeline mechanics built on them
 // (shared-memory alignment, the mbarrier ring, the producer / consumer role split, the 3xTF32 k-step, accumulation chains,
-// the consumer loop of the batch-reduction weight-gradient GEMMs) and the host side of a tensor-core launch (workspace
-// check, tensor-map encoding, batch slices and ring depth of the weight-gradient kernels).
+// the consumer loop of the batch-reduction weight-gradient GEMMs, the row-chunk GEMMs of the dense-layer kernels) and the
+// host side of a tensor-core launch (workspace check, tensor-map encoding, batch slices and ring depth of the weight-gradient
+// kernels).
 #pragma once
 #include <cuda.h>
 
@@ -321,6 +322,111 @@ __device__ __forceinline__ void batch_reduce(float (&acc)[N / 2], Ring& ring, ui
   }
 }
 
+// Row-chunk GEMMs of the dense-layer kernels (residual unit, MMoE): 64 staged rows of an input of width DP (32 / 64 / 96 /
+// 128) times a chunk of HC hidden units, whose result stays in registers and feeds the next GEMM as A fragments.
+//   rows operand    [HC units x DP] K-major, streamed from a [2 R][DP] map (hi copy, then the lo copy R rows on);
+//   hidden operand  [DP x HC units] K-major, streamed from a [2 DP][R] map whose units are in perm8 order.
+namespace rows {
+
+constexpr int HC = 32;                       // hidden units per chunk: N of the row GEMMs, K of the hidden GEMMs
+constexpr int CHAIN = 32 / (HC / 8);         // hidden chunks per accumulation chain: 32 k-steps x 3 = 96 MMAs
+
+// The wgmma accumulator gives thread (g, t) columns 8c + 2t and 8c + 2t + 1 of each 8-column group c, and the A fragment of
+// k-step c wants columns 8c + t and 8c + t + 4.  Since a sum over k does not depend on its order, the fragment takes the
+// accumulator's two columns as its k = t and k = t + 4, and the hidden operand holds its units permuted within each group of
+// 8 to match: unit held at k position `k` is, within its group of 8, 2m for k = m < 4 and 2(m - 4) + 1 for k = m >= 4.
+__host__ __device__ __forceinline__ int perm8(int k) {
+  const int m = k & 7;
+  return (k & ~7) | (m < 4 ? 2 * m : 2 * m - 7);
+}
+
+__host__ __device__ constexpr int row_pitch(int DP) { return DP + 4; }   // staged rows: conflict-free A-fragment reads
+__host__ __device__ constexpr int stage_bytes(int DP) { return 2 * HC * DP * 4; }
+
+// TMA loads of chunk j (units j HC ..) into a stage (hi tile, then lo tile): a rows operand is DP / 32 boxes of [HC x 32]
+// per copy from a map of 2 R rows; a hidden operand one box of [DP x 32] per copy.
+template <int DP>
+__device__ __forceinline__ void load_rows_operand(uint32_t dst, const CUtensorMap* map, int j, int R, uint32_t bar) {
+#pragma unroll
+  for (int kb = 0; kb < DP / KB; ++kb) {
+    tma_load_2d(dst + kb * HC * 128, map, kb * KB, j * HC, bar);
+    tma_load_2d(dst + HC * DP * 4 + kb * HC * 128, map, kb * KB, R + j * HC, bar);
+  }
+}
+template <int DP>
+__device__ __forceinline__ void load_hidden_operand(uint32_t dst, const CUtensorMap* map, int j, uint32_t bar) {
+  tma_load_2d(dst, map, j * HC, 0, bar);
+  tma_load_2d(dst + DP * 128, map, j * HC, DP, bar);
+}
+
+// D[64 x HC] = R[64 x DP] . B: R = this warpgroup's 64 staged rows (pitch row_pitch(DP)), B = a rows-operand stage.
+// Issued one 32-column block (4 k-steps) at a time, so that only 32 fragment registers are live.
+template <int DP>
+__device__ __forceinline__ void gemm_rows(float (&d)[HC / 2], const float* rows, int r0, int t, uint32_t stage) {
+  constexpr int LD = row_pitch(DP);
+  const uint64_t bhi = gmma_desc_kmajor(stage, 128);
+  const uint64_t blo = gmma_desc_kmajor(stage + HC * DP * 4, 128);
+#pragma unroll
+  for (int kb = 0; kb < DP / KB; ++kb) {
+    uint32_t ah[4][4], al[4][4];
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) {
+      float a[4];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) a[q] = rows[(r0 + 8 * (q & 1)) * LD + kb * KB + 8 * ks + t + 4 * (q >> 1)];
+      tf32_split(a, ah[ks], al[ks]);
+    }
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks)
+      mma_3xtf32<HC>(d, ah[ks], al[ks], bhi, blo, (uint64_t)(kb * (HC * 128 / 16) + 2 * ks), (kb | ks) ? 1 : 0);
+    wgmma_commit();
+    wgmma_wait_keep(ah, al);
+  }
+}
+
+// A fragments of a hidden chunk held in accumulator layout: k-step c takes the thread's columns 8c + 2t (as k = t) and
+// 8c + 2t + 1 (as k = t + 4) of rows g and g + 8 -- the order perm8 gives the B operand.
+__device__ __forceinline__ void acc_to_a(const float (&v)[HC / 2], uint32_t (&hh)[HC / 8][4], uint32_t (&hl)[HC / 8][4]) {
+#pragma unroll
+  for (int c = 0; c < HC / 8; ++c) {
+    const float a[4] = {v[4 * c], v[4 * c + 2], v[4 * c + 1], v[4 * c + 3]};
+    tf32_split(a, hh[c], hl[c]);
+  }
+}
+
+// D[64 x DP] (+)= Hc[64 x HC] . B: Hc from acc_to_a, B = a hidden-operand stage; `start` begins a new chain.
+template <int DP>
+__device__ __forceinline__ void gemm_hidden(float (&d)[DP / 2], uint32_t (&hh)[HC / 8][4], uint32_t (&hl)[HC / 8][4],
+                                            uint32_t stage, bool start) {
+  const uint64_t bhi = gmma_desc_kmajor(stage, 128);
+  const uint64_t blo = gmma_desc_kmajor(stage + DP * 128, 128);
+  wgmma_fence();
+#pragma unroll
+  for (int c = 0; c < HC / 8; ++c) mma_3xtf32<DP>(d, hh[c], hl[c], bhi, blo, (uint64_t)(2 * c), (start && c == 0) ? 0 : 1);
+  wgmma_commit();
+  wgmma_wait_keep(hh, hl);
+}
+
+// Stages this warpgroup's 64 rows of a (B, d) tensor, zero padded to DP columns and past B, with ordinary loads (the rows
+// need not be 16-byte aligned); with `mask`, the rows of src [mask > 0] instead.
+template <int DP>
+__device__ __forceinline__ void stage_rows(float* dst, const float* __restrict__ src, const float* __restrict__ mask,
+                                           long long base, int B, int d, int tw) {
+  constexpr int LD = row_pitch(DP);
+  for (int idx = tw; idx < WG_M * DP; idx += 128) {
+    const int r = idx / DP, c = idx % DP;
+    float v = 0.f;
+    if (c < d && base + r < B) {
+      const size_t o = (size_t)(base + r) * d + c;
+      v = (mask == nullptr || __ldg(mask + o) > 0.f) ? __ldg(src + o) : 0.f;
+    }
+    dst[r * LD + c] = v;
+  }
+}
+
+}  // namespace rows
+
 // ------------------------------------------------------------------------------------------------ host
 constexpr size_t SMEM_CAP = 226 * 1024;     // dynamic shared memory per CTA on sm_90 (227 KB) less slack
 
@@ -384,6 +490,19 @@ static inline int stages_that_fit(size_t fixed, size_t stage) {
   const size_t sb = (SMEM_CAP - fixed) / stage;
   return (int)(sb < 4 ? sb : 4);
 }
+
+namespace rows {
+// Maps of the prepped operands at `base` (hi copy, then lo copy): rows operand [2 R][DP], boxes of [HC x 32]; hidden
+// operand [2 DP][R], boxes of [DP x 32].
+static inline int encode_rows_operand(const char* fn, CUtensorMap* map, const float* base, int DP, int64_t R) {
+  return encode_2d(fn, map, base, DP, 2 * R, KB, HC, CU_TENSOR_MAP_SWIZZLE_128B);
+}
+static inline int encode_hidden_operand(const char* fn, CUtensorMap* map, const float* base, int DP, int64_t R) {
+  return encode_2d(fn, map, base, R, 2 * DP, KB, DP, CU_TENSOR_MAP_SWIZZLE_128B);
+}
+// input width class of the row GEMMs: d rounded up to 32, 64, 96 or 128
+static inline int dp_class(int64_t d) { return d <= 32 ? 32 : d <= 64 ? 64 : d <= 96 ? 96 : 128; }
+}  // namespace rows
 
 }  // namespace tc
 }  // namespace ctr

@@ -327,6 +327,38 @@ def residual_unit(input: torch.Tensor, internal_dim=None, index=None) -> torch.T
     return autograd.residual_unit(input, w0, b0, w1, b1)
 
 
+# --------------------------------------------------------------------------------------------------- MMoE
+def mmoe_experts_gates(concat_all_input: torch.Tensor, num_experts, expert_hidden_units, num_tasks,
+                       return_gates: bool = False):
+    """MMoE experts, gates and gated sums -- MMOE/mmoe.py:207-236, one kernel each way: returns the ``num_tasks`` towers
+    ``sum_e softmax_e(x . gate_t)[e] relu(x . expert_e + bias_e)`` as contiguous (B, expert_hidden_units) tensors, and with
+    ``return_gates`` also the gate weights (the reference's ``gate_log``) as a list of (B, num_experts) tensors.
+
+    Creates, in the caller's scope, the variables of the reference's ``tf.layers.dense`` calls: ``experts/expert_{i}/kernel``
+    (d, expert_hidden_units) glorot-uniform and ``experts/expert_{i}/bias`` zeros for i < num_experts, then
+    ``gates/gate_{i}/kernel`` (d, num_experts) glorot-uniform and no bias for i < num_tasks -- gates are named by task
+    index, not by task name.  The three sizes go through ``int()``.  The variables are stacked into the packed (E,d,H),
+    (E,H) and (T,d,E) layout of the kernels on every call; torch.stack routes the gradients back to each variable."""
+    E, H, T = int(num_experts), int(expert_hidden_units), int(num_tasks)
+    d = int(concat_all_input.shape[-1])
+    zeros = lambda s: torch.zeros(s)
+    kernels, biases, gate_kernels = [], [], []
+    with variable_scope("experts"):
+        for i in range(E):
+            with variable_scope(f"expert_{i}"):
+                kernels.append(get_variable("kernel", (d, H)))
+                biases.append(get_variable("bias", (H,), initializer=zeros))
+    with variable_scope("gates"):
+        for i in range(T):
+            with variable_scope(f"gate_{i}"):
+                gate_kernels.append(get_variable("kernel", (d, E)))
+    towers, gates = autograd.mmoe(concat_all_input, torch.stack(kernels), torch.stack(biases), torch.stack(gate_kernels))
+    towers = list(towers.unbind(0))
+    if return_gates:
+        return towers, list(gates.unbind(0))
+    return towers
+
+
 # --------------------------------------------------------------------------------------------------- DIN loss-side term
 def mini_batch_aware_regularization(embedding_tensors, l2_lambda: float) -> torch.Tensor:
     """DIN/din.py:254-257 (SURVEY parity note 7): ``l2_lambda * tf.nn.l2_loss(concat(tensors, -1)) / batch`` -- an L2 on the

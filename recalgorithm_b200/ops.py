@@ -754,3 +754,49 @@ def residual_unit_bwd(x, w0, b0, w1, b1, out, g_out):
                                                 H, _ptr(d_x), _ptr(d_w0), _ptr(d_b0), _ptr(d_w1), _ptr(d_b1), _ptr(ws),
                                                 ws.numel(), _stream()))
     return d_x, d_w0, d_b0, d_w1, d_b1
+
+
+# ------------------------------------------------------------------------------------ MMoE expert-gate layer
+def mmoe_workspace(B: int, d: int, E: int, H: int, T: int, device) -> torch.Tensor:
+    """Caller-owned workspace: the prepped weights (B = 0, what the forward needs) plus, for the backward, the expert and
+    gate-logit gradients."""
+    nbytes = ctypes.c_int64(0)
+    _lib.check(_lib.lib().ctr_mmoe_workspace_bytes(B, d, E, H, T, ctypes.byref(nbytes)))
+    return torch.empty((int(nbytes.value),), dtype=torch.uint8, device=device)
+
+
+def _mmoe_args(x, w_experts, b_experts, w_gates):
+    _chk(x, F32, "concat_all_input")
+    if x.dim() != 2 or w_experts.dim() != 3 or w_gates.dim() != 3:
+        raise ValueError("mmoe: x (B,d), w_experts (E,d,H) and w_gates (T,d,E) expected")
+    B, d = x.shape
+    E, _, H = w_experts.shape
+    T = w_gates.shape[0]
+    _chk(w_experts, F32, "w_experts", (E, d, H)); _chk(b_experts, F32, "b_experts", (E, H))
+    _chk(w_gates, F32, "w_gates", (T, d, E))
+    return B, d, E, H, T
+
+
+def mmoe_fwd(x, w_experts, b_experts, w_gates):
+    """MMOE/mmoe.py:207-236: x (B,d), w_experts (E,d,H), b_experts (E,H), w_gates (T,d,E) -> (towers (T,B,H), gates (T,B,E)),
+    tower_t = sum_e softmax_e(x . w_gates[t])[e] relu(x . w_experts[e] + b_experts[e])."""
+    B, d, E, H, T = _mmoe_args(x, w_experts, b_experts, w_gates)
+    towers = torch.empty((T, B, H), dtype=F32, device=x.device)
+    gates = torch.empty((T, B, E), dtype=F32, device=x.device)
+    ws = mmoe_workspace(0, d, E, H, T, x.device)
+    _lib.check(_lib.lib().ctr_mmoe_fwd(_ptr(x), _ptr(w_experts), _ptr(b_experts), _ptr(w_gates), B, d, E, H, T, _ptr(towers),
+                                       _ptr(gates), _ptr(ws), ws.numel(), _stream()))
+    return towers, gates
+
+
+def mmoe_bwd(x, w_experts, b_experts, w_gates, gates, g_towers):
+    """Gradients of mmoe_fwd given its gates (T,B,E) and g_towers (T,B,H): (d_x, d_w_experts, d_b_experts, d_w_gates).
+    The expert outputs are recomputed from x."""
+    B, d, E, H, T = _mmoe_args(x, w_experts, b_experts, w_gates)
+    _chk(gates, F32, "gates", (T, B, E)); _chk(g_towers, F32, "g_towers", (T, B, H))
+    d_x, d_we, d_be, d_wg = (torch.empty_like(t) for t in (x, w_experts, b_experts, w_gates))
+    ws = mmoe_workspace(B, d, E, H, T, x.device)
+    _lib.check(_lib.lib().ctr_mmoe_bwd(_ptr(x), _ptr(w_experts), _ptr(b_experts), _ptr(w_gates), _ptr(gates), _ptr(g_towers),
+                                       B, d, E, H, T, _ptr(d_x), _ptr(d_we), _ptr(d_be), _ptr(d_wg), _ptr(ws), ws.numel(),
+                                       _stream()))
+    return d_x, d_we, d_be, d_wg

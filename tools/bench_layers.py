@@ -4,7 +4,7 @@
 Each kernel is timed alone with CUDA events; an L2 flush (a 256 MB write) runs between timed iterations because these
 working sets are flushed from the 50 MB L2.  Prints one JSON line per measurement.
 
-    python tools/bench_layers.py [--iters 20] [--only cin,dcn,din,fibinet]     (also: pairwise, bst, adam, pnn, dien, deepcrossing)
+    python tools/bench_layers.py [--iters 20] [--only cin,dcn,din,fibinet]     (also: pairwise, bst, adam, pnn, dien, deepcrossing, mmoe)
 """
 import argparse
 import json
@@ -260,6 +260,61 @@ def deepcrossing_rows(iters, flush, rn):
         torch.backends.cuda.matmul.allow_tf32 = prev_tf32
 
 
+
+def mmoe_rows(iters, flush, rn):
+    """MMoE expert-gate layer (ctr_mmoe_fwd / _bwd) at the reference shape d = 82, E = 3, H = 512, T = 3, B = 1024 and 65 536,
+    next to plain torch running the same block (fp32 einsum / softmax, TF32 disabled, autograd backward).  Floors from
+    data-sheet rates of the H100 SXM (700 W), not measured: FLOPs over the 67 TFLOP/s FP32 rate, the executed 3xTF32 FLOPs
+    (3 passes over DP = 96 inputs and R = E HP + 32 = 1568 units, plus the backward's hidden GEMMs and dW) over the
+    495 TFLOP/s TF32 rate, and x + towers + gates (forward) or x, gates, g, d_x and the dz | dlogit round trip (backward)
+    over 3.35 TB/s of HBM."""
+    d, E, H, T, DP = 82, 3, 512, 3, 96
+    R = E * H + 32
+    print(json.dumps({"mmoe_card": card()}), flush=True)
+
+    def torch_form(x, we, be, wg):
+        h = torch.relu(torch.einsum("bd,edh->ebh", x, we) + be[:, None, :])
+        p = torch.softmax(torch.einsum("bd,tde->tbe", x, wg), dim=-1)
+        return torch.einsum("tbe,ebh->tbh", p, h), p
+
+    prev_tf32 = torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cuda.matmul.allow_tf32 = False
+    try:
+        lim_e, lim_g = (6.0 / (d + H)) ** 0.5, (6.0 / (d + E)) ** 0.5
+        we = (torch.rand(E, d, H, device="cuda") * 2 - 1) * lim_e
+        be = rn(E, H, std=0.1)
+        wg = (torch.rand(T, d, E, device="cuda") * 2 - 1) * lim_g
+        for B in (1024, 65536):
+            x, g = rn(B, d, std=0.7), rn(T, B, H)
+            cfg = {"B": B, "d": d, "E": E, "H": H, "T": T}
+            fl_fwd = 2.0 * B * d * (E * H + T * E) + 2.0 * B * T * E * H
+            flops = {"fwd": fl_fwd, "bwd": 3 * fl_fwd}
+            tc = {"fwd": 3 * 2.0 * B * DP * R, "bwd": 3 * 2.0 * B * DP * (3 * R - 32)}   # dx: rows + hidden GEMMs; dW
+            hbm = {"fwd": B * (d + T * H + T * E) * 4, "bwd": B * (2 * d + T * E + T * H + 2 * R) * 4}
+            towers, gates = ops.mmoe_fwd(x, we, be, wg)
+            grads = ops.mmoe_bwd(x, we, be, wg, gates, g)
+            ps = [t.clone().requires_grad_() for t in (x, we, be, wg)]
+            ref_towers, _ = torch_form(*ps)
+            ref_grads = torch.autograd.grad(ref_towers, ps, g, retain_graph=True)
+            diff = {"fwd": float((ref_towers.detach() - towers).abs().max() / ref_towers.detach().abs().max()),
+                    "bwd": max(float((a - b).abs().max() / b.abs().max()) for a, b in zip(grads, ref_grads))}
+            runs = {"fwd": (lambda: ops.mmoe_fwd(x, we, be, wg), lambda: torch_form(x, we, be, wg)),
+                    "bwd": (lambda: ops.mmoe_bwd(x, we, be, wg, gates, g),
+                            lambda: torch.autograd.grad(ref_towers, ps, g, retain_graph=True))}
+            for way in ("fwd", "bwd"):
+                m, bst = timeit(runs[way][0], iters, flush)
+                tm, tbst = timeit(runs[way][1], iters, flush)
+                print(json.dumps({
+                    "kernel": f"mmoe_{way}", "config": cfg, "ms_median": m, "ms_best": bst,
+                    "torch_fp32_ms_median": tm, "torch_fp32_ms_best": tbst, "speedup_vs_torch": tm / m,
+                    "max_norm_rel_diff_vs_torch": diff[way], "l2": "flushed between iterations",
+                    "floor_fp32_us": flops[way] / 67e12 * 1e6, "floor_3xtf32_us": tc[way] / 495e12 * 1e6,
+                    "floor_hbm_us": hbm[way] / 3.35e12 * 1e6,
+                    "note": "floors are data-sheet rates (H100 SXM, 700 W), not measured; torch: same block, fp32, TF32 off"}),
+                    flush=True)
+    finally:
+        torch.backends.cuda.matmul.allow_tf32 = prev_tf32
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=20)
@@ -438,6 +493,8 @@ def main():
         dien_rows(args.iters, flush, hbm)
     if "deepcrossing" in only:  # DeepCrossing residual unit at the reference width (d = 82) and both result.md H; not in the default list
         deepcrossing_rows(args.iters, flush, rn)
+    if "mmoe" in only:  # MMoE expert-gate layer at the reference shape (d = 82, E = 3, H = 512, T = 3); not in the default list
+        mmoe_rows(args.iters, flush, rn)
 
 
 if __name__ == "__main__" and "--configs" not in sys.argv:

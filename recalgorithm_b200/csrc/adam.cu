@@ -14,7 +14,7 @@
 //   ctr_adam_dense_rest  streams over ALL other rows with g = 0: m*=b1, v*=b2, var -= lr_t*m/(sqrt(v)+eps)   (TF variant only)
 // so the faithful variant costs 6 table-sized streams per step (77 GB at config 5 -> ~12 ms at HBM peak, 40x the hot
 // path itself) and the lazy variant a few hundred MB.
-#include "ctr_common.cuh"
+#include "lookup_bwd.cuh"
 
 namespace ctr {
 
@@ -198,8 +198,8 @@ __device__ __forceinline__ void adam_apply(float4& w, float4& mm, float4& vv, co
   w.z -= lr_t * mm.z / (sqrtf(vv.z) + eps); w.w -= lr_t * mm.w / (sqrtf(vv.w) + eps);
 }
 
-// warp per sample; HOLD float4 per lane cover the sample's F*LPR chunks (F*D <= HOLD*128 floats); GK chunks are in flight
-// together in the update phase (d_tile, m, v, var loads issued before the first use).
+// The register-resident lookup backward of lookup_bwd.cuh (HOLD > 0) with the Adam update as its sink; GK chunks are in
+// flight together in the update phase (d_tile, m, v, var loads issued before the first use).
 template <int LPR, int HOLD>
 __global__ void __launch_bounds__(256, 1)
 embed_fm2_bwd_adam_kernel(const float4* __restrict__ tile, const float4* __restrict__ d_tile, const float* __restrict__ d_fm2,
@@ -209,7 +209,6 @@ embed_fm2_bwd_adam_kernel(const float4* __restrict__ tile, const float4* __restr
                           float lr_t, float b1, float b2, float eps, unsigned int* __restrict__ touched,
                           long long* __restrict__ n_unique) {
   constexpr int GK = HOLD < 4 ? HOLD : 4;
-  const unsigned full = 0xffffffffu;
   const int lane = threadIdx.x & 31;
   const int warp0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
@@ -223,28 +222,16 @@ embed_fm2_bwd_adam_kernel(const float4* __restrict__ tile, const float4* __restr
     float4 e[HOLD];
     long long row[HOLD];
 #pragma unroll
-    for (int k = 0; k < HOLD; ++k) {
-      const int j = k * 32 + lane;
-      e[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-      row[k] = -1;
-      if (j < n4) {
-        e[k] = ldg_stream_f4(e_row + j);
-        const int f = j / LPR;
-        const long long id = __ldg(ids + (size_t)b * F + f), lo = __ldg(row_off + f);
-        if (id >= 0 && id < __ldg(row_off + f + 1) - lo) row[k] = lo + id;
-      }
-    }
+    for (int k = 0; k < HOLD; ++k) row[k] = -1;
+    load_tile_row(e, e_row, n4, lane, [&](int k, int j) {
+      const int f = j / LPR;
+      const long long id = __ldg(ids + (size_t)b * F + f), lo = __ldg(row_off + f);
+      if (id >= 0 && id < __ldg(row_off + f + 1) - lo) row[k] = lo + id;
+    });
     int s[HOLD];
 #pragma unroll
     for (int k = 0; k < HOLD; ++k) s[k] = row[k] >= 0 ? __ldg(slot + row[k]) : -1;   // read-only during this launch for non-dup rows' peers
-    float4 S = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-    for (int k = 0; k < HOLD; ++k) { S.x += e[k].x; S.y += e[k].y; S.z += e[k].z; S.w += e[k].w; }
-#pragma unroll
-    for (int o = LPR; o < 32; o <<= 1) {
-      S.x += __shfl_xor_sync(full, S.x, o); S.y += __shfl_xor_sync(full, S.y, o);
-      S.z += __shfl_xor_sync(full, S.z, o); S.w += __shfl_xor_sync(full, S.w, o);
-    }
+    const float4 S = tile_row_sum<LPR>(e);
 #pragma unroll
     for (int k0 = 0; k0 < HOLD; k0 += GK) {
       float4 dt[GK], mm[GK], vv[GK], ww[GK];
@@ -262,9 +249,7 @@ embed_fm2_bwd_adam_kernel(const float4* __restrict__ tile, const float4* __restr
       for (int u = 0; u < GK; ++u) {
         const int k = k0 + u, j = k * 32 + lane;
         if (k >= HOLD || row[k] < 0) continue;
-        float4 r;
-        r.x = dt[u].x + g * (S.x - e[k].x); r.y = dt[u].y + g * (S.y - e[k].y);
-        r.z = dt[u].z + g * (S.z - e[k].z); r.w = dt[u].w + g * (S.w - e[k].w);
+        const float4 r = fm2_row_grad(dt[u], make_float4(g, g, g, g), S, e[k]);
         const int entry = b * F + j / LPR;
         if (!(s[k] & DUP_FLAG)) {
           const size_t o = (size_t)row[k] * LPR + c, so = (size_t)row[k] * SS + c;
@@ -283,7 +268,7 @@ embed_fm2_bwd_adam_kernel(const float4* __restrict__ tile, const float4* __restr
     }
   }
   if (n_unique != nullptr) {
-    mine = __reduce_add_sync(full, mine);
+    mine = __reduce_add_sync(0xffffffffu, mine);
     if (lane == 0 && mine) atomicAdd(reinterpret_cast<unsigned long long*>(n_unique), (unsigned long long)mine);
   }
 }
@@ -455,42 +440,6 @@ extern "C" int ctr_adam_rows_dedup(float* var, float* m, float* v, int64_t state
                            touched_bitmap, n_unique, as_stream(stream));
 }
 
-template <int LPR, int HOLD>
-static int launch_bwd_adam(const float* tile, const float* d_tile, const float* d_fm2, const EntrySrc& src, int64_t B, int64_t F,
-                           float* var, float* m, float* v, int SS, int32_t* slot, float* dup_grads, int32_t* dup_list, float lr_t, float b1,
-                           float b2, float eps, uint32_t* touched, int64_t* n_unique, cudaStream_t st) {
-  const char* fn = "ctr_embed_fm2_bwd_adam";
-  int* n_dup = dup_list + B * F;
-  int rc = launch_resident(fn, embed_fm2_bwd_adam_kernel<LPR, HOLD>, (B + 7) / 8, 256, 0, st, reinterpret_cast<const float4*>(tile),
-                           reinterpret_cast<const float4*>(d_tile), d_fm2, src.off, src.ids, (int)B, (int)F,
-                           reinterpret_cast<float4*>(var), reinterpret_cast<float4*>(m), reinterpret_cast<float4*>(v), SS, slot,
-                           reinterpret_cast<float4*>(dup_grads), dup_list, n_dup, lr_t, b1, b2, eps, touched,
-                           reinterpret_cast<long long*>(n_unique));
-  if (rc) return rc;
-  const int g2 = sm_count() * 2;
-  rc = launch(fn, adam_dup_merge_kernel<LPR>, g2, 256, 0, st, src, slot, reinterpret_cast<float4*>(dup_grads), dup_list, n_dup);
-  if (rc) return rc;
-  return launch(fn, adam_dup_update_kernel<LPR>, g2, 256, 0, st, reinterpret_cast<float4*>(var), reinterpret_cast<float4*>(m),
-                reinterpret_cast<float4*>(v), SS, src, slot, reinterpret_cast<const float4*>(dup_grads), dup_list, n_dup, lr_t, b1, b2,
-                eps, touched, reinterpret_cast<long long*>(n_unique));
-}
-
-template <int LPR>
-static int dispatch_bwd_adam(const float* tile, const float* d_tile, const float* d_fm2, const EntrySrc& src, int64_t B, int64_t F,
-                             float* var, float* m, float* v, int SS, int32_t* slot, float* dup_grads, int32_t* dup_list, float lr_t, float b1,
-                             float b2, float eps, uint32_t* touched, int64_t* n_unique, cudaStream_t st) {
-  const int64_t per_lane = (F * LPR + 31) / 32;
-  if (per_lane > 12) {
-    set_error("ctr_embed_fm2_bwd_adam: F*D = %lld exceeds the register-resident limit of 1536 (use ctr_embed_fm2_bwd + ctr_adam_indexed_slices)",
-              (long long)(F * LPR * 4));
-    return CTR_ERR_UNSUPPORTED;
-  }
-  return with_const<4, 8, 12>(per_lane <= 4 ? 4 : per_lane <= 8 ? 8 : 12, [&](auto H) {
-    return launch_bwd_adam<LPR, H>(tile, d_tile, d_fm2, src, B, F, var, m, v, SS, slot, dup_grads, dup_list, lr_t, b1, b2, eps, touched,
-                                   n_unique, st);
-  });
-}
-
 extern "C" int ctr_embed_fm2_bwd_adam(const float* tile, const float* d_tile, const float* d_fm2, const int64_t* field_row_offset,
                                       const int64_t* ids, int64_t B, int64_t F, int64_t D, float* var, float* m, float* v,
                                       int64_t state_stride, int32_t* slot_of_row, float* dup_grads, int32_t* dup_list, float lr_t, float beta1, float beta2,
@@ -511,8 +460,25 @@ extern "C" int ctr_embed_fm2_bwd_adam(const float* tile, const float* d_tile, co
   rc = launch("ctr_embed_fm2_bwd_adam", adam_claim_dup_kernel, capped_grid((n + 255) / 256, (long long)sm_count() * 16), 256, 0, st, src,
               n, slot_of_row);
   if (rc) return rc;
-  return with_lpr(D, [&](auto L) {
-    return dispatch_bwd_adam<L>(tile, d_tile, d_fm2, src, B, F, var, m, v, (int)(state_stride / 4), slot_of_row, dup_grads, dup_list,
-                                lr_t, beta1, beta2, eps, touched_bitmap, n_unique, st);
+  const char* fn = "ctr_embed_fm2_bwd_adam";
+  const int SS = (int)(state_stride / 4);
+  int* n_dup = dup_list + n;
+  auto* dg = reinterpret_cast<float4*>(dup_grads);
+  auto* var4 = reinterpret_cast<float4*>(var);
+  auto* m4 = reinterpret_cast<float4*>(m);
+  auto* v4 = reinterpret_cast<float4*>(v);
+  auto* uniq = reinterpret_cast<long long*>(n_unique);
+  return with_lpr(D, [&](auto LPR) {
+    return with_hold<false>(F, LPR, [&](auto HOLD) {
+      int r = launch_resident(fn, embed_fm2_bwd_adam_kernel<LPR, HOLD>, (B + 7) / 8, 256, 0, st, reinterpret_cast<const float4*>(tile),
+                              reinterpret_cast<const float4*>(d_tile), d_fm2, src.off, src.ids, (int)B, (int)F, var4, m4, v4, SS,
+                              slot_of_row, dg, dup_list, n_dup, lr_t, beta1, beta2, eps, touched_bitmap, uniq);
+      if (r) return r;
+      const int g2 = sm_count() * 2;
+      r = launch(fn, adam_dup_merge_kernel<LPR>, g2, 256, 0, st, src, slot_of_row, dg, dup_list, n_dup);
+      if (r) return r;
+      return launch(fn, adam_dup_update_kernel<LPR>, g2, 256, 0, st, var4, m4, v4, SS, src, slot_of_row,
+                    static_cast<const float4*>(dg), dup_list, n_dup, lr_t, beta1, beta2, eps, touched_bitmap, uniq);
+    }, fn, " (use ctr_embed_fm2_bwd + ctr_adam_indexed_slices)");
   });
 }

@@ -14,11 +14,9 @@
 //   128-bit loads in flight per lane (enough outstanding bytes per SM to cover HBM latency).
 //   S = sum_f e and Q = sum_f e^2 accumulate in registers; the FM2 logit is a shuffle reduction.
 //   The (B,F,D) tile is written with evict-first stores so it does not displace hot table rows in L2.
-#include "ctr_common.cuh"
+#include "lookup_bwd.cuh"
 
 namespace ctr {
-
-__device__ __forceinline__ float4 f4_zero() { return make_float4(0.f, 0.f, 0.f, 0.f); }
 
 // Row-sharded tables (SURVEY 8e): global row gr lives on rank gr % G at local row gr / G (G a power of two <= 8).
 // `base[r]` is rank r's shard as seen from THIS GPU (peer-mapped over NVLink for r != my rank), so the gather pulls
@@ -143,150 +141,48 @@ embed_fm2_fwd_kernel(const float4* __restrict__ table, const PeerTables peers, c
   }
 }
 
-// Backward: row_grads[b,f,:] = d_tile[b,f,:] + g[b] * (S[b,:] - e[b,f,:]).
-// HOLD > 0: the sample's tile row (F*D fp32 <= HOLD*128 floats) stays in registers between the S pass and
-// the gradient pass; HOLD == 0: generic two-pass variant (second pass re-reads through L1/L2).
-// BI: d_fm2 is the (B, D) gradient of the bi-interaction vector (g becomes per-dimension).
-template <int LPR, int HOLD, bool BI = false>
-__global__ void __launch_bounds__(256)
-embed_fm2_bwd_kernel(const float4* __restrict__ tile, const float4* __restrict__ d_tile,
-                     const float* __restrict__ d_fm2, int B, int F, float4* __restrict__ row_grads) {
-  const unsigned full = 0xffffffffu;
+// Backward: row_grads[b,f,:] = d_tile[b,f,:] + g[b] * (S[b,:] - e[b,f,:]), the per-sample body of lookup_bwd.cuh.
+// FM2_BI: d_fm2 is the (B, D) gradient of the bi-interaction vector (g becomes per-dimension).
+// FM2_LIN (HOLD > 0 only): the backward of the fused dense(1) head, d_tile carries wlin (F*D) and d_wlin = sum_b d_lin[b]*e[b]
+// is accumulated (LinHead); row_grads[b,f,:] = d_lin[b]*wlin[f,:] + d_fm2[b]*(S[b,:] - e[b,f,:]).
+enum { FM2_PLAIN, FM2_BI, FM2_LIN };
+
+struct StoreRow {
+  float4* __restrict__ o_row;
+  __device__ __forceinline__ void fetch(int, int) {}
+  __device__ __forceinline__ void operator()(int, int j, const float4& r) { stg_stream_f4(o_row + j, r); }
+};
+
+// LIN asks for 2 CTAs per SM; the plain and BI forms set no floor, so ptxas keeps their register count low.
+template <int LPR, int HOLD, int MODE>
+__global__ void __launch_bounds__(256, MODE == FM2_LIN ? 2 : 0)
+embed_fm2_bwd_kernel(const float4* __restrict__ tile, const float4* __restrict__ d_tile, const float* __restrict__ d_fm2,
+                     const float* __restrict__ d_lin, int B, int F, float4* __restrict__ row_grads, float4* __restrict__ d_wlin) {
+  extern __shared__ float4 s_lin[];
   const int lane = threadIdx.x & 31;
   const int warp0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
-  const int n4 = F * LPR;                                     // float4 per sample; chunk of element j is j % LPR == lane % LPR
-
+  const int n4 = F * LPR;
+  LinHead<MODE == FM2_LIN ? HOLD : 1> lin;
+  if (MODE == FM2_LIN) lin.stage(s_lin, d_tile, n4);
   for (int b = warp0; b < B; b += nwarps) {
-    const float4* e_row = tile + (size_t)b * n4;
-    float4* o_row = row_grads + (size_t)b * n4;
-    const float4* dt_row = d_tile ? d_tile + (size_t)b * n4 : nullptr;
+    StoreRow sink{row_grads + (size_t)b * n4};
+    RowGrad rows{d_tile ? d_tile + (size_t)b * n4 : nullptr};   // not read in LIN mode
     float4 g4;
-    if (BI) {
+    if (MODE == FM2_BI) {
       g4 = __ldg(reinterpret_cast<const float4*>(d_fm2) + (size_t)b * LPR + lane % LPR);
     } else {
       const float g = d_fm2 ? __ldg(d_fm2 + b) : 0.f;
       g4 = make_float4(g, g, g, g);
     }
-    float4 S = f4_zero();
-    if (HOLD > 0) {
-      constexpr int H = HOLD > 0 ? HOLD : 1;
-      float4 e[H];
-#pragma unroll
-      for (int k = 0; k < H; ++k) {
-        const int j = k * 32 + lane;
-        e[k] = f4_zero();
-        if (j < n4) e[k] = ldg_stream_f4(e_row + j);
-      }
-      float4 dt[H];
-#pragma unroll
-      for (int k = 0; k < H; ++k) {
-        const int j = k * 32 + lane;
-        dt[k] = f4_zero();
-        if (dt_row != nullptr && j < n4) dt[k] = ldg_stream_f4(dt_row + j);
-      }
-#pragma unroll
-      for (int k = 0; k < H; ++k) { S.x += e[k].x; S.y += e[k].y; S.z += e[k].z; S.w += e[k].w; }
-#pragma unroll
-      for (int o = LPR; o < 32; o <<= 1) {
-        S.x += __shfl_xor_sync(full, S.x, o); S.y += __shfl_xor_sync(full, S.y, o);
-        S.z += __shfl_xor_sync(full, S.z, o); S.w += __shfl_xor_sync(full, S.w, o);
-      }
-#pragma unroll
-      for (int k = 0; k < H; ++k) {
-        const int j = k * 32 + lane;
-        if (j < n4) {
-          float4 r;
-          r.x = dt[k].x + g4.x * (S.x - e[k].x); r.y = dt[k].y + g4.y * (S.y - e[k].y);
-          r.z = dt[k].z + g4.z * (S.z - e[k].z); r.w = dt[k].w + g4.w * (S.w - e[k].w);
-          stg_stream_f4(o_row + j, r);
-        }
-      }
+    if constexpr (MODE == FM2_LIN) {
+      lin.gl = d_lin ? __ldg(d_lin + b) : 0.f;
+      lookup_bwd_sample<LPR, HOLD>(tile + (size_t)b * n4, n4, lane, g4, lin, sink);
     } else {
-      for (int j = lane; j < n4; j += 32) {
-        const float4 v = __ldg(e_row + j);
-        S.x += v.x; S.y += v.y; S.z += v.z; S.w += v.w;
-      }
-#pragma unroll
-      for (int o = LPR; o < 32; o <<= 1) {
-        S.x += __shfl_xor_sync(full, S.x, o); S.y += __shfl_xor_sync(full, S.y, o);
-        S.z += __shfl_xor_sync(full, S.z, o); S.w += __shfl_xor_sync(full, S.w, o);
-      }
-      for (int j = lane; j < n4; j += 32) {
-        const float4 v = __ldg(e_row + j);
-        float4 r = dt_row ? ldg_stream_f4(dt_row + j) : f4_zero();
-        r.x += g4.x * (S.x - v.x); r.y += g4.y * (S.y - v.y); r.z += g4.z * (S.z - v.z); r.w += g4.w * (S.w - v.w);
-        stg_stream_f4(o_row + j, r);
-      }
+      lookup_bwd_sample<LPR, HOLD>(tile + (size_t)b * n4, n4, lane, g4, rows, sink);
     }
   }
-}
-
-// Backward of the LIN form: d_tile is the rank-1 product d_lin[b] * wlin[f,d], so it is never materialised:
-//   row_grads[b,f,:] = d_lin[b]*wlin[f,:] + d_fm2[b]*(S[b,:] - e[b,f,:]) ;  d_wlin[f,:] = sum_b d_lin[b]*e[b,f,:].
-// Warp per sample; the tile row and the warp's share of d_wlin live in registers (HOLD float4 each), wlin in shared memory;
-// per CTA one shared-memory reduction and one vector red.global.add per element.  Reads (tile), writes (row_grads) only.
-template <int LPR, int HOLD>
-__global__ void __launch_bounds__(256, 2)
-embed_fm2_lin_bwd_kernel(const float4* __restrict__ tile, const float4* __restrict__ wlin, const float* __restrict__ d_fm2,
-                         const float* __restrict__ d_lin, int B, int F, float4* __restrict__ row_grads,
-                         float4* __restrict__ d_wlin) {
-  extern __shared__ float4 s_lin[];                 // [n4] wlin, then [n4] d_wlin accumulator
-  const unsigned full = 0xffffffffu;
-  const int lane = threadIdx.x & 31;
-  const int warp0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int nwarps = (gridDim.x * blockDim.x) >> 5;
-  const int n4 = F * LPR;
-  float4* s_w = s_lin;
-  float4* s_dw = s_lin + n4;
-  for (int j = threadIdx.x; j < n4; j += blockDim.x) { s_w[j] = __ldg(wlin + j); s_dw[j] = f4_zero(); }
-  __syncthreads();
-  float4 acc[HOLD];
-#pragma unroll
-  for (int k = 0; k < HOLD; ++k) acc[k] = f4_zero();
-  for (int b = warp0; b < B; b += nwarps) {
-    const float4* e_row = tile + (size_t)b * n4;
-    float4* o_row = row_grads + (size_t)b * n4;
-    const float g = d_fm2 ? __ldg(d_fm2 + b) : 0.f;
-    const float gl = d_lin ? __ldg(d_lin + b) : 0.f;
-    float4 e[HOLD];
-#pragma unroll
-    for (int k = 0; k < HOLD; ++k) {
-      const int j = k * 32 + lane;
-      e[k] = f4_zero();
-      if (j < n4) e[k] = ldg_stream_f4(e_row + j);
-    }
-    float4 S = f4_zero();
-#pragma unroll
-    for (int k = 0; k < HOLD; ++k) { S.x += e[k].x; S.y += e[k].y; S.z += e[k].z; S.w += e[k].w; }
-#pragma unroll
-    for (int o = LPR; o < 32; o <<= 1) {
-      S.x += __shfl_xor_sync(full, S.x, o); S.y += __shfl_xor_sync(full, S.y, o);
-      S.z += __shfl_xor_sync(full, S.z, o); S.w += __shfl_xor_sync(full, S.w, o);
-    }
-#pragma unroll
-    for (int k = 0; k < HOLD; ++k) {
-      const int j = k * 32 + lane;
-      if (j < n4) {
-        const float4 w = s_w[j];
-        float4 r;
-        r.x = gl * w.x + g * (S.x - e[k].x); r.y = gl * w.y + g * (S.y - e[k].y);
-        r.z = gl * w.z + g * (S.z - e[k].z); r.w = gl * w.w + g * (S.w - e[k].w);
-        stg_stream_f4(o_row + j, r);
-        acc[k].x += gl * e[k].x; acc[k].y += gl * e[k].y; acc[k].z += gl * e[k].z; acc[k].w += gl * e[k].w;
-      }
-    }
-  }
-#pragma unroll
-  for (int k = 0; k < HOLD; ++k) {
-    const int j = k * 32 + lane;
-    if (j < n4) {
-      atomicAdd(&s_dw[j].x, acc[k].x); atomicAdd(&s_dw[j].y, acc[k].y);
-      atomicAdd(&s_dw[j].z, acc[k].z); atomicAdd(&s_dw[j].w, acc[k].w);
-    }
-  }
-  __syncthreads();
-  for (int j = threadIdx.x; j < n4; j += blockDim.x) atomicAdd(d_wlin + j, s_dw[j]);
+  if (MODE == FM2_LIN) lin.flush(d_wlin, lane);
 }
 
 // grad_table[row(b,f), :] += row_grads[b,f,:]  (valid ids only) -- vector red.global.add.
@@ -404,22 +300,18 @@ static int launch_fwd(const float* table, const PeerTables* peers, const int64_t
   return peers != nullptr ? go(embed_fm2_fwd_kernel<LPR, true, 1, false, IdT>) : go(embed_fm2_fwd_kernel<LPR, false, 4, false, IdT>);
 }
 
-template <int LPR, int HOLD, bool BI = false>
-static int launch_bwd(const float* tile, const float* d_tile, const float* d_fm2, int64_t B, int64_t F,
-                      float* row_grads, cudaStream_t st) {
-  return launch_resident("ctr_embed_fm2_bwd", embed_fm2_bwd_kernel<LPR, HOLD, BI>, (B + 7) / 8, 256, 0, st,
-                         reinterpret_cast<const float4*>(tile), reinterpret_cast<const float4*>(d_tile), d_fm2, (int)B, (int)F,
-                         reinterpret_cast<float4*>(row_grads));
-}
-
-template <int LPR, bool BI = false>
-static int dispatch_bwd(const float* tile, const float* d_tile, const float* d_fm2, int64_t B, int64_t F,
-                        float* row_grads, cudaStream_t st) {
-  const int64_t per_lane = (F * LPR + 31) / 32;
-  if (per_lane <= 4) return launch_bwd<LPR, 4, BI>(tile, d_tile, d_fm2, B, F, row_grads, st);
-  if (per_lane <= 8) return launch_bwd<LPR, 8, BI>(tile, d_tile, d_fm2, B, F, row_grads, st);
-  if (per_lane <= 12) return launch_bwd<LPR, 12, BI>(tile, d_tile, d_fm2, B, F, row_grads, st);
-  return launch_bwd<LPR, 0, BI>(tile, d_tile, d_fm2, B, F, row_grads, st);
+// FM2_LIN has no two-pass form: wider rows fail in with_hold with `what` in the message.
+template <int MODE>
+static int launch_bwd(const char* what, const float* tile, const float* d_tile, const float* d_fm2, const float* d_lin, int64_t B,
+                      int64_t F, int64_t D, float* row_grads, float* d_wlin, cudaStream_t st) {
+  return with_lpr(D, [&](auto LPR) {
+    return with_hold<MODE != FM2_LIN>(F, LPR, [&](auto HOLD) {
+      return launch_resident(what, embed_fm2_bwd_kernel<LPR, HOLD, MODE>, (B + 7) / 8, 256,
+                             MODE == FM2_LIN ? sizeof(float4) * 2 * (size_t)F * LPR : 0, st, reinterpret_cast<const float4*>(tile),
+                             reinterpret_cast<const float4*>(d_tile), d_fm2, d_lin, (int)B, (int)F,
+                             reinterpret_cast<float4*>(row_grads), reinterpret_cast<float4*>(d_wlin));
+    }, what);
+  });
 }
 
 template <int LPR>
@@ -527,8 +419,7 @@ extern "C" int ctr_embed_fm2_bwd(const float* tile, const float* d_tile, const f
   CTR_REQUIRE(aligned16(tile) && aligned16(d_tile) && aligned16(row_grads),
               "ctr_embed_fm2_bwd: tile, d_tile and row_grads must be 16-byte aligned");
   if (B == 0) return CTR_OK;
-  cudaStream_t st = as_stream(stream);
-  return with_lpr(D, [&](auto LPR) { return dispatch_bwd<LPR>(tile, d_tile, d_fm2, B, F, row_grads, st); });
+  return launch_bwd<FM2_PLAIN>("ctr_embed_fm2_bwd", tile, d_tile, d_fm2, nullptr, B, F, D, row_grads, nullptr, as_stream(stream));
 }
 
 extern "C" int ctr_embed_scatter_add(float* grad_table, const int64_t* field_row_offset, const int64_t* ids,
@@ -608,8 +499,7 @@ extern "C" int ctr_embed_bi_bwd(const float* tile, const float* d_tile, const fl
   CTR_REQUIRE(aligned16(tile) && aligned16(d_tile) && aligned16(d_bi) && aligned16(row_grads),
               "ctr_embed_bi_bwd: tile, d_tile, d_bi and row_grads must be 16-byte aligned");
   if (B == 0) return CTR_OK;
-  cudaStream_t st = as_stream(stream);
-  return with_lpr(D, [&](auto LPR) { return dispatch_bwd<LPR, true>(tile, d_tile, d_bi, B, F, row_grads, st); });
+  return launch_bwd<FM2_BI>("ctr_embed_fm2_bwd", tile, d_tile, d_bi, nullptr, B, F, D, row_grads, nullptr, as_stream(stream));
 }
 
 // ---- lookup + FM2 + fused dense(1) head over the flattened tile (e2e form: the consumer does not re-stream the tile) ------
@@ -663,26 +553,6 @@ extern "C" int ctr_embed_fm2_lin_fwd_sharded(const float* const* shard_ptrs, int
   return dispatch_fwd_lin(nullptr, &peers, field_row_offset, reinterpret_cast<const long long*>(ids), B, F, D, tile, fm2, nullptr, wlin, lin, st);
 }
 
-template <int LPR, int HOLD>
-static int launch_lin_bwd(const float* tile, const float* wlin, const float* d_fm2, const float* d_lin, int64_t B, int64_t F,
-                          float* row_grads, float* d_wlin, cudaStream_t st) {
-  return launch_resident("ctr_embed_fm2_lin_bwd", embed_fm2_lin_bwd_kernel<LPR, HOLD>, (B + 7) / 8, 256,
-                         sizeof(float4) * 2 * (size_t)F * LPR, st, reinterpret_cast<const float4*>(tile),
-                         reinterpret_cast<const float4*>(wlin), d_fm2, d_lin, (int)B, (int)F, reinterpret_cast<float4*>(row_grads),
-                         reinterpret_cast<float4*>(d_wlin));
-}
-
-template <int LPR>
-static int dispatch_lin_bwd(const float* tile, const float* wlin, const float* d_fm2, const float* d_lin, int64_t B, int64_t F,
-                            float* row_grads, float* d_wlin, cudaStream_t st) {
-  const int64_t per_lane = (F * LPR + 31) / 32;
-  if (per_lane <= 4) return launch_lin_bwd<LPR, 4>(tile, wlin, d_fm2, d_lin, B, F, row_grads, d_wlin, st);
-  if (per_lane <= 8) return launch_lin_bwd<LPR, 8>(tile, wlin, d_fm2, d_lin, B, F, row_grads, d_wlin, st);
-  if (per_lane <= 12) return launch_lin_bwd<LPR, 12>(tile, wlin, d_fm2, d_lin, B, F, row_grads, d_wlin, st);
-  set_error("ctr_embed_fm2_lin_bwd: F*D = %lld exceeds the register-resident limit of 1536", (long long)(F * LPR * 4));
-  return CTR_ERR_UNSUPPORTED;
-}
-
 extern "C" int ctr_embed_fm2_lin_bwd(const float* tile, const float* wlin, const float* d_fm2, const float* d_lin, int64_t B,
                                      int64_t F, int64_t D, float* row_grads, float* d_wlin, void* stream) {
   int rc = check_bfd("ctr_embed_fm2_lin_bwd", B, F, D);
@@ -693,7 +563,7 @@ extern "C" int ctr_embed_fm2_lin_bwd(const float* tile, const float* wlin, const
   cudaStream_t st = as_stream(stream);
   CTR_CUDA(cudaMemsetAsync(d_wlin, 0, sizeof(float) * F * D, st));
   if (B == 0) return CTR_OK;
-  return with_lpr(D, [&](auto LPR) { return dispatch_lin_bwd<LPR>(tile, wlin, d_fm2, d_lin, B, F, row_grads, d_wlin, st); });
+  return launch_bwd<FM2_LIN>("ctr_embed_fm2_lin_bwd", tile, wlin, d_fm2, d_lin, B, F, D, row_grads, d_wlin, st);
 }
 
 // ---- sequence lookup: (B, T) ids into ONE table -> (B, T, D), zero rows for id -1 / out of range (the zero padding of

@@ -20,7 +20,7 @@
 // Measured link ceilings for this access pattern (tools/peerbench.cu, all ranks active at once, 128-byte rows): pull
 // 650 GB/s with L1-allocating loads (622 with .nc.L1::no_allocate), push 680-690 GB/s with plain 128-bit stores, per
 // direction per rank; random rows == sequential rows, bulk-async (TMA) copies == LDG/STG, 8 GB == 32 GB shards.
-#include "ctr_common.cuh"
+#include "lookup_bwd.cuh"
 
 namespace ctr {
 
@@ -125,112 +125,57 @@ __device__ __forceinline__ float4* queue_slot(const PeerQueues& q, size_t qbase,
   return q.vals[word >> PLAN_SLOT_BITS] + (qbase + (size_t)(word & PLAN_SLOT_MASK)) * lpr + c;
 }
 
-// Lookup backward fused with the gradient exchange (arithmetic of embed_fm2_bwd_kernel): warp per sample, the sample's
-// tile row is held in registers between the S pass and the gradient pass (HOLD float4 per lane; HOLD == 0 = generic
-// two-pass form); every finished 128-bit piece goes to owner.vals[(my_rank*capacity + slot)*LPR + c].
-// LIN (HOLD > 0 only): the upstream gradient of the tile is the rank-1 product d_lin[b]*wlin[f,d] of a fused dense(1) head
-// (ctr_embed_fm2_lin_fwd): d_tile is not read, `d_tile` carries wlin (F*D) instead, and d_wlin = sum_b d_lin[b]*e[b] is
-// accumulated in registers (per CTA one shared-memory reduction + one vector red.global.add per element).
+// Sink of the push backward: every finished 128-bit piece goes to owner.vals[(my_rank*capacity + slot)*LPR + c] (and to
+// row_grads when given).  PREFETCH: the plan words are loaded with the d_tile rows, before the S reduction, and held in
+// registers; otherwise each is loaded at use.  The LIN form loads at use: with the d_wlin accumulator in registers,
+// holding the plan words as well spills under its 2-CTA bound at HOLD = 12.
+template <int LPR, int HOLD, bool PREFETCH>
+struct QueueSink {
+  const PeerQueues& q;
+  size_t qbase;
+  const int* __restrict__ p_row;
+  float4* __restrict__ o_row;
+  int pw[PREFETCH ? HOLD : 1];
+  __device__ __forceinline__ void fetch(int k, int j) {
+    if (PREFETCH) pw[k] = __ldg(p_row + j / LPR);
+  }
+  __device__ __forceinline__ void operator()(int k, int j, const float4& r) {
+    if (o_row != nullptr) stg_stream_f4(o_row + j, r);
+    const int w = PREFETCH ? pw[k] : __ldg(p_row + j / LPR);
+    if (w >= 0) stg_f4(queue_slot(q, qbase, w, LPR, j % LPR), r);
+  }
+};
+
+// Lookup backward fused with the gradient exchange: the per-sample body of lookup_bwd.cuh with the queue store as sink.
+// LIN (HOLD > 0 only): the backward of the fused dense(1) head (ctr_embed_fm2_lin_fwd), as in embed_fm2_bwd_kernel:
+// `d_tile` carries wlin (F*D) and d_wlin = sum_b d_lin[b]*e[b] is accumulated (LinHead).
 template <int LPR, int HOLD, bool LIN = false>
 __global__ void __launch_bounds__(256, LIN ? 2 : 1)
 embed_fm2_bwd_push_kernel(const float4* __restrict__ tile, const float4* __restrict__ d_tile, const float* __restrict__ d_fm2,
                           const int* __restrict__ plan, int B, int F, const PeerQueues q, float4* __restrict__ row_grads,
                           const float* __restrict__ d_lin, float4* __restrict__ d_wlin) {
-  extern __shared__ float4 s_lin[];                 // LIN: [n4] wlin, then [n4] d_wlin accumulator
-  const unsigned full = 0xffffffffu;
+  extern __shared__ float4 s_lin[];
   const int lane = threadIdx.x & 31;
   const int warp0 = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int nwarps = (gridDim.x * blockDim.x) >> 5;
   const int n4 = F * LPR;
   const size_t qbase = (size_t)q.my_rank * q.capacity;
-  constexpr int HA = (LIN && HOLD > 0) ? HOLD : 1;
-  float4 acc[HA];
-  if (LIN) {
-    for (int j = threadIdx.x; j < n4; j += blockDim.x) { s_lin[j] = __ldg(d_tile + j); s_lin[n4 + j] = make_float4(0.f, 0.f, 0.f, 0.f); }
-    __syncthreads();
-#pragma unroll
-    for (int k = 0; k < HA; ++k) acc[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-  }
+  LinHead<LIN ? HOLD : 1> lin;
+  if (LIN) lin.stage(s_lin, d_tile, n4);
   for (int b = warp0; b < B; b += nwarps) {
     const float4* e_row = tile + (size_t)b * n4;
-    const float4* dt_row = (d_tile && !LIN) ? d_tile + (size_t)b * n4 : nullptr;
-    const int* p_row = plan + (size_t)b * F;
-    float4* o_row = row_grads ? row_grads + (size_t)b * n4 : nullptr;
+    RowGrad rows{(d_tile && !LIN) ? d_tile + (size_t)b * n4 : nullptr};
+    QueueSink<LPR, HOLD, (HOLD > 0 && !LIN)> sink{q, qbase, plan + (size_t)b * F, row_grads ? row_grads + (size_t)b * n4 : nullptr};
     const float g = d_fm2 ? __ldg(d_fm2 + b) : 0.f;
-    const float gl = (LIN && d_lin) ? __ldg(d_lin + b) : 0.f;
-    float4 S = make_float4(0.f, 0.f, 0.f, 0.f);
-    if (HOLD > 0) {
-      constexpr int H = HOLD > 0 ? HOLD : 1;
-      float4 e[H], dt[H];
-      int pw[H];
-#pragma unroll
-      for (int k = 0; k < H; ++k) {
-        const int j = k * 32 + lane;
-        e[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-        if (j < n4) e[k] = ldg_stream_f4(e_row + j);
-      }
-#pragma unroll
-      for (int k = 0; k < H; ++k) {
-        const int j = k * 32 + lane;
-        dt[k] = make_float4(0.f, 0.f, 0.f, 0.f);
-        pw[k] = -1;
-        if (j < n4) {
-          if (LIN) { const float4 w = s_lin[j]; dt[k] = make_float4(gl * w.x, gl * w.y, gl * w.z, gl * w.w); }
-          else if (dt_row != nullptr) dt[k] = ldg_stream_f4(dt_row + j);
-          pw[k] = __ldg(p_row + j / LPR);
-        }
-      }
-#pragma unroll
-      for (int k = 0; k < H; ++k) { S.x += e[k].x; S.y += e[k].y; S.z += e[k].z; S.w += e[k].w; }
-#pragma unroll
-      for (int o = LPR; o < 32; o <<= 1) {
-        S.x += __shfl_xor_sync(full, S.x, o); S.y += __shfl_xor_sync(full, S.y, o);
-        S.z += __shfl_xor_sync(full, S.z, o); S.w += __shfl_xor_sync(full, S.w, o);
-      }
-#pragma unroll
-      for (int k = 0; k < H; ++k) {
-        const int j = k * 32 + lane;
-        if (j < n4) {
-          float4 r;
-          r.x = dt[k].x + g * (S.x - e[k].x); r.y = dt[k].y + g * (S.y - e[k].y);
-          r.z = dt[k].z + g * (S.z - e[k].z); r.w = dt[k].w + g * (S.w - e[k].w);
-          if (o_row != nullptr) stg_stream_f4(o_row + j, r);
-          if (pw[k] >= 0) stg_f4(queue_slot(q, qbase, pw[k], LPR, j % LPR), r);
-          if (LIN) { acc[k % HA].x += gl * e[k].x; acc[k % HA].y += gl * e[k].y; acc[k % HA].z += gl * e[k].z; acc[k % HA].w += gl * e[k].w; }
-        }
-      }
+    const float4 g4 = make_float4(g, g, g, g);
+    if constexpr (LIN) {
+      lin.gl = d_lin ? __ldg(d_lin + b) : 0.f;
+      lookup_bwd_sample<LPR, HOLD>(e_row, n4, lane, g4, lin, sink);
     } else {
-      for (int j = lane; j < n4; j += 32) {
-        const float4 v = __ldg(e_row + j);
-        S.x += v.x; S.y += v.y; S.z += v.z; S.w += v.w;
-      }
-#pragma unroll
-      for (int o = LPR; o < 32; o <<= 1) {
-        S.x += __shfl_xor_sync(full, S.x, o); S.y += __shfl_xor_sync(full, S.y, o);
-        S.z += __shfl_xor_sync(full, S.z, o); S.w += __shfl_xor_sync(full, S.w, o);
-      }
-      for (int j = lane; j < n4; j += 32) {
-        const float4 v = __ldg(e_row + j);
-        float4 r = dt_row ? ldg_stream_f4(dt_row + j) : make_float4(0.f, 0.f, 0.f, 0.f);
-        r.x += g * (S.x - v.x); r.y += g * (S.y - v.y); r.z += g * (S.z - v.z); r.w += g * (S.w - v.w);
-        if (o_row != nullptr) stg_stream_f4(o_row + j, r);
-        const int pw = __ldg(p_row + j / LPR);
-        if (pw >= 0) stg_f4(queue_slot(q, qbase, pw, LPR, j % LPR), r);
-      }
+      lookup_bwd_sample<LPR, HOLD>(e_row, n4, lane, g4, rows, sink);
     }
   }
-  if (LIN) {
-#pragma unroll
-    for (int k = 0; k < HA; ++k) {
-      const int j = k * 32 + lane;
-      if (j < n4) {
-        float* a = reinterpret_cast<float*>(s_lin + n4 + j);
-        atomicAdd(a + 0, acc[k].x); atomicAdd(a + 1, acc[k].y); atomicAdd(a + 2, acc[k].z); atomicAdd(a + 3, acc[k].w);
-      }
-    }
-    __syncthreads();
-    for (int j = threadIdx.x; j < n4; j += blockDim.x) atomicAdd(d_wlin + j, s_lin[n4 + j]);
-  }
+  if (LIN) lin.flush(d_wlin, lane);
 }
 
 // The exchange alone: row_grads (B,F,D) already exist; every planned row is copied into its owner's queue.
@@ -289,44 +234,6 @@ static int fill_queues(const char* fn, PeerQueues& q, int64_t G, int64_t my_rank
   return CTR_OK;
 }
 
-template <int LPR, int HOLD>
-static int launch_bwd_push(const float* tile, const float* d_tile, const float* d_fm2, const int32_t* plan, int64_t B, int64_t F,
-                           const PeerQueues& q, float* row_grads, cudaStream_t st) {
-  return launch_resident("ctr_embed_fm2_bwd_push", embed_fm2_bwd_push_kernel<LPR, HOLD, false>, (B + 7) / 8, 256, 0, st,
-                         reinterpret_cast<const float4*>(tile), reinterpret_cast<const float4*>(d_tile), d_fm2, plan, (int)B, (int)F, q,
-                         reinterpret_cast<float4*>(row_grads), nullptr, nullptr);
-}
-
-template <int LPR, int HOLD>
-static int launch_lin_bwd_push(const float* tile, const float* wlin, const float* d_fm2, const float* d_lin, const int32_t* plan,
-                               int64_t B, int64_t F, const PeerQueues& q, float* row_grads, float* d_wlin, cudaStream_t st) {
-  return launch_resident("ctr_embed_fm2_lin_bwd_push", embed_fm2_bwd_push_kernel<LPR, HOLD, true>, (B + 7) / 8, 256,
-                         sizeof(float4) * 2 * (size_t)F * LPR, st, reinterpret_cast<const float4*>(tile),
-                         reinterpret_cast<const float4*>(wlin), d_fm2, plan, (int)B, (int)F, q, reinterpret_cast<float4*>(row_grads),
-                         d_lin, reinterpret_cast<float4*>(d_wlin));
-}
-
-template <int LPR>
-static int dispatch_lin_bwd_push(const float* tile, const float* wlin, const float* d_fm2, const float* d_lin, const int32_t* plan,
-                                 int64_t B, int64_t F, const PeerQueues& q, float* row_grads, float* d_wlin, cudaStream_t st) {
-  const int64_t per_lane = (F * LPR + 31) / 32;
-  if (per_lane <= 4) return launch_lin_bwd_push<LPR, 4>(tile, wlin, d_fm2, d_lin, plan, B, F, q, row_grads, d_wlin, st);
-  if (per_lane <= 8) return launch_lin_bwd_push<LPR, 8>(tile, wlin, d_fm2, d_lin, plan, B, F, q, row_grads, d_wlin, st);
-  if (per_lane <= 12) return launch_lin_bwd_push<LPR, 12>(tile, wlin, d_fm2, d_lin, plan, B, F, q, row_grads, d_wlin, st);
-  set_error("ctr_embed_fm2_lin_bwd_push: F*D = %lld exceeds the register-resident limit of 1536", (long long)(F * LPR * 4));
-  return CTR_ERR_UNSUPPORTED;
-}
-
-template <int LPR>
-static int dispatch_bwd_push(const float* tile, const float* d_tile, const float* d_fm2, const int32_t* plan, int64_t B,
-                             int64_t F, const PeerQueues& q, float* row_grads, cudaStream_t st) {
-  const int64_t per_lane = (F * LPR + 31) / 32;
-  if (per_lane <= 4) return launch_bwd_push<LPR, 4>(tile, d_tile, d_fm2, plan, B, F, q, row_grads, st);
-  if (per_lane <= 8) return launch_bwd_push<LPR, 8>(tile, d_tile, d_fm2, plan, B, F, q, row_grads, st);
-  if (per_lane <= 12) return launch_bwd_push<LPR, 12>(tile, d_tile, d_fm2, plan, B, F, q, row_grads, st);
-  return launch_bwd_push<LPR, 0>(tile, d_tile, d_fm2, plan, B, F, q, row_grads, st);
-}
-
 }  // namespace ctr
 
 using namespace ctr;
@@ -366,8 +273,13 @@ extern "C" int ctr_embed_fm2_bwd_push(const float* tile, const float* d_tile, co
   CTR_REQUIRE(aligned16(tile) && aligned16(d_tile) && aligned16(row_grads),
               "ctr_embed_fm2_bwd_push: tile, d_tile and row_grads must be 16-byte aligned");
   if (B == 0) return CTR_OK;
-  cudaStream_t st = as_stream(stream);
-  return with_lpr(D, [&](auto LPR) { return dispatch_bwd_push<LPR>(tile, d_tile, d_fm2, plan, B, F, q, row_grads, st); });
+  return with_lpr(D, [&](auto LPR) {
+    return with_hold<true>(F, LPR, [&](auto HOLD) {
+      return launch_resident("ctr_embed_fm2_bwd_push", embed_fm2_bwd_push_kernel<LPR, HOLD, false>, (B + 7) / 8, 256, 0,
+                             as_stream(stream), reinterpret_cast<const float4*>(tile), reinterpret_cast<const float4*>(d_tile), d_fm2,
+                             plan, (int)B, (int)F, q, reinterpret_cast<float4*>(row_grads), nullptr, nullptr);
+    });
+  });
 }
 
 extern "C" int ctr_embed_fm2_lin_bwd_push(const float* tile, const float* wlin, const float* d_fm2, const float* d_lin,
@@ -386,7 +298,12 @@ extern "C" int ctr_embed_fm2_lin_bwd_push(const float* tile, const float* wlin, 
   CTR_CUDA(cudaMemsetAsync(d_wlin, 0, sizeof(float) * F * D, st));
   if (B == 0) return CTR_OK;
   return with_lpr(D, [&](auto LPR) {
-    return dispatch_lin_bwd_push<LPR>(tile, wlin, d_fm2, d_lin, plan, B, F, q, row_grads, d_wlin, st);
+    return with_hold<false>(F, LPR, [&](auto HOLD) {
+      return launch_resident("ctr_embed_fm2_lin_bwd_push", embed_fm2_bwd_push_kernel<LPR, HOLD, true>, (B + 7) / 8, 256,
+                             sizeof(float4) * 2 * (size_t)F * LPR, st, reinterpret_cast<const float4*>(tile),
+                             reinterpret_cast<const float4*>(wlin), d_fm2, plan, (int)B, (int)F, q,
+                             reinterpret_cast<float4*>(row_grads), d_lin, reinterpret_cast<float4*>(d_wlin));
+    }, "ctr_embed_fm2_lin_bwd_push");
   });
 }
 

@@ -112,7 +112,8 @@ def _half_ulp(w):
     return (torch.nextafter(w, torch.full_like(w, float("inf"))) - w).double() / 2
 
 @pytest.mark.parametrize("lazy", [False, True])
-@pytest.mark.parametrize("B,F,D,rows", [(64, 5, 16, 37), (512, 3, 8, 3), (300, 40, 32, 1000), (129, 33, 4, 11), (40, 12, 128, 50)])
+@pytest.mark.parametrize("B,F,D,rows", [(64, 5, 16, 37), (512, 3, 8, 3), (300, 40, 32, 1000), (129, 33, 4, 11), (40, 12, 128, 50),
+                                         (200, 24, 32, 500)])
 def test_backward_fused_with_adam_equals_unfused(lazy, B, F, D, rows):
     """ctr_embed_fm2_bwd_adam (backward + row update in one pass, duplicates finished through the parked list) against
     ctr_embed_fm2_bwd + ctr_adam_indexed_slices and the float64 oracle, three steps, duplicates / OOV / out-of-range ids."""

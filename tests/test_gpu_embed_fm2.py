@@ -27,7 +27,7 @@ def oracle_lookup(table, off, ids):
 
 
 @pytest.mark.parametrize("B,F,D", [(1, 1, 4), (7, 6, 8), (33, 30, 16), (64, 40, 32), (19, 33, 32), (5, 70, 64),
-                                   (9, 3, 128), (130, 8, 4), (257, 65, 16)])
+                                   (9, 3, 128), (130, 8, 4), (257, 65, 16), (20, 24, 32)])
 def test_fwd_bwd_parity(B, F, D):
     from recalgorithm_b200 import ops
     rng = np.random.default_rng(B * 1000 + F * 10 + D)
@@ -48,6 +48,10 @@ def test_fwd_bwd_parity(B, F, D):
     assert_close(ops.embed_fm2_bwd(tile, dev(d_tile), dev(g)), want, TOL, "row_grads")
     assert_close(ops.embed_fm2_bwd(tile, None, dev(g)), O.fm2_bwd(e.astype(np.float64), g.astype(np.float64)), TOL, "fm2-only grads")
     assert torch.equal(ops.embed_fm2_bwd(tile, dev(d_tile), None), dev(d_tile))
+    d_bi = trunc_normal(rng, (B, D), 1.0)
+    e64 = e.astype(np.float64)
+    want_bi = d_tile.astype(np.float64) + d_bi.astype(np.float64)[:, None, :] * (e64.sum(1, keepdims=True) - e64)
+    assert_close(ops.embed_bi_bwd(tile, dev(d_tile), dev(d_bi)), want_bi, TOL, "bi row_grads")
     # IndexedSlices densified (duplicates summed, invalid ids dropped)
     rg = ops.embed_fm2_bwd(tile, dev(d_tile), dev(g))
     dense = torch.zeros_like(dev(table))
@@ -157,7 +161,8 @@ def test_full_size_properties():
     assert torch.equal(tile, tile2) and torch.equal(fm2, fm2b)
 
 
-@pytest.mark.parametrize("B,F,D", [(7, 6, 8), (64, 40, 32), (19, 33, 32), (130, 8, 4), (257, 65, 16), (9, 3, 128)])
+@pytest.mark.parametrize("B,F,D", [(7, 6, 8), (64, 40, 32), (19, 33, 32), (130, 8, 4), (257, 65, 16), (9, 3, 128),
+                                   (50, 24, 32), (8192, 40, 32)])
 def test_int32_ids_and_fused_linear_head(B, F, D):
     """int32 ids (half the PCIe bytes) give the identical tile and a widened int64 copy; the fused dense(1) head equals the
     unfused chain tile.reshape(B, F*D) @ w and its backward equals ctr_embed_fm2_bwd fed with the rank-1 d_tile."""

@@ -105,7 +105,8 @@ def _reference_dense(grp, ids_per_rank, rg_per_rank):
 
 
 @pytest.mark.parametrize("G", [2, 4, 8])
-@pytest.mark.parametrize("B,F,D,rows_each", [(257, 40, 32, 5000), (64, 6, 8, 300), (1000, 33, 16, 1), (513, 100, 4, 50)])
+@pytest.mark.parametrize("B,F,D,rows_each", [(257, 40, 32, 5000), (64, 6, 8, 300), (1000, 33, 16, 1), (513, 100, 4, 50),
+                                              (40, 20, 128, 30)])
 def test_selfpeer_lookup_plan_push(G, B, F, D, rows_each):
     from recalgorithm_b200 import ops
     dev = torch.device("cuda", 0)
@@ -230,12 +231,11 @@ def test_selfpeer_owner_adam(lazy):
                 assert_close(a, b_, what=f"owner adam lazy={lazy} step {step} owner {d} {name}")
 
 
-@pytest.mark.parametrize("G", [2, 8])
-def test_selfpeer_fused_linear_head(G):
+@pytest.mark.parametrize("B,F,D,G", [(300, 40, 32, 2), (300, 40, 32, 8), (300, 16, 32, 2), (300, 24, 32, 8), (8192, 40, 32, 2)])
+def test_selfpeer_fused_linear_head(B, F, D, G):
     """Sharded lookup + FM2 + fused dense(1) head and its backward+push equal the unsharded fused kernels / the plain chain."""
     from recalgorithm_b200 import _lib, ops
     dev = torch.device("cuda", 0)
-    B, F, D = 300, 40, 32
     rows = [500 + 3 * f for f in range(F)]
     grp = LocalShardGroup(rows, D, G, B)
     rows_t = torch.tensor(rows, device=dev)
@@ -262,7 +262,7 @@ def test_selfpeer_fused_linear_head(G):
         rg = torch.empty_like(tile); dw = torch.empty((F * D,), device=dev)
         _lib.check(L.ctr_embed_fm2_lin_bwd_push(ops._ptr(tile), ops._ptr(wlin), ops._ptr(d_fm2), ops._ptr(d_lin), ops._ptr(plan), B, F, D, G,
                                                 rank, grp.v_ptrs, grp.capacity, ops._ptr(rg), ops._ptr(dw), ops._stream()))
-        assert_close(rg, rg_ref.double(), what="row_grads (fused head + push vs fused head)")     # same math, different FMA contraction
+        assert torch.equal(rg, rg_ref), "row_grads (fused head + push vs fused head)"             # one kernel body
         assert_close(dw, dw_ref.double(), what="d_wlin")
         ids_all.append(ids); rg_all.append(rg_ref)
     want = _reference_dense(grp, ids_all, rg_all)

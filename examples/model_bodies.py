@@ -171,3 +171,28 @@ def mmoe_logits(dense_input, category_input, labels, task_names=("read_comment",
     losses = [torch.nn.functional.binary_cross_entropy_with_logits(logit, labels[task_name])          # :261-263
               for logit, task_name in zip(logits, task_names)]
     return logits, sum(losses[1:], losses[0])
+
+
+def ple_logits(dense_input, category_input, labels, task_names=("read_comment", "like", "click_avatar"),
+               num_extract_network=1, num_experts_per_task=(5, 5, 5), num_experts_in_shared=10, expert_hidden_units=256,
+               hidden_units=(512, 256, 128)):
+    """PLE/ple.py:160-254: num_extract_network extraction networks, then the final experts and gates, each in one kernel
+    each way; one tower_layer per task (MMOE/tower_layer.py, which ple.py imports: relu dense stack, tower_{task}_logit; its batch norm and
+    dropout left out) in scope tower, and the sum of the per-task mean sigmoid cross-entropies.  labels maps task name ->
+    (B, 1).  Returns (logits, total_loss)."""
+    net = torch.cat([dense_input, category_input], dim=-1)                                # :169
+    for i in range(num_extract_network):                                                  # :172-180
+        net = L.extraction_network(net, task_names, num_experts_per_task, num_experts_in_shared, expert_hidden_units,
+                                   f"extract_network_{i}")
+    towers = L.ple_final_experts_gates(net, task_names, num_experts_per_task, num_experts_in_shared,
+                                       expert_hidden_units)                               # :185-226
+    logits, n_dense = [], 0
+    with L.variable_scope("tower"):
+        for x, task_name in zip(towers, task_names):                                      # :229-235
+            for unit in hidden_units:                                                     # TF uniquifies dense, dense_1, ...
+                x = dense(x, unit, activation=torch.relu, name=f"dense_{n_dense}" if n_dense else "dense")
+                n_dense += 1
+            logits.append(dense(x, 1, name=f"tower_{task_name}_logit"))
+    losses = [torch.nn.functional.binary_cross_entropy_with_logits(logit, labels[task_name])          # :251-254
+              for logit, task_name in zip(logits, task_names)]
+    return logits, sum(losses[1:], losses[0])

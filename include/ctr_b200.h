@@ -331,6 +331,34 @@ int ctr_mmoe_bwd(const float* x, const float* w_experts, const float* b_experts,
                  float* d_w_experts, float* d_b_experts, float* d_w_gates, void* workspace, int64_t workspace_bytes,
                  void* stream);
 
+/* ---- PLE extraction network and final gate layer ---------------------------------------------------------
+ * Replaces extraction_network (PLE/extraction_network.py:4-85, extraction = 1) and the final experts and gates of
+ * ple_model_fn (PLE/ple.py:185-226, extraction = 0).  T tasks with experts_per_task[t] = n_t >= 1 experts each (a host
+ * array of T int64), S >= 1 shared experts, E = sum_t n_t + S experts in [task 0 .. task T-1, shared] order:
+ *   h_e   = relu(x . w_e + b_e)           x (B,d); w_experts (E,d,H), b_experts (E,H)
+ *   p_t   = softmax(x . gate_t)           over [task t's experts, shared experts]: n_t + S columns, no bias
+ *   p_all = softmax(x . all_gate)         over all E experts (extraction = 1 only)
+ *   w_gates (d, GC): the gate kernels concatenated by columns, gate_0 .. gate_{T-1} (then all_gate);
+ *   GC = sum_t (n_t + S) (+ E).  gates (B, GC): the softmax probabilities, the same column layout.
+ *   extraction = 0: out (T,B,H), out_t = sum_j p_t[j] h_(t, j);
+ *   extraction = 1: out (B,H), the sum of the T task outputs and the all-gate output.
+ * fp32-class accuracy (3xTF32 on the tensor cores); the (B,E,H) expert outputs stay on chip.  1 <= d <= 512,
+ * 1 <= H <= 512, 1 <= T <= 4, E <= 64 and GC <= 160 (CTR_ERR_UNSUPPORTED otherwise); B = 0 launches nothing.
+ * workspace: 128-byte aligned, at least ctr_ple_workspace_bytes(0, ...) bytes for the forward (the prepped weights) and
+ * ctr_ple_workspace_bytes(B, ...) for the backward, which adds the expert and gate-logit gradients: (B, E*HP + GP)
+ * floats with HP = H and GP = GC rounded up to 64 -- about 25.6 KB per sample at E = 25, H = 256.  The backward takes the
+ * forward's gates and g_out (shaped as out), and overwrites d_x (B,d), d_w_experts (E,d,H), d_b_experts (E,H) and
+ * d_w_gates (d,GC) (zeros at B = 0). */
+int ctr_ple_workspace_bytes(int64_t B, int64_t d, int64_t H, int64_t T, const int64_t* experts_per_task, int64_t S,
+                            int64_t extraction, int64_t* bytes);
+int ctr_ple_fwd(const float* x, const float* w_experts, const float* b_experts, const float* w_gates, int64_t B, int64_t d,
+                int64_t H, int64_t T, const int64_t* experts_per_task, int64_t S, int64_t extraction, float* out,
+                float* gates, void* workspace, int64_t workspace_bytes, void* stream);
+int ctr_ple_bwd(const float* x, const float* w_experts, const float* b_experts, const float* w_gates, const float* gates,
+                const float* g_out, int64_t B, int64_t d, int64_t H, int64_t T, const int64_t* experts_per_task, int64_t S,
+                int64_t extraction, float* d_x, float* d_w_experts, float* d_b_experts, float* d_w_gates, void* workspace,
+                int64_t workspace_bytes, void* stream);
+
 /* ---- Row DIN-ATT: DIN attention unit -----------------------------------------------------------------
  * Replaces din_attention(query, keys, keys_length, is_softmax) (DIN/din_attention.py:17-43).
  * query (B,H); keys (B,T,H); keys_length int64 (B); dense layers f1_att (4H->64, relu), f2_att (64->32,

@@ -99,6 +99,9 @@ SIGNATURES = {
     "ctr_mmoe_workspace_bytes": (c_int, [_I, _I, _I, _I, _I, POINTER(c_int64)]),
     "ctr_mmoe_fwd": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _I, _P]),
     "ctr_mmoe_bwd": (c_int, [_P] * 6 + [_I] * 5 + [_P] * 5 + [_I, _P]),
+    "ctr_ple_workspace_bytes": (c_int, [_I, _I, _I, _I, _P, _I, _I, POINTER(c_int64)]),
+    "ctr_ple_fwd": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _P, _I, _I, _P, _P, _P, _I, _P]),
+    "ctr_ple_bwd": (c_int, [_P] * 6 + [_I] * 4 + [_P, _I, _I] + [_P] * 5 + [_I, _P]),
 }
 
 

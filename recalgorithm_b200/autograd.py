@@ -474,3 +474,26 @@ def mmoe(x: torch.Tensor, w_experts: torch.Tensor, b_experts: torch.Tensor, w_ga
     """MMoE expert-gate layer: (towers (T,B,H), gates (T,B,E), forward only) from x (B,d), w_experts (E,d,H), b_experts (E,H)
     and w_gates (T,d,E)."""
     return _MMoE.apply(x, w_experts, b_experts, w_gates)
+
+
+class _PLE(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, w_experts, b_experts, w_gates, experts_per_task, num_experts_in_shared, extraction):
+        x, w_experts, b_experts, w_gates = (t.contiguous() for t in (x, w_experts, b_experts, w_gates))
+        out, gates = ops.ple_fwd(x, w_experts, b_experts, w_gates, experts_per_task, num_experts_in_shared, extraction)
+        ctx.save_for_backward(x, w_experts, b_experts, w_gates, gates)   # the expert outputs are recomputed from x
+        ctx.counts = (experts_per_task, num_experts_in_shared, extraction)
+        ctx.mark_non_differentiable(gates)
+        return out, gates
+
+    @staticmethod
+    def backward(ctx, g_out, _g_gates):
+        return (*ops.ple_bwd(*ctx.saved_tensors, g_out.contiguous(), *ctx.counts), None, None, None)
+
+
+def ple(x: torch.Tensor, w_experts: torch.Tensor, b_experts: torch.Tensor, w_gates: torch.Tensor, experts_per_task,
+        num_experts_in_shared: int, extraction: bool):
+    """PLE expert-gate block: (out, gates (B,GC), forward only) from x (B,d), w_experts (E,d,H), b_experts (E,H) and
+    w_gates (d,GC); out is (B,H) for the extraction network and (T,B,H) for the final layer (see ops.ple_fwd)."""
+    return _PLE.apply(x, w_experts, b_experts, w_gates, tuple(int(v) for v in experts_per_task), int(num_experts_in_shared),
+                      bool(extraction))

@@ -359,6 +359,88 @@ def mmoe_experts_gates(concat_all_input: torch.Tensor, num_experts, expert_hidde
     return towers
 
 
+# --------------------------------------------------------------------------------------------------- PLE
+def _ple_sizes(task_names, num_experts_per_task, num_experts_in_shared, expert_hidden_units):
+    task_names = list(task_names)
+    n = [int(v) for v in num_experts_per_task]
+    if len(task_names) != len(n):
+        raise ValueError(f"task_names has {len(task_names)} entries but num_experts_per_task has {len(n)}: the all-gate "
+                         "width and the task outputs depend on both")
+    return task_names, n, int(num_experts_in_shared), int(expert_hidden_units)
+
+
+def _expert(name, d, H, kernels, biases):
+    with variable_scope(name):
+        kernels.append(get_variable("kernel", (d, H)))
+        biases.append(get_variable("bias", (H,), initializer=lambda s: torch.zeros(s)))
+
+
+def _ple_call(x, task_expert_lists, shared, gate_kernels, n, S, extraction):
+    """Stacks the variables into the packed layout ([task 0 .. task T-1, shared] experts, gate kernels by columns)."""
+    kernels = [k for ks, _ in task_expert_lists for k in ks] + shared[0]
+    biases = [b for _, bs in task_expert_lists for b in bs] + shared[1]
+    return autograd.ple(x, torch.stack(kernels), torch.stack(biases), torch.cat(gate_kernels, dim=1), n, S, extraction)
+
+
+def extraction_network(input: torch.Tensor, task_names, num_experts_per_task, num_experts_in_shared, expert_hidden_units,
+                       name) -> torch.Tensor:
+    """PLE extraction network -- same signature as PLE/extraction_network.py:4, one kernel each way: the sum of every
+    task's gated output (over its own experts, then the shared ones) and the all-gate's output (over all experts), (B, H).
+
+    Creates, in scope ``name``, the variables of the reference's ``tf.layers.dense`` calls in its order: the shared experts
+    ``shared_expert_{i}``, then per task its experts ``task_specific_expert_{task}_{i}`` and its gate ``gate_{task}``
+    (width n_t + S), then ``all_gate`` (width sum n_t + S).  Expert kernels are glorot-uniform with zero biases; gates have
+    a glorot-uniform kernel and no bias.  The sizes go through ``int()``.  ``task_names`` and ``num_experts_per_task`` must
+    have the same length (ValueError otherwise: the reference's zip would drop tasks and size its all-gate wrongly)."""
+    task_names, n, S, H = _ple_sizes(task_names, num_experts_per_task, num_experts_in_shared, expert_hidden_units)
+    d = int(input.shape[-1])
+    shared, tasks, gates = ([], []), [], []
+    with variable_scope(name):
+        for i in range(S):
+            _expert(f"shared_expert_{i}", d, H, *shared)
+        for task, nt in zip(task_names, n):
+            ks, bs = [], []
+            for i in range(nt):
+                _expert(f"task_specific_expert_{task}_{i}", d, H, ks, bs)
+            tasks.append((ks, bs))
+            with variable_scope(f"gate_{task}"):
+                gates.append(get_variable("kernel", (d, nt + S)))
+        with variable_scope("all_gate"):
+            gates.append(get_variable("kernel", (d, sum(n) + S)))
+    return _ple_call(input, tasks, shared, gates, n, S, True)[0]
+
+
+def ple_final_experts_gates(input: torch.Tensor, task_names, num_experts_per_task, num_experts_in_shared,
+                            expert_hidden_units, return_gates: bool = False):
+    """PLE's last layer -- PLE/ple.py:185-226, one kernel each way: per task, the gated sum over its own experts and the
+    shared ones, returned as T contiguous (B, H) tensors (the tower inputs), and with ``return_gates`` also each task's
+    gate weights (B, n_t + S).
+
+    Creates the reference's variables in its order: ``shared_experts_final/shared_expert_final_{i}``, then per task its
+    experts ``task_specific_experts_final/task_specific_expert_final_{task}_{i}`` and its gate
+    ``task_specific_experts_final/task_gate_final/gate_final_{task}``.  Initialisers, the int() sizes and the length check
+    are those of extraction_network."""
+    task_names, n, S, H = _ple_sizes(task_names, num_experts_per_task, num_experts_in_shared, expert_hidden_units)
+    d = int(input.shape[-1])
+    shared, tasks, gates = ([], []), [], []
+    with variable_scope("shared_experts_final"):
+        for i in range(S):
+            _expert(f"shared_expert_final_{i}", d, H, *shared)
+    with variable_scope("task_specific_experts_final"):
+        for task, nt in zip(task_names, n):
+            ks, bs = [], []
+            for i in range(nt):
+                _expert(f"task_specific_expert_final_{task}_{i}", d, H, ks, bs)
+            tasks.append((ks, bs))
+            with variable_scope("task_gate_final"), variable_scope(f"gate_final_{task}"):
+                gates.append(get_variable("kernel", (d, nt + S)))
+    out, p = _ple_call(input, tasks, shared, gates, n, S, False)
+    out = list(out.unbind(0))
+    if return_gates:
+        return out, list(p.split([nt + S for nt in n], dim=1))
+    return out
+
+
 # --------------------------------------------------------------------------------------------------- DIN loss-side term
 def mini_batch_aware_regularization(embedding_tensors, l2_lambda: float) -> torch.Tensor:
     """DIN/din.py:254-257 (SURVEY parity note 7): ``l2_lambda * tf.nn.l2_loss(concat(tensors, -1)) / batch`` -- an L2 on the

@@ -800,3 +800,67 @@ def mmoe_bwd(x, w_experts, b_experts, w_gates, gates, g_towers):
                                        B, d, E, H, T, _ptr(d_x), _ptr(d_we), _ptr(d_be), _ptr(d_wg), _ptr(ws), ws.numel(),
                                        _stream()))
     return d_x, d_we, d_be, d_wg
+
+
+# ------------------------------------------------------------------------------------ PLE expert-gate blocks
+def _ple_counts(experts_per_task, num_experts_in_shared, extraction):
+    n = [int(v) for v in experts_per_task]
+    return (ctypes.c_int64 * max(1, len(n)))(*n), n, int(num_experts_in_shared), 1 if extraction else 0
+
+
+def ple_gate_width(experts_per_task, num_experts_in_shared, extraction) -> int:
+    """GC, the number of gate columns: sum_t (n_t + S), plus the all-gate's sum_t n_t + S in the extraction network."""
+    n, S = [int(v) for v in experts_per_task], int(num_experts_in_shared)
+    return sum(n) + len(n) * S + ((sum(n) + S) if extraction else 0)
+
+
+def ple_workspace(B: int, d: int, H: int, experts_per_task, num_experts_in_shared, extraction, device) -> torch.Tensor:
+    """Caller-owned workspace: the prepped weights (B = 0, what the forward needs) plus, for the backward, the expert and
+    gate-logit gradients."""
+    arr, n, S, ext = _ple_counts(experts_per_task, num_experts_in_shared, extraction)
+    nbytes = ctypes.c_int64(0)
+    _lib.check(_lib.lib().ctr_ple_workspace_bytes(B, d, H, len(n), arr, S, ext, ctypes.byref(nbytes)))
+    return torch.empty((int(nbytes.value),), dtype=torch.uint8, device=device)
+
+
+def _ple_args(x, w_experts, b_experts, w_gates, experts_per_task, num_experts_in_shared, extraction):
+    _chk(x, F32, "input")
+    if x.dim() != 2 or w_experts.dim() != 3 or w_gates.dim() != 2:
+        raise ValueError("ple: x (B,d), w_experts (E,d,H) and w_gates (d,GC) expected")
+    B, d = x.shape
+    E, _, H = w_experts.shape
+    n, S = [int(v) for v in experts_per_task], int(num_experts_in_shared)
+    if E != sum(n) + S:
+        raise ValueError(f"ple: w_experts holds {E} experts, experts_per_task and num_experts_in_shared give {sum(n) + S}")
+    _chk(w_experts, F32, "w_experts", (E, d, H)); _chk(b_experts, F32, "b_experts", (E, H))
+    _chk(w_gates, F32, "w_gates", (d, ple_gate_width(n, S, extraction)))
+    return B, d, H
+
+
+def ple_fwd(x, w_experts, b_experts, w_gates, experts_per_task, num_experts_in_shared, extraction):
+    """PLE/extraction_network.py:4-85 (extraction = True) or PLE/ple.py:185-226 (False): x (B,d), w_experts (E,d,H) and
+    b_experts (E,H) in [task 0 .. task T-1, shared] order, w_gates (d,GC) the gate kernels concatenated by columns ->
+    (out, gates (B,GC)).  out is (B,H) for the extraction network, (T,B,H) for the final layer."""
+    B, d, H = _ple_args(x, w_experts, b_experts, w_gates, experts_per_task, num_experts_in_shared, extraction)
+    arr, n, S, ext = _ple_counts(experts_per_task, num_experts_in_shared, extraction)
+    out = torch.empty((B, H) if ext else (len(n), B, H), dtype=F32, device=x.device)
+    gates = torch.empty((B, w_gates.shape[1]), dtype=F32, device=x.device)
+    ws = ple_workspace(0, d, H, n, S, ext, x.device)
+    _lib.check(_lib.lib().ctr_ple_fwd(_ptr(x), _ptr(w_experts), _ptr(b_experts), _ptr(w_gates), B, d, H, len(n), arr, S, ext,
+                                      _ptr(out), _ptr(gates), _ptr(ws), ws.numel(), _stream()))
+    return out, gates
+
+
+def ple_bwd(x, w_experts, b_experts, w_gates, gates, g_out, experts_per_task, num_experts_in_shared, extraction):
+    """Gradients of ple_fwd given its gates (B,GC) and g_out (shaped as out): (d_x, d_w_experts, d_b_experts, d_w_gates).
+    The expert outputs are recomputed from x."""
+    B, d, H = _ple_args(x, w_experts, b_experts, w_gates, experts_per_task, num_experts_in_shared, extraction)
+    arr, n, S, ext = _ple_counts(experts_per_task, num_experts_in_shared, extraction)
+    _chk(gates, F32, "gates", (B, w_gates.shape[1]))
+    _chk(g_out, F32, "g_out", (B, H) if ext else (len(n), B, H))
+    d_x, d_we, d_be, d_wg = (torch.empty_like(t) for t in (x, w_experts, b_experts, w_gates))
+    ws = ple_workspace(B, d, H, n, S, ext, x.device)
+    _lib.check(_lib.lib().ctr_ple_bwd(_ptr(x), _ptr(w_experts), _ptr(b_experts), _ptr(w_gates), _ptr(gates), _ptr(g_out), B, d,
+                                      H, len(n), arr, S, ext, _ptr(d_x), _ptr(d_we), _ptr(d_be), _ptr(d_wg), _ptr(ws),
+                                      ws.numel(), _stream()))
+    return d_x, d_we, d_be, d_wg

@@ -4,7 +4,7 @@
 Each kernel is timed alone with CUDA events; an L2 flush (a 256 MB write) runs between timed iterations because these
 working sets are flushed from the 50 MB L2.  Prints one JSON line per measurement.
 
-    python tools/bench_layers.py [--iters 20] [--only cin,dcn,din,fibinet]     (also: pairwise, bst, adam, pnn, dien, deepcrossing, mmoe)
+    python tools/bench_layers.py [--iters 20] [--only cin,dcn,din,fibinet]     (also: pairwise, bst, adam, pnn, dien, deepcrossing, mmoe, ple)
 """
 import argparse
 import json
@@ -315,6 +315,71 @@ def mmoe_rows(iters, flush, rn):
     finally:
         torch.backends.cuda.matmul.allow_tf32 = prev_tf32
 
+
+def ple_rows(iters, flush, rn):
+    """PLE expert-gate blocks (ctr_ple_fwd / _bwd) at the default result.md row, n = 5,5,5 and S = 10 (E = 25), H = 256:
+    the extraction network at the input width d = 82 and the final layer at d = H = 256, B = 1024 and 65 536, next to plain
+    torch running the same block (fp32 matmul / softmax, TF32 disabled, autograd backward).  The floor is the block's FP32
+    FLOPs (expert and gate GEMMs plus the gated sums; the backward counted as 3x) over the data-sheet 67 TFLOP/s of the
+    H100 SXM at 700 W, not measured."""
+    n, S, H = (5, 5, 5), 10, 256
+    E, es = sum(n) + S, sum(n)
+    print(json.dumps({"ple_card": card()}), flush=True)
+
+    def gate_lists(ext):
+        e0 = [sum(n[:t]) for t in range(len(n))]
+        lists = [list(range(e0[t], e0[t] + n[t])) + list(range(es, E)) for t in range(len(n))]
+        return lists + ([list(range(E))] if ext else [])
+
+    def torch_form(x, we, be, wg, ext):
+        h = torch.relu(x @ we + be[:, None, :])
+        z = x @ wg
+        outs, c = [], 0
+        for experts in gate_lists(ext):
+            p = torch.softmax(z[:, c:c + len(experts)], dim=-1)
+            outs.append(torch.einsum("bj,jbh->bh", p, h[experts]))
+            c += len(experts)
+        return sum(outs) if ext else torch.stack(outs)
+
+    prev_tf32 = torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cuda.matmul.allow_tf32 = False
+    try:
+        for d, ext in ((82, True), (256, False)):
+            GC = sum(len(g) for g in gate_lists(ext))
+            we = (torch.rand(E, d, H, device="cuda") * 2 - 1) * (6.0 / (d + H)) ** 0.5
+            be = rn(E, H, std=0.1)
+            wg = (torch.rand(d, GC, device="cuda") * 2 - 1) * (6.0 / (d + GC)) ** 0.5
+            for B in (1024, 65536):
+                x = rn(B, d, std=0.7)
+                g = rn(B, H) if ext else rn(len(n), B, H)
+                cfg = {"block": "extraction_network" if ext else "final_layer", "B": B, "d": d, "n": list(n), "S": S, "H": H}
+                fl_fwd = 2.0 * B * (d * (E * H + GC) + GC * H)
+                flops = {"fwd": fl_fwd, "bwd": 3 * fl_fwd}
+                out, gates = ops.ple_fwd(x, we, be, wg, n, S, ext)
+                grads = ops.ple_bwd(x, we, be, wg, gates, g, n, S, ext)
+                ps = [t.clone().requires_grad_() for t in (x, we, be, wg)]
+                ref_out = torch_form(*ps, ext)
+                ref_grads = torch.autograd.grad(ref_out, ps, g, retain_graph=True)
+                diff = {"fwd": float((ref_out.detach() - out).abs().max() / ref_out.detach().abs().max()),
+                        "bwd": max(float((a - b).abs().max() / b.abs().max()) for a, b in zip(grads, ref_grads))}
+                runs = {"fwd": (lambda: ops.ple_fwd(x, we, be, wg, n, S, ext), lambda: torch_form(x, we, be, wg, ext)),
+                        "bwd": (lambda: ops.ple_bwd(x, we, be, wg, gates, g, n, S, ext),
+                                lambda: torch.autograd.grad(ref_out, ps, g, retain_graph=True))}
+                for way in ("fwd", "bwd"):
+                    m, bst = timeit(runs[way][0], iters, flush)
+                    tm, tbst = timeit(runs[way][1], iters, flush)
+                    print(json.dumps({
+                        "kernel": f"ple_{way}", "config": cfg, "ms_median": m, "ms_best": bst,
+                        "torch_fp32_ms_median": tm, "torch_fp32_ms_best": tbst, "speedup_vs_torch": tm / m,
+                        "max_norm_rel_diff_vs_torch": diff[way], "l2": "flushed between iterations",
+                        "floor_fp32_us": flops[way] / 67e12 * 1e6,
+                        "note": "floor: data-sheet FP32 rate (H100 SXM, 700 W), not measured; torch: same block, fp32, TF32 off"}),
+                        flush=True)
+                del out, gates, grads, ps, ref_out, ref_grads
+    finally:
+        torch.backends.cuda.matmul.allow_tf32 = prev_tf32
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=20)
@@ -495,6 +560,8 @@ def main():
         deepcrossing_rows(args.iters, flush, rn)
     if "mmoe" in only:  # MMoE expert-gate layer at the reference shape (d = 82, E = 3, H = 512, T = 3); not in the default list
         mmoe_rows(args.iters, flush, rn)
+    if "ple" in only:   # PLE extraction network (d = 82) and final layer (d = 256) at the default row; not in the default list
+        ple_rows(args.iters, flush, rn)
 
 
 if __name__ == "__main__" and "--configs" not in sys.argv:

@@ -13,6 +13,7 @@ from __future__ import annotations
 import torch
 
 from recalgorithm_b200 import autograd
+from recalgorithm_b200 import feature_column as fc
 from recalgorithm_b200 import layers as L
 
 
@@ -196,3 +197,19 @@ def ple_logits(dense_input, category_input, labels, task_names=("read_comment", 
     losses = [torch.nn.functional.binary_cross_entropy_with_logits(logit, labels[task_name])          # :251-254
               for logit, task_name in zip(logits, task_names)]
     return logits, sum(losses[1:], losses[0])
+
+
+def wide_and_deep_logit(features, wide_part_feature_columns, deep_part_feature_columns, hidden_units=(512, 256, 128),
+                        ctx=None):
+    """WideAndDeep/wide_and_deep.py:207-225.  The wide part is the crossed indicator columns' dense(1) (one hashed gather-sum
+    kernel per column each way) in scope wide_part; its variables are what optim.Ftrl trains (:254-257).  The deep part is
+    input_layer plus the relu dense stack in scope deep_part (its dropout and batch norm left out); the embedding tables'
+    IndexedSlices gradients go to ctx (feature_column.LookupContext)."""
+    with L.variable_scope("wide_part", reuse=L.AUTO_REUSE):                               # :208-210
+        wide_logit = fc.indicator_dense(features, wide_part_feature_columns, units=1, name="wide_part_variables")
+    with L.variable_scope("deep_part"):                                                   # :213-222 (TF names dense, dense_1, ...)
+        net = fc.input_layer(features, deep_part_feature_columns, ctx=ctx)
+        for i, unit in enumerate(hidden_units):
+            net = dense(net, unit, activation=torch.relu, name=f"dense_{i}" if i else "dense")
+        deep_logit = dense(net, 1, name=f"dense_{len(hidden_units)}" if hidden_units else "dense")
+    return wide_logit + deep_logit                                                        # :225

@@ -219,6 +219,29 @@ int ctr_adam_rows_dedup(float* var, float* m, float* v, int64_t state_stride, in
 int ctr_first_order_fwd(const float* w, const int64_t* field_row_offset, const int64_t* ids, int64_t B, int64_t F,
                         float bias, float* out, void* stream);
 
+/* ---- Wide & Deep wide part: hashed crossed column @ dense(1), FTRL-Proximal --------------------------
+ * Replaces indicator_column(crossed_column([userid, manual_tag_list], hash_bucket_size=100000)) -> fc.input_layer ->
+ * tf.layers.dense(wide_input, 1) (WideAndDeep/wide_and_deep.py:121-122,208-210) without the (B, num_buckets) multi-hot.
+ * values (nnz) int64 vocabulary ids of the K keys (OOV -1 is hashed like any id); offsets (K, B+1) int64: key k of sample b is
+ * values[offsets[k,b] : offsets[k,b+1]].  The crosses of b are the Cartesian product of its keys' values, last key fastest
+ * (none if a key is empty); the bucket of (v_1..v_K) is  h = hash_key; h = FingerprintCat64(h, (uint64) v_k) for each k;
+ * h % num_buckets  (SURVEY A.11; TF's default hash_key is 0xDECAFCAFFE).
+ * Forward: out[b] = *bias + sum over b's crosses of kernel[bucket] (duplicates count); bias is read on the device.
+ * Backward: d_kernel (num_buckets) is OVERWRITTEN with the dense gradient multi_hot^T d_logit; d_bias (1), optional, with
+ * sum_b d_logit[b].  2 <= K <= 4 and 2 <= num_buckets < 2^31, else CTR_ERR_UNSUPPORTED.  B = 0 launches no kernel (the
+ * backward still zeroes d_kernel and d_bias). */
+int ctr_crossed_indicator_fwd(const int64_t* values, const int64_t* offsets, int64_t K, int64_t B, int64_t num_buckets,
+                              uint64_t hash_key, const float* kernel, const float* bias, float* out, void* stream);
+int ctr_crossed_indicator_bwd(const int64_t* values, const int64_t* offsets, int64_t K, int64_t B, int64_t num_buckets,
+                              uint64_t hash_key, const float* d_logit, float* d_kernel, float* d_bias, void* stream);
+/* TF's dense ApplyFtrl (tf.train.FtrlOptimizer, wide_and_deep.py:254-257; SURVEY A.12) on n elements, in place:
+ *   new_accum = accum + g^2;  linear += g - (new_accum^-p - accum^-p) / lr * var;  y = new_accum^-p / lr + 2 l2;
+ *   var = |linear| > l1 ? (l1 sign(linear) - linear) / y : 0;  accum = new_accum          (p = lr_power; sqrt at p = -0.5)
+ * lr > 0, lr_power <= 0, l1 >= 0 and l2 >= 0 as TF takes them, else CTR_ERR_INVALID_ARG.  Any float-aligned buffers: the pass
+ * is 128-bit wide when the four share their offset within 16 bytes, element-wise otherwise. */
+int ctr_ftrl_apply(float* var, float* accum, float* linear, const float* grad, int64_t n, float lr, float lr_power, float l1,
+                   float l2, void* stream);
+
 /* ---- Row L (general): multi-valued bag lookup, combiner='mean' ----------------------------------
  * Replaces fc.input_layer over embedding_column(col, D, combiner='mean') on a VarLen feature
  * (DCN/dcn.py:98,103; xDeepFM/xdeepfm.py:103,108) and any single-valued column whose D is not a

@@ -71,6 +71,9 @@ SIGNATURES = {
                                     ctypes.c_float, _P, _P, _P]),
     "ctr_adam_dense_rest": (c_int, [_P, _P, _P, _I, _I, _I, ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_float, _P, _P]),
     "ctr_first_order_fwd": (c_int, [_P, _P, _P, _I, _I, ctypes.c_float, _P, _P]),
+    "ctr_crossed_indicator_fwd": (c_int, [_P, _P, _I, _I, _I, ctypes.c_uint64, _P, _P, _P, _P]),
+    "ctr_crossed_indicator_bwd": (c_int, [_P, _P, _I, _I, _I, ctypes.c_uint64, _P, _P, _P, _P]),
+    "ctr_ftrl_apply": (c_int, [_P, _P, _P, _P, _I, ctypes.c_float, ctypes.c_float, ctypes.c_float, ctypes.c_float, _P]),
     "ctr_bag_lookup_fwd": (c_int, [_P, _I, _I, _P, _P, _I, _P, _I, _P]),
     "ctr_bag_lookup_bwd": (c_int, [_P, _I, _I, _I, _P, _P, _I, _P, _P]),
     "ctr_cross_fwd": (c_int, [_P, _P, _P, _P, _I, _I, _I, _P, _P]),

@@ -8,6 +8,8 @@ Same names and argument meaning as the reference's ``create_feature_columns()`` 
     shared   = fc.shared_embedding_columns([feedid, his_seq], 16, combiner='mean')
     x        = fc.input_layer(features, [userid_e, ...])            # (B, sum d), columns sorted by NAME
     seq, n   = fc.sequence_input_layer(features, [shared[1]])       # (B, T, D), (B,)
+    cross    = fc.indicator_column(fc.crossed_column([userid, manual_tag_list], hash_bucket_size=100000))
+    wide     = fc.indicator_dense(features, [cross], units=1, name="wide_part_variables")   # (B, 1)
 
 ``features`` is what ``io.parse_example`` returns (ragged byte strings per key, dense floats for numeric keys).
 String -> id mapping runs on the host (vocabulary dict); everything after it is one kernel call per column
@@ -73,12 +75,28 @@ class EmbeddingColumn:
 
 
 @dataclass(eq=False)
-class IndicatorColumn:
-    categorical_column: CategoricalColumn
+class CrossedColumn:
+    """tf.feature_column.crossed_column over categorical columns: hashes the keys' vocabulary ids (SURVEY A.11)."""
+    keys: Tuple[CategoricalColumn, ...]
+    hash_bucket_size: int
+    hash_key: int = ops.CROSS_HASH_KEY
 
     @property
     def name(self):
-        return f"{self.categorical_column.key}_indicator"
+        return "_X_".join(sorted(k.key for k in self.keys))
+
+    @property
+    def num_buckets(self):
+        return self.hash_bucket_size
+
+
+@dataclass(eq=False)
+class IndicatorColumn:
+    categorical_column: object                  # CategoricalColumn | CrossedColumn
+
+    @property
+    def name(self):
+        return f"{self.categorical_column.name}_indicator"
 
 
 def categorical_column_with_vocabulary_file(key, vocabulary_file, vocabulary_size=None, num_oov_buckets=0, default_value=None):
@@ -110,8 +128,33 @@ def shared_embedding_columns(categorical_columns, dimension, combiner="mean"):
     return [EmbeddingColumn(c, int(dimension), combiner, shared_name=shared) for c in categorical_columns]
 
 
+def crossed_column(keys, hash_bucket_size, hash_key=None):
+    """The cross of 2 to 4 categorical columns (WideAndDeep/wide_and_deep.py:121).  Raw-string keys (TF hashes their strings
+    with Fingerprint64) and crosses of crosses are not implemented."""
+    keys = list(keys) if keys is not None else []
+    if not hash_bucket_size or hash_bucket_size <= 1:
+        raise ValueError(f"hash_bucket_size must be > 1. hash_bucket_size: {hash_bucket_size}")
+    if len(keys) < 2:
+        raise ValueError(f"keys must be a list with length > 1. Given: {keys}")
+    if len(keys) > 4:
+        raise ValueError(f"crossed_column: at most 4 keys are implemented, got {len(keys)}")
+    for k in keys:
+        if not isinstance(k, CategoricalColumn):
+            raise ValueError(f"crossed_column: keys must be categorical columns (string keys are not implemented), got {k!r}")
+    if int(hash_bucket_size) >= 2 ** 31:
+        raise ValueError(f"crossed_column: hash_bucket_size must be < 2**31, got {hash_bucket_size}")
+    # sparse_cross_hashed takes `hash_key if hash_key else _DEFAULT_HASH_KEY`: None and 0 both mean the default
+    return CrossedColumn(tuple(keys), int(hash_bucket_size), int(hash_key) if hash_key else ops.CROSS_HASH_KEY)
+
+
 def indicator_column(categorical_column):
     return IndicatorColumn(categorical_column)
+
+
+def _base_columns(c) -> List[CategoricalColumn]:
+    """The categorical columns a feature column reads (a crossed column reads each of its keys)."""
+    base = c if isinstance(c, (CategoricalColumn, CrossedColumn)) else c.categorical_column
+    return list(base.keys) if isinstance(base, CrossedColumn) else [base]
 
 
 def make_parse_example_spec(feature_columns) -> Dict[str, object]:
@@ -121,8 +164,8 @@ def make_parse_example_spec(feature_columns) -> Dict[str, object]:
         if isinstance(c, NumericColumn):
             spec[c.key] = FixedLenFeature(c.shape, "float", c.default_value)
         else:
-            base = c if isinstance(c, CategoricalColumn) else c.categorical_column
-            spec[base.key] = VarLenFeature("bytes")
+            for base in _base_columns(c):
+                spec[base.key] = VarLenFeature("bytes")
     return spec
 
 
@@ -216,8 +259,8 @@ def parse_example_native(buf, offsets, lengths, feature_columns, read_feature_li
         if isinstance(c, NumericColumn):
             dense[c.key] = (int(np.prod(c.shape)), float(c.default_value))
         else:
-            base = c if isinstance(c, CategoricalColumn) else c.categorical_column
-            cats[base.key] = base.vocabulary.native()
+            for base in _base_columns(c):
+                cats[base.key] = base.vocabulary.native()
     out = native.parse_examples(buf, offsets, lengths, cats, dense, read_feature_lists=read_feature_lists, num_threads=num_threads)
     for c in feature_columns:
         if isinstance(c, NumericColumn):
@@ -296,6 +339,11 @@ def indicator_dense(features, indicator_columns, units: int = 1, name: str = "fm
     if units != 1:
         raise ValueError("only units=1 (the reference's first-order term) is implemented")
     cols = sorted(indicator_columns, key=lambda c: c.name)
+    crossed = [isinstance(c.categorical_column, CrossedColumn) for c in cols]
+    if any(crossed):
+        if not all(crossed):
+            raise ValueError("indicator_dense: a list that mixes crossed and plain indicator columns is not implemented")
+        return _crossed_dense(features, cols, name, device)
     sizes = [c.categorical_column.num_buckets for c in cols]
     with layers.variable_scope(name):
         kernel = layers.get_variable("kernel", (sum(sizes), 1))
@@ -334,3 +382,58 @@ class _FirstOrder(torch.autograd.Function):
         dk = torch.zeros(ctx.shape, dtype=g.dtype, device=g.device)
         dk.index_add_(0, gr, g.expand(-1, ids.shape[1])[valid].unsqueeze(-1))   # tiny (sum V, 1) dense(1) kernel gradient
         return dk, g.sum().reshape(1), None, None
+
+
+def crossed_ragged_ids(features, col: CrossedColumn) -> Tuple[np.ndarray, np.ndarray]:
+    """The keys of a crossed column as one ragged block: values (nnz,) int64 vocabulary ids (OOV -1 kept) and offsets (K, B+1)
+    int64, key k of sample b = values[offsets[k,b] : offsets[k,b+1]] (the input of ctr_crossed_indicator_fwd / _bwd)."""
+    vals, offs, base = [], [], 0
+    for k in col.keys:
+        values, offsets = features[k.key]
+        offsets = np.asarray(offsets, np.int64)
+        vals.append(np.asarray(_ids_of(k, values), np.int64))
+        offs.append(offsets + base)
+        base += len(vals[-1])
+    if len({len(o) for o in offs}) != 1:
+        raise ValueError(f"crossed column {col.name}: its keys hold different batch sizes")
+    return np.concatenate(vals), np.stack(offs)
+
+
+def _crossed_dense(features, cols, name, device) -> torch.Tensor:
+    """indicator_dense over crossed indicator columns (WideAndDeep/wide_and_deep.py:208-210): one (sum buckets, 1) kernel with
+    the columns' blocks in name order; each block is one hashed gather-sum per sample, and the crossed ids never exist."""
+    sizes = [c.categorical_column.num_buckets for c in cols]
+    with layers.variable_scope(name):
+        kernel = layers.get_variable("kernel", (sum(sizes), 1))
+        bias = layers.get_variable("bias", (1,), initializer=lambda s: torch.zeros(s))
+    blocks, lo = [], 0
+    for c, nb in zip(cols, sizes):
+        values, offsets = crossed_ragged_ids(features, c.categorical_column)
+        blocks.append((torch.from_numpy(values).to(device), torch.from_numpy(offsets).to(device), lo, nb, c.categorical_column.hash_key))
+        lo += nb
+    return _CrossedDense.apply(kernel, bias, blocks)
+
+
+class _CrossedDense(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, kernel, bias, blocks):
+        ctx.blocks, ctx.shape = blocks, kernel.shape
+        w = kernel.data.reshape(-1)
+        out = None
+        for values, offsets, lo, nb, hash_key in blocks:
+            # the bias goes into the first block's launch (read on the device); later blocks add a zero bias
+            b = bias.data if out is None else torch.zeros((1,), dtype=torch.float32, device=w.device)
+            y = ops.crossed_indicator_fwd(values, offsets, nb, w[lo:lo + nb], b, hash_key)
+            out = y if out is None else out + y
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        g = g.contiguous()
+        dk, db = [], None
+        for values, offsets, lo, nb, hash_key in ctx.blocks:
+            d, b = ops.crossed_indicator_bwd(values, offsets, nb, g, hash_key, want_bias=db is None)
+            dk.append(d)
+            db = b if db is None else db
+        dk = dk[0] if len(dk) == 1 else torch.cat(dk)
+        return dk.reshape(ctx.shape), db, None

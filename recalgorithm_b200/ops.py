@@ -193,6 +193,46 @@ def first_order_fwd(w: torch.Tensor, field_row_offset: torch.Tensor, ids: torch.
     return out
 
 
+CROSS_HASH_KEY = 0xDECAFCAFFE        # TF's default hash_key of crossed_column / sparse_cross_hashed
+
+
+def crossed_indicator_fwd(values: torch.Tensor, offsets: torch.Tensor, num_buckets: int, kernel: torch.Tensor, bias: torch.Tensor,
+                          hash_key: int = CROSS_HASH_KEY) -> torch.Tensor:
+    """Wide logit (B,1) of one hashed crossed column: bias + sum over each sample's crosses of kernel[bucket].  values (nnz,)
+    int64 ids of the K keys; offsets (K, B+1) int64 (key k of sample b = values[offsets[k,b]:offsets[k,b+1]]); kernel
+    (num_buckets,); bias (1,) read on the device."""
+    K, B = offsets.shape[0], offsets.shape[1] - 1
+    _chk(values, I64, "values"); _chk(offsets, I64, "offsets"); _chk(kernel, F32, "kernel", (num_buckets,)); _chk(bias, F32, "bias", (1,))
+    out = torch.empty((B, 1), dtype=F32, device=kernel.device)
+    _lib.check(_lib.lib().ctr_crossed_indicator_fwd(_ptr(values), _ptr(offsets), K, B, num_buckets, hash_key, _ptr(kernel), _ptr(bias),
+                                                    _ptr(out), _stream()))
+    return out
+
+
+def crossed_indicator_bwd(values: torch.Tensor, offsets: torch.Tensor, num_buckets: int, d_logit: torch.Tensor,
+                          hash_key: int = CROSS_HASH_KEY, want_bias: bool = True):
+    """Dense gradients of the wide logit: (d_kernel (num_buckets,), d_bias (1,) | None)."""
+    K, B = offsets.shape[0], offsets.shape[1] - 1
+    _chk(values, I64, "values"); _chk(offsets, I64, "offsets"); _chk(d_logit, F32, "d_logit")
+    if d_logit.numel() != B:
+        raise ValueError(f"d_logit: expected {B} elements, got {d_logit.numel()}")
+    d_kernel = torch.empty((num_buckets,), dtype=F32, device=d_logit.device)
+    d_bias = torch.empty((1,), dtype=F32, device=d_logit.device) if want_bias else None
+    _lib.check(_lib.lib().ctr_crossed_indicator_bwd(_ptr(values), _ptr(offsets), K, B, num_buckets, hash_key, _ptr(d_logit),
+                                                    _ptr(d_kernel), _ptr(d_bias), _stream()))
+    return d_kernel, d_bias
+
+
+def ftrl_apply(var: torch.Tensor, accum: torch.Tensor, linear: torch.Tensor, grad: torch.Tensor, lr: float, lr_power: float = -0.5,
+               l1: float = 0.0, l2: float = 0.0) -> None:
+    """TF's dense ApplyFtrl, in place on var, accum and linear (same shape as grad, contiguous)."""
+    n = var.numel()
+    for t, name in ((var, "var"), (accum, "accum"), (linear, "linear"), (grad, "grad")):
+        _chk(t, F32, name, tuple(var.shape))
+    _lib.check(_lib.lib().ctr_ftrl_apply(_ptr(var), _ptr(accum), _ptr(linear), _ptr(grad), n, float(lr), float(lr_power), float(l1),
+                                         float(l2), _stream()))
+
+
 def bag_lookup_fwd(table: torch.Tensor, ids: torch.Tensor, offsets: torch.Tensor,
                    out: Optional[torch.Tensor] = None, out_col: int = 0) -> torch.Tensor:
     """Multi-valued lookup, combiner='mean'.  Writes out[:, out_col:out_col+D] of a (B, stride) buffer."""

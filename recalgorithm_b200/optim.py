@@ -5,6 +5,9 @@ whose gradient is IndexedSlices (DeepFM/deepfm.py:246-250): duplicates summed fi
 updated for EVERY row each step [TF-internal, SURVEY A.8].  ``lazy=True`` is DIEN's LazyAdamOptimizer
 (DIEN/dien.py:328): only the referenced rows move.  De-duplication, row sums, updates and the dense sweep are kernels of
 libctr_b200.so (ctr_adam_indexed_slices: claim / merge / update, no sort and no host round trip).
+
+``Ftrl(var_list, learning_rate)`` is ``tf.train.FtrlOptimizer`` on dense gradients (the Wide & Deep wide part,
+WideAndDeep/wide_and_deep.py:254-257): TF's dense ApplyFtrl on every element of every variable (``ctr_ftrl_apply``).
 """
 from __future__ import annotations
 
@@ -154,3 +157,45 @@ class ShardedTableAdam:
 
     def last_unique_rows(self) -> int:
         return int(self._n_unique.item())
+
+
+class Ftrl:
+    """``tf.train.FtrlOptimizer(learning_rate, learning_rate_power, initial_accumulator_value, l1_regularization_strength,
+    l2_regularization_strength)`` applied to variables whose ``.grad`` is dense (SURVEY A.12): slots ``accum`` (starts at
+    initial_accumulator_value) and ``linear`` (starts at 0) per variable, one ``ctr_ftrl_apply`` per variable and step.
+    l2_shrinkage_regularization_strength (TF's ApplyFtrlV2) is not implemented."""
+
+    def __init__(self, var_list, learning_rate: float, learning_rate_power: float = -0.5, initial_accumulator_value: float = 0.1,
+                 l1_regularization_strength: float = 0.0, l2_regularization_strength: float = 0.0,
+                 l2_shrinkage_regularization_strength: float = 0.0):
+        if initial_accumulator_value < 0.0:
+            raise ValueError(f"initial_accumulator_value {initial_accumulator_value} needs to be positive or zero")
+        if learning_rate_power > 0.0:
+            raise ValueError(f"learning_rate_power {learning_rate_power} needs to be negative or zero")
+        if l1_regularization_strength < 0.0:
+            raise ValueError(f"l1_regularization_strength {l1_regularization_strength} needs to be positive or zero")
+        if l2_regularization_strength < 0.0:
+            raise ValueError(f"l2_regularization_strength {l2_regularization_strength} needs to be positive or zero")
+        if l2_shrinkage_regularization_strength != 0.0:
+            raise ValueError("l2_shrinkage_regularization_strength is not implemented (only TF's ApplyFtrl, shrinkage 0)")
+        self.var_list = list(var_list)
+        self.lr, self.lr_power = float(learning_rate), float(learning_rate_power)
+        self.l1, self.l2 = float(l1_regularization_strength), float(l2_regularization_strength)
+        self._slots = {id(v): {"accum": torch.full_like(v.data, float(initial_accumulator_value)), "linear": torch.zeros_like(v.data)}
+                       for v in self.var_list}
+
+    def get_slot(self, var, name: str) -> torch.Tensor:
+        return self._slots[id(var)][name]
+
+    def step(self) -> None:
+        """One FTRL step on every variable that has a gradient; raises if none has (as minimize does)."""
+        have = [v for v in self.var_list if v.grad is not None]
+        if not have:
+            raise ValueError(f"No gradients provided for any variable: {[tuple(v.shape) for v in self.var_list]}")
+        for v in have:
+            sl = self._slots[id(v)]
+            ops.ftrl_apply(v.data, sl["accum"], sl["linear"], v.grad.contiguous(), self.lr, self.lr_power, self.l1, self.l2)
+
+    def zero_grad(self) -> None:
+        for v in self.var_list:
+            v.grad = None

@@ -4,7 +4,7 @@
 Each kernel is timed alone with CUDA events; an L2 flush (a 256 MB write) runs between timed iterations because these
 working sets are flushed from the 50 MB L2.  Prints one JSON line per measurement.
 
-    python tools/bench_layers.py [--iters 20] [--only cin,dcn,din,fibinet]     (also: pairwise, bst, adam, pnn, dien, deepcrossing, mmoe, ple)
+    python tools/bench_layers.py [--iters 20] [--only cin,dcn,din,fibinet]     (also: pairwise, bst, adam, pnn, dien, deepcrossing, mmoe, ple, wide)
 """
 import argparse
 import json
@@ -380,6 +380,101 @@ def ple_rows(iters, flush, rn):
         torch.backends.cuda.matmul.allow_tf32 = prev_tf32
 
 
+def wide_rows(iters, flush):
+    """Wide & Deep wide part: ctr_crossed_indicator_fwd / _bwd on crossed_column([userid, manual_tag_list]) and ctr_ftrl_apply on
+    its kernel, at B = 1024 (the reference batch) and 65 536, num_buckets = 100 000 (the reference) and 10^7.  One userid
+    per sample (uniform over 200 000) and 1-12 tags per sample (uniform; the tag count is an assumption, the reference's data is
+    not here) over 350 tag ids.  Plain torch runs the same computation on the same GPU: the hash in int64 tensor ops, the
+    gather-sum and the scatter with index_add_, FTRL as elementwise ops.  Bytes are what the algorithm moves (ids, offsets,
+    one 4-byte kernel entry per cross, the logit; the backward adds the gradient zeroing; FTRL reads 4 and writes 3 arrays)
+    over kernel time: the cross kernels are gather / scatter bound, FTRL is HBM bound."""
+    print(json.dumps({"wide_card": card()}), flush=True)
+    K64 = 0xc6a4a7935bd1e995 - (1 << 64)                       # kMul as a signed int64
+    low17 = (1 << 17) - 1
+
+    def mix(x):
+        return x ^ ((x >> 47) & low17)                          # logical shift on int64
+
+    def cat64(a, b):
+        r = a ^ K64
+        r = r ^ (mix(b * K64) * K64)
+        r = r * K64
+        return mix(mix(r) * K64)
+
+    def umod(h, n):                                             # uint64 h % n, n < 2^31, in int64 arithmetic
+        hi, lo = (h >> 32) & 0xFFFFFFFF, h & 0xFFFFFFFF
+        return ((hi % n) * ((1 << 32) % n) + lo) % n
+
+    def torch_ids(uid, tags, sample_of_tag, nb):
+        return umod(cat64(cat64(torch.full_like(tags, ops.CROSS_HASH_KEY), uid[sample_of_tag]), tags), nb)
+
+    def torch_fwd(uid, tags, sample_of_tag, kernel, bias, B, nb):
+        ids = torch_ids(uid, tags, sample_of_tag, nb)
+        return torch.zeros(B, device="cuda").index_add_(0, sample_of_tag, kernel[ids]) + bias
+
+    def torch_bwd(uid, tags, sample_of_tag, g, nb):
+        ids = torch_ids(uid, tags, sample_of_tag, nb)
+        return torch.zeros(nb, device="cuda").index_add_(0, ids, g[sample_of_tag]), g.sum()
+
+    def torch_ftrl(var, acc, lin, g, lr):
+        na = acc + g * g
+        lin += g - (na.sqrt() - acc.sqrt()) / lr * var
+        var.copy_(torch.where(lin.abs() > 0, -lin / (na.sqrt() / lr), torch.zeros_like(var)))
+        acc.copy_(na)
+
+    gen = torch.Generator(device="cuda").manual_seed(7)
+    for B in (1024, 65536):
+        n_tags = torch.randint(1, 13, (B,), device="cuda", generator=gen)
+        uid = torch.randint(0, 200000, (B,), device="cuda", generator=gen)
+        tags = torch.randint(0, 350, (int(n_tags.sum()),), device="cuda", generator=gen)
+        values = torch.cat([uid, tags])
+        offsets = torch.stack([torch.arange(B + 1, device="cuda"),
+                               B + torch.cat([torch.zeros(1, dtype=torch.int64, device="cuda"), n_tags.cumsum(0)])]).contiguous()
+        sample_of_tag = torch.repeat_interleave(torch.arange(B, device="cuda"), n_tags)
+        nnz, crosses = values.numel(), tags.numel()
+        for nb in (100000, 10 ** 7):
+            kernel = (torch.rand(nb, device="cuda", generator=gen) * 2 - 1) * (6.0 / (nb + 1)) ** 0.5
+            bias = torch.full((1,), 0.25, device="cuda")
+            g = torch.randn(B, device="cuda", generator=gen)
+            cfg = {"B": B, "num_buckets": nb, "K": 2, "crosses": crosses, "tags_per_sample": "uniform 1..12 (assumed)"}
+            out = ops.crossed_indicator_fwd(values, offsets, nb, kernel, bias)
+            dk, db = ops.crossed_indicator_bwd(values, offsets, nb, g)
+            ref_out = torch_fwd(uid, tags, sample_of_tag, kernel, bias, B, nb)
+            ref_dk, ref_db = torch_bwd(uid, tags, sample_of_tag, g, nb)
+            diff = {"fwd": float((out.reshape(-1) - ref_out).abs().max()), "bwd": float((dk - ref_dk).abs().max())}
+            io = nnz * 8 + 2 * (B + 1) * 8
+            bytes_ = {"fwd": io + crosses * 4 + B * 4, "bwd": io + B * 4 + nb * 4 + crosses * 4}
+            runs = {"fwd": (lambda: ops.crossed_indicator_fwd(values, offsets, nb, kernel, bias),
+                            lambda: torch_fwd(uid, tags, sample_of_tag, kernel, bias, B, nb)),
+                    "bwd": (lambda: ops.crossed_indicator_bwd(values, offsets, nb, g),
+                            lambda: torch_bwd(uid, tags, sample_of_tag, g, nb))}
+            for way in ("fwd", "bwd"):
+                m, bst = timeit(runs[way][0], iters, flush)
+                tm, tbst = timeit(runs[way][1], iters, flush)
+                print(json.dumps({
+                    "kernel": f"crossed_indicator_{way}", "config": cfg, "ms_median": m, "ms_best": bst,
+                    "torch_ms_median": tm, "torch_ms_best": tbst, "speedup_vs_torch": tm / m, "max_abs_diff_vs_torch": diff[way],
+                    "algorithmic_GBps": bytes_[way] / (m * 1e-3) / 1e9, "bound": "gather" if way == "fwd" else "scatter (atomics)",
+                    "l2": "flushed between iterations", "note": "bytes are algorithmic (4 B per gathered / scattered kernel entry)"}),
+                    flush=True)
+    for n in (100000, 10 ** 7):
+        var = torch.randn(n, device="cuda", generator=gen) * 0.01
+        acc, lin = torch.full((n,), 0.1, device="cuda"), torch.zeros(n, device="cuda")
+        grad = torch.randn(n, device="cuda", generator=gen)
+        tv, ta, tl = var.clone(), acc.clone(), lin.clone()
+        ops.ftrl_apply(var, acc, lin, grad, 0.005)
+        torch_ftrl(tv, ta, tl, grad, 0.005)
+        diff = float((var - tv).abs().max() / tv.abs().max())
+        m, bst = timeit(lambda: ops.ftrl_apply(var, acc, lin, grad, 0.005), iters, flush)
+        tm, tbst = timeit(lambda: torch_ftrl(tv, ta, tl, grad, 0.005), iters, flush)
+        print(json.dumps({
+            "kernel": "ftrl_apply", "config": {"n": n, "lr": 0.005, "lr_power": -0.5}, "ms_median": m, "ms_best": bst,
+            "torch_ms_median": tm, "torch_ms_best": tbst, "speedup_vs_torch": tm / m, "max_norm_rel_diff_vs_torch": diff,
+            "algorithmic_GBps": 28 * n / (m * 1e-3) / 1e9, "frac_of_hbm_3_35TBps": 28 * n / (m * 1e-3) / 3.35e12, "bound": "HBM",
+            "l2": "flushed between iterations", "note": "28 B per element (read var, accum, linear, grad; write var, accum, linear)"}),
+            flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=20)
@@ -562,6 +657,8 @@ def main():
         mmoe_rows(args.iters, flush, rn)
     if "ple" in only:   # PLE extraction network (d = 82) and final layer (d = 256) at the default row; not in the default list
         ple_rows(args.iters, flush, rn)
+    if "wide" in only:  # Wide & Deep wide part (crossed column, FTRL) at the reference bucket count and 10^7; not in the default list
+        wide_rows(args.iters, flush)
 
 
 if __name__ == "__main__" and "--configs" not in sys.argv:

@@ -154,6 +154,18 @@ def deepcrossing_logit(dense_input, category_input, residual_internal_dim=256, r
     return dense(net, 1)                                                                  # :159
 
 
+def autoint_logit(dense_input, fields_embeddings, att_layer_num=3, att_head_num=2, att_embedding_size=8):
+    """AutoInt (Song et al., CIKM 2019, arXiv:1810.11921; the reference README lists it as a to-do, so there is no reference
+    file to follow): each dense feature m becomes the field x_m v_m with v = `dense_embedding` (n_dense, d), concatenated
+    with the categorical field embeddings (B, F, d); then att_layer_num interacting layers (each opens its own
+    interacting_layer_{i} scope), a flatten and dense(1)."""
+    v = L.get_variable("dense_embedding", (dense_input.shape[-1], fields_embeddings.shape[-1]))
+    net = torch.cat([dense_input.unsqueeze(-1) * v, fields_embeddings], dim=1)
+    for i in range(att_layer_num):                                                        # one kernel each way per layer
+        net = L.interacting_layer(net, att_embedding_size, att_head_num, index=i)
+    return dense(net.reshape(net.shape[0], -1), 1)
+
+
 def mmoe_logits(dense_input, category_input, labels, task_names=("read_comment", "like", "click_avatar"), num_experts=3,
                 expert_hidden_units=512, hidden_units=(512, 256, 128)):
     """MMOE/mmoe.py:205-263: experts, gates and gated sums in one kernel each way, then one tower_layer per task

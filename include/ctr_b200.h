@@ -333,6 +333,28 @@ int ctr_residual_unit_bwd(const float* x, const float* w0, const float* b0, cons
                           const float* out, const float* g_out, int64_t B, int64_t d, int64_t H, float* d_x, float* d_w0,
                           float* d_b0, float* d_w1, float* d_b1, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- AutoInt interacting layer ---------------------------------------------------------------------------
+ * Multi-head self-attention over fields (Song et al., CIKM 2019, arXiv:1810.11921, eq. 5-8).  The reference tree has no
+ * AutoInt code (its README lists AutoInt as a to-do), so this row follows the paper and is checked against a float64
+ * restatement of it:
+ *   Q = x . w_query, K = x . w_key, V = x . w_value, R = x . w_res   x (B,F,d); each w (d, H*dk), head h = columns
+ *                                                                    h*dk .. h*dk+dk-1; no biases;
+ *   A_h = softmax_j(Q_h[i] . K_h[j])  (no 1/sqrt(dk) scaling),  out = relu(concat_h A_h V_h + R)   out (B,F,H*dk).
+ * fp32-class accuracy (3xTF32 on the tensor cores); Q, K, V, R and the scores of the forward stay on chip.
+ * 1 <= F <= 64, 1 <= d <= 128, 1 <= dk <= 64, 1 <= H <= 8, H*dk <= 128 (CTR_ERR_UNSUPPORTED otherwise); B = 0 launches
+ * nothing.  workspace: 128-byte aligned, at least ctr_autoint_workspace_bytes(0, F, d, H, dk) bytes for the forward (the
+ * prepped weights) and ctr_autoint_workspace_bytes(B, F, d, H, dk) for the backward (also the projection gradients,
+ * (B*F, 4*H*dk)).  The backward takes the forward's out (its relu mask) and g_out (B,F,H*dk), and overwrites d_x (B,F,d)
+ * and the four weight gradients (zeros at B = 0). */
+int ctr_autoint_workspace_bytes(int64_t B, int64_t F, int64_t d, int64_t H, int64_t dk, int64_t* bytes);
+int ctr_autoint_fwd(const float* x, const float* w_query, const float* w_key, const float* w_value, const float* w_res,
+                    int64_t B, int64_t F, int64_t d, int64_t H, int64_t dk, float* out, void* workspace,
+                    int64_t workspace_bytes, void* stream);
+int ctr_autoint_bwd(const float* x, const float* w_query, const float* w_key, const float* w_value, const float* w_res,
+                    const float* out, const float* g_out, int64_t B, int64_t F, int64_t d, int64_t H, int64_t dk, float* d_x,
+                    float* d_w_query, float* d_w_key, float* d_w_value, float* d_w_res, void* workspace,
+                    int64_t workspace_bytes, void* stream);
+
 /* ---- MMoE expert-gate layer ------------------------------------------------------------------------------
  * Replaces the experts / gates / tower blocks of mmoe_model_fn (MMOE/mmoe.py:207-236) up to the task towers:
  *   h_e     = relu(x . w_e + b_e)        x (B,d) = concat_all_input; w_experts (E,d,H): w_e = experts/expert_{e}/kernel,

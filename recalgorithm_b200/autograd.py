@@ -456,6 +456,26 @@ def residual_unit(x: torch.Tensor, w0: torch.Tensor, b0: torch.Tensor, w1: torch
     return _ResidualUnit.apply(x, w0, b0, w1, b1)
 
 
+class _AutoInt(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x, w_query, w_key, w_value, w_res, heads, dk):
+        x, w_query, w_key, w_value, w_res = (t.contiguous() for t in (x, w_query, w_key, w_value, w_res))
+        out = ops.autoint_fwd(x, w_query, w_key, w_value, w_res, heads, dk)
+        ctx.save_for_backward(x, w_query, w_key, w_value, w_res, out)   # Q, K, V and the attention are recomputed
+        ctx.cfg = (heads, dk)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        return ops.autoint_bwd(*ctx.saved_tensors, g.contiguous(), *ctx.cfg) + (None, None)
+
+
+def autoint_interacting(x: torch.Tensor, w_query: torch.Tensor, w_key: torch.Tensor, w_value: torch.Tensor,
+                        w_res: torch.Tensor, heads: int, dk: int) -> torch.Tensor:
+    """AutoInt interacting layer: relu(concat_h softmax(Q_h K_h^T) V_h + x . w_res), (B,F,d) -> (B,F,heads*dk)."""
+    return _AutoInt.apply(x, w_query, w_key, w_value, w_res, int(heads), int(dk))
+
+
 class _MMoE(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, w_experts, b_experts, w_gates):

@@ -327,6 +327,23 @@ def residual_unit(input: torch.Tensor, internal_dim=None, index=None) -> torch.T
     return autograd.residual_unit(input, w0, b0, w1, b1)
 
 
+# --------------------------------------------------------------------------------------------------- AutoInt
+def interacting_layer(input: torch.Tensor, att_embedding_size=None, head_num=None, index=None) -> torch.Tensor:
+    """AutoInt interacting layer (Song et al., CIKM 2019, arXiv:1810.11921, eq. 5-8), one kernel each way: multi-head
+    self-attention over the fields of ``input`` (B, F, d) with a residual projection and relu, -> (B, F, head_num *
+    att_embedding_size).
+
+    The reference tree has no AutoInt file, so the variable names are this project's choice: in the caller's scope, a scope
+    ``interacting_layer_{index}`` holding ``query``, ``key``, ``value`` and ``res``, each (d, head_num *
+    att_embedding_size) with the store's default glorot-uniform initializer; head h owns columns h * att_embedding_size ..
+    (h + 1) * att_embedding_size - 1.  The widths go through ``int()`` (a string width works, None raises)."""
+    d = int(input.shape[-1])
+    dk, H = int(att_embedding_size), int(head_num)
+    with variable_scope(f"interacting_layer_{index}"):
+        wq, wk, wv, wr = (get_variable(n, (d, H * dk)) for n in ("query", "key", "value", "res"))
+    return autograd.autoint_interacting(input, wq, wk, wv, wr, H, dk)
+
+
 # --------------------------------------------------------------------------------------------------- MMoE
 def mmoe_experts_gates(concat_all_input: torch.Tensor, num_experts, expert_hidden_units, num_tasks,
                        return_gates: bool = False):

@@ -796,6 +796,51 @@ def residual_unit_bwd(x, w0, b0, w1, b1, out, g_out):
     return d_x, d_w0, d_b0, d_w1, d_b1
 
 
+# ------------------------------------------------------------------------------------ AutoInt interacting layer
+def autoint_workspace(B: int, F: int, d: int, H: int, dk: int, device) -> torch.Tensor:
+    """Caller-owned workspace: the prepped weights (B = 0, what the forward needs) plus, for the backward, the per-row
+    projection gradients (B*F, 4*H*dk)."""
+    nbytes = ctypes.c_int64(0)
+    _lib.check(_lib.lib().ctr_autoint_workspace_bytes(B, F, d, H, dk, ctypes.byref(nbytes)))
+    return torch.empty((int(nbytes.value),), dtype=torch.uint8, device=device)
+
+
+def _autoint_args(x, wq, wk, wv, wr, heads, dk):
+    _chk(x, F32, "input")
+    if x.dim() != 3:
+        raise ValueError(f"input must be (B, F, d), got shape {tuple(x.shape)}")
+    B, F, d = x.shape
+    H, dk = int(heads), int(dk)
+    for name, w in (("w_query", wq), ("w_key", wk), ("w_value", wv), ("w_res", wr)):
+        _chk(w, F32, name, (d, H * dk))
+    return B, F, d, H, dk
+
+
+def autoint_fwd(x, w_query, w_key, w_value, w_res, heads: int, dk: int) -> torch.Tensor:
+    """AutoInt interacting layer (arXiv:1810.11921 eq. 5-8): relu(concat_h softmax(Q_h K_h^T) V_h + x . w_res),
+    x (B,F,d), each w (d, heads*dk) -> (B, F, heads*dk)."""
+    B, F, d, H, dk = _autoint_args(x, w_query, w_key, w_value, w_res, heads, dk)
+    out = torch.empty((B, F, H * dk), dtype=F32, device=x.device)
+    ws = autoint_workspace(0, F, d, H, dk, x.device)
+    _lib.check(_lib.lib().ctr_autoint_fwd(_ptr(x), _ptr(w_query), _ptr(w_key), _ptr(w_value), _ptr(w_res), B, F, d, H, dk,
+                                          _ptr(out), _ptr(ws), ws.numel(), _stream()))
+    return out
+
+
+def autoint_bwd(x, w_query, w_key, w_value, w_res, out, g_out, heads: int, dk: int):
+    """Gradients of autoint_fwd given its output `out` (the relu mask) and g_out (B,F,heads*dk):
+    (d_x, d_w_query, d_w_key, d_w_value, d_w_res).  Q, K, V and the attention are recomputed from x."""
+    B, F, d, H, dk = _autoint_args(x, w_query, w_key, w_value, w_res, heads, dk)
+    _chk(out, F32, "out", (B, F, H * dk)); _chk(g_out, F32, "g_out", (B, F, H * dk))
+    d_x = torch.empty_like(x)
+    dws = [torch.empty_like(w) for w in (w_query, w_key, w_value, w_res)]
+    ws = autoint_workspace(B, F, d, H, dk, x.device)
+    _lib.check(_lib.lib().ctr_autoint_bwd(_ptr(x), _ptr(w_query), _ptr(w_key), _ptr(w_value), _ptr(w_res), _ptr(out),
+                                          _ptr(g_out), B, F, d, H, dk, _ptr(d_x), *(_ptr(t) for t in dws), _ptr(ws),
+                                          ws.numel(), _stream()))
+    return (d_x, *dws)
+
+
 # ------------------------------------------------------------------------------------ MMoE expert-gate layer
 def mmoe_workspace(B: int, d: int, E: int, H: int, T: int, device) -> torch.Tensor:
     """Caller-owned workspace: the prepped weights (B = 0, what the forward needs) plus, for the backward, the expert and

@@ -4,7 +4,7 @@
 Each kernel is timed alone with CUDA events; an L2 flush (a 256 MB write) runs between timed iterations because these
 working sets are flushed from the 50 MB L2.  Prints one JSON line per measurement.
 
-    python tools/bench_layers.py [--iters 20] [--only cin,dcn,din,fibinet]     (also: pairwise, bst, adam, pnn, dien, deepcrossing, mmoe, ple, wide)
+    python tools/bench_layers.py [--iters 20] [--only cin,dcn,din,fibinet]     (also: pairwise, bst, adam, pnn, dien, deepcrossing, mmoe, ple, wide, autoint)
 """
 import argparse
 import json
@@ -475,6 +475,72 @@ def wide_rows(iters, flush):
             flush=True)
 
 
+def autoint_rows(iters, flush, rn):
+    """AutoInt interacting layer (ctr_autoint_fwd / _bwd) at the paper's setting F = 40, H = 2, dk = 32, for the first layer
+    (d = 16) and a later one (d = 64), B = 1024 and 65 536; plus DeepCTR's default head width dk = 8 at B = 65 536 (heads
+    are padded to 32 columns, so that row spends 4x the padded work).  Each row is timed next to plain torch running the
+    same layer: fp32 matmuls with TF32 off, F.scaled_dot_product_attention(..., scale=1.0), the residual matmul and relu,
+    autograd for the backward.  Algorithmic FLOPs: projections 2 B F d 4 H dk, attention 4 B H F^2 dk (forward); the
+    backward recomputes Q, K, V and the scores and adds dx and dW (2.75x the projections, 2.5x the attention).  Floors from
+    data-sheet rates of the H100 SXM (700 W), not measured: 3 x FLOPs (3xTF32) over 495 TFLOP/s, and bytes over 3.35 TB/s
+    (forward x + out; backward x, out, g_out, d_x plus the staged projection gradients, written once and read twice)."""
+    import torch.nn.functional as Fn
+    print(json.dumps({"autoint_card": card()}), flush=True)
+    F = 40
+
+    def torch_pre(x, wq, wk, wv, wr, H, dk):
+        B = x.shape[0]
+        heads = lambda t: t.reshape(B, F, H, dk).transpose(1, 2)
+        o = Fn.scaled_dot_product_attention(heads(x @ wq), heads(x @ wk), heads(x @ wv), scale=1.0)
+        return o.transpose(1, 2).reshape(B, F, H * dk) + x @ wr
+
+    def torch_form(x, wq, wk, wv, wr, H, dk):
+        return torch.relu(torch_pre(x, wq, wk, wv, wr, H, dk))
+
+    prev_tf32 = torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cuda.matmul.allow_tf32 = False
+    try:
+        shapes = [(d, 2, 32, B) for d in (16, 64) for B in (1024, 65536)] + [(16, 2, 8, 65536)]
+        for d, H, dk, B in shapes:
+            HD = H * dk
+            ws = [rn(d, HD, std=(1.0 / d) ** 0.5) for _ in range(4)]
+            x, g = rn(B, F, d), rn(B, F, HD)
+            cfg = {"B": B, "F": F, "d": d, "H": H, "dk": dk}
+            proj, attn = 2.0 * B * F * d * 4 * HD, 4.0 * B * H * F * F * dk
+            flops = {"fwd": proj + attn, "bwd": 2.75 * proj + 2.5 * attn}
+            hbm = {"fwd": 4.0 * B * F * (d + HD), "bwd": 4.0 * B * F * (2 * d + 2 * HD) + 3 * 4.0 * B * F * 4 * HD}
+            out = ops.autoint_fwd(x, *ws, H, dk)
+            grads = ops.autoint_bwd(x, *ws, out, g, H, dk)
+            ps = [t.clone().requires_grad_() for t in (x, *ws)]
+            ref_out = torch_form(*ps, H, dk)
+            ref_grads = torch.autograd.grad(ref_out, ps, g, retain_graph=True)
+            # the gradient comparison takes the relu mask from the kernel's out: where the two forwards round to opposite
+            # sides of 0, comparing each against its own mask would measure that flip, not the backward
+            masked = torch.autograd.grad(torch_pre(*ps, H, dk), ps, g * (out > 0))
+            diff = {"fwd": float((ref_out.detach() - out).abs().max() / ref_out.detach().abs().max()),
+                    "bwd": max(float((a - b).abs().max() / b.abs().max()) for a, b in zip(grads, masked))}
+            del masked
+            runs = {"fwd": (lambda: ops.autoint_fwd(x, *ws, H, dk), lambda: torch_form(x, *ws, H, dk)),
+                    "bwd": (lambda: ops.autoint_bwd(x, *ws, out, g, H, dk),
+                            lambda: torch.autograd.grad(ref_out, ps, g, retain_graph=True))}
+            for way in ("fwd", "bwd"):
+                m, bst = timeit(runs[way][0], iters, flush)
+                tm, tbst = timeit(runs[way][1], iters, flush)
+                f_tc, f_hbm = 3 * flops[way] / 495e12 * 1e6, hbm[way] / 3.35e12 * 1e6
+                print(json.dumps({
+                    "kernel": f"autoint_{way}", "config": cfg, "ms_median": m, "ms_best": bst,
+                    "torch_fp32_ms_median": tm, "torch_fp32_ms_best": tbst, "speedup_vs_torch": tm / m,
+                    "max_norm_rel_diff_vs_torch": diff[way], "l2": "flushed between iterations",
+                    "algorithmic_TFLOPs": flops[way] / (m * 1e-3) / 1e12, "algorithmic_GBps": hbm[way] / (m * 1e-3) / 1e9,
+                    "floor_3xtf32_us": f_tc, "floor_hbm_us": f_hbm, "bound": "tensor" if f_tc >= f_hbm else "hbm",
+                    "floor_over_kernel": max(f_tc, f_hbm) / (m * 1e3),
+                    "note": "floors are data-sheet rates (H100 SXM, 700 W), not measured; torch: same layer, fp32, TF32 off"}),
+                    flush=True)
+            del out, grads, ps, ref_out, ref_grads
+    finally:
+        torch.backends.cuda.matmul.allow_tf32 = prev_tf32
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=20)
@@ -659,6 +725,8 @@ def main():
         ple_rows(args.iters, flush, rn)
     if "wide" in only:  # Wide & Deep wide part (crossed column, FTRL) at the reference bucket count and 10^7; not in the default list
         wide_rows(args.iters, flush)
+    if "autoint" in only:  # AutoInt interacting layer at the paper's setting (F = 40, H = 2, dk = 32, d = 16 and 64); not in the default list
+        autoint_rows(args.iters, flush, rn)
 
 
 if __name__ == "__main__" and "--configs" not in sys.argv:

@@ -166,6 +166,21 @@ def autoint_logit(dense_input, fields_embeddings, att_layer_num=3, att_head_num=
     return dense(net.reshape(net.shape[0], -1), 1)
 
 
+def flen_logit(tables: autograd.EmbeddingTables, ids: torch.Tensor, field_groups, first_order_logit: torch.Tensor,
+               hidden_units=(64, 32)):
+    """FLEN (Chen et al., arXiv:1911.04690; the reference README lists it as a to-do, so there is no reference file to
+    follow): the fused lookup and field-wise bi-interaction h (B, D) in one kernel each way, a DNN over the flattened
+    embeddings, dense(concat([h, dnn]), 1), plus the first-order logit (feature_column.indicator_dense, as for DeepFM).
+    The paper's DiceFactor dropout is left out."""
+    fields_embeddings, h = L.field_wise_bi_interaction_lookup(tables, ids, field_groups)
+    with L.variable_scope("dnn_part"):
+        net = fields_embeddings.reshape(ids.shape[0], -1)
+        for i, unit in enumerate(hidden_units):
+            net = dense(net, unit, activation=torch.relu, name=f"dense_{i}")
+    with L.variable_scope("output_part"):
+        return dense(torch.cat([h, net], dim=-1), 1) + first_order_logit
+
+
 def mmoe_logits(dense_input, category_input, labels, task_names=("read_comment", "like", "click_avatar"), num_experts=3,
                 expert_hidden_units=512, hidden_units=(512, 256, 128)):
     """MMOE/mmoe.py:205-263: experts, gates and gated sums in one kernel each way, then one tower_layer per task

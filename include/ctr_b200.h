@@ -479,6 +479,33 @@ int ctr_embed_bi_fwd(const float* table, const int64_t* field_row_offset, const 
 int ctr_embed_bi_bwd(const float* tile, const float* d_tile, const float* d_bi, int64_t B, int64_t F, int64_t D,
                      float* row_grads, void* stream);
 
+/* FLEN field-wise bi-interaction (FwBI; Chen et al., arXiv:1911.04690).  The reference tree has no FLEN code (its README
+ * lists FLEN as a to-do), so this definition is the contract.  field_group: a HOST array of F int32, each in [0, M), read
+ * before any launch (the call stays capturable in a CUDA graph).  With p_m = sum_{f: group[f]=m} e_f and
+ * q_m = sum_{f: group[f]=m} e_f^2 (element-wise over D):
+ *   h[b,:] = sum_{i<j} kernel_mf[pair(i,j)] p_i p_j + bias_mf + sum_m kernel_fm[m] (p_m^2 - q_m) + bias_fm        h (B,D)
+ * pair(i,j): row-major strict upper triangle of M x M (FwFM's utils.py:67-82 order); kernel_mf (M(M-1)/2,), may be NULL
+ * only when M == 1; kernel_fm (M,); bias_mf, bias_fm (D,).  A group with no field contributes zero; a singleton group's
+ * p_m^2 - q_m is exactly 0.
+ * ctr_embed_fwbi_fwd: the fused gather of ctr_embed_fm2_fwd (ids int64, or int32 with ids_are_int32 != 0, when
+ * ids64_out (nullable) receives the widened ids; OOV / out-of-range ids give zero rows); tile (nullable) receives the rows.
+ * ctr_fwbi_fwd: the same layer over a given (B,F,D) tile.
+ * ctr_fwbi_bwd (both forms): row_grads[b,f,:] = d_tile[b,f,:] (nullable) + d_h[b,:] * (sum_{j != m} kernel_mf[pair(m,j)] p_j
+ * + 2 kernel_fm[m] (p_m - e_f)) for f in group m -- the IndexedSlices values of the fused form, d_tile of the tile form;
+ * overwrites d_kernel_mf (may be NULL only when M == 1), d_kernel_fm, d_bias_mf and d_bias_fm (both sum_b d_h[b,:]), zeros
+ * at B = 0.  D a power of two in 4..128, 1 <= F <= 256, 1 <= M <= 8 (CTR_ERR_UNSUPPORTED otherwise); table, tile, d_tile,
+ * h, d_h and row_grads 16-byte aligned, the weights float-aligned.  B = 0 launches nothing. */
+int ctr_embed_fwbi_fwd(const float* table, const int64_t* field_row_offset, const void* ids, int ids_are_int32, int64_t B,
+                       int64_t F, int64_t D, const int32_t* field_group, int64_t M, const float* kernel_mf,
+                       const float* kernel_fm, const float* bias_mf, const float* bias_fm, float* tile, float* h,
+                       int64_t* ids64_out, void* stream);
+int ctr_fwbi_fwd(const float* tile, int64_t B, int64_t F, int64_t D, const int32_t* field_group, int64_t M,
+                 const float* kernel_mf, const float* kernel_fm, const float* bias_mf, const float* bias_fm, float* h,
+                 void* stream);
+int ctr_fwbi_bwd(const float* tile, const float* d_tile, const float* d_h, int64_t B, int64_t F, int64_t D,
+                 const int32_t* field_group, int64_t M, const float* kernel_mf, const float* kernel_fm, float* row_grads,
+                 float* d_kernel_mf, float* d_kernel_fm, float* d_bias_mf, float* d_bias_fm, void* stream);
+
 /* FwFM second-order logit (FwFM/fwfm.py:140-158): out[b] = sum_{i<j} r[pair(i,j)] * <tile[b,i,:], tile[b,j,:]>, r (F(F-1)/2,)
  * indexed like utils.py:67-82 (row-major strict upper triangle).  Backward: d_tile (B,F,K) and d_r (overwritten). */
 int ctr_fwfm_fwd(const float* tile, const float* r, int64_t B, int64_t F, int64_t K, float* out, void* stream);

@@ -54,6 +54,9 @@ SIGNATURES = {
                               ctypes.c_float, _P, _P]),
     "ctr_embed_bi_fwd": (c_int, [_P, _P, _P, _I, _I, _I, _P, _P, _P]),
     "ctr_embed_bi_bwd": (c_int, [_P, _P, _P, _I, _I, _I, _P, _P]),
+    "ctr_embed_fwbi_fwd": (c_int, [_P, _P, _P, c_int, _I, _I, _I, _P, _I, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "ctr_fwbi_fwd": (c_int, [_P, _I, _I, _I, _P, _I, _P, _P, _P, _P, _P, _P]),
+    "ctr_fwbi_bwd": (c_int, [_P, _P, _P, _I, _I, _I, _P, _I] + [_P] * 8),
     "ctr_fwfm_fwd": (c_int, [_P, _P, _I, _I, _I, _P, _P]),
     "ctr_fwfm_bwd": (c_int, [_P, _P, _P, _I, _I, _I, _P, _P, _P]),
     "ctr_ffm_fwd": (c_int, [_P, _I, _I, _I, _P, _P]),

@@ -314,6 +314,57 @@ def lookup_bi(tables: EmbeddingTables, ids: torch.Tensor):
     return _LookupBI.apply(tables._anchor, tables, ids)
 
 
+class _LookupFwBI(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, anchor, kernel_mf, kernel_fm, bias_mf, bias_fm, tables: EmbeddingTables, ids: torch.Tensor, field_group):
+        ctx.set_materialize_grads(False)            # an unused tile gradient arrives as None and goes down as NULL d_tile
+        ids64 = _ids64_for(ids)
+        kernel_mf, kernel_fm, bias_mf, bias_fm = (t.contiguous() for t in (kernel_mf, kernel_fm, bias_mf, bias_fm))
+        tile, h = ops.embed_fwbi_fwd(tables.weight, tables.field_row_offset, ids, field_group, kernel_mf, kernel_fm, bias_mf,
+                                     bias_fm, ids64_out=ids64)
+        ctx.tables, ctx.ids, ctx.field_group = tables, (ids if ids64 is None else ids64), field_group
+        ctx.save_for_backward(tile, kernel_mf, kernel_fm)
+        return tile, h
+
+    @staticmethod
+    def backward(ctx, d_tile, d_h):
+        tile, kernel_mf, kernel_fm = ctx.saved_tensors
+        if d_tile is None and d_h is None:
+            return (None,) * 8
+        d_tile = d_tile.contiguous() if d_tile is not None else None
+        d_h = d_h.contiguous() if d_h is not None else torch.zeros((tile.shape[0], tile.shape[2]), device=tile.device)
+        values, *dw = ops.fwbi_bwd(tile, d_tile, d_h, ctx.field_group, kernel_mf, kernel_fm)
+        ctx.tables.grad_slices.append(IndexedSlices(values, ctx.ids, ctx.tables.field_row_offset))
+        return (None, *dw, None, None, None)
+
+
+def lookup_fwbi(tables: EmbeddingTables, ids: torch.Tensor, field_group, kernel_mf: torch.Tensor, kernel_fm: torch.Tensor,
+                bias_mf: torch.Tensor, bias_fm: torch.Tensor):
+    """(B,F) ids -> (tile (B,F,D), FLEN field-wise bi-interaction h (B,D)); field_group: F group indices in [0, M),
+    M = len(kernel_fm).  Differentiable w.r.t. the tables (IndexedSlices) and the four weights."""
+    return _LookupFwBI.apply(tables._anchor, kernel_mf, kernel_fm, bias_mf, bias_fm, tables, ids, tuple(field_group))
+
+
+class _FwBI(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, tile, kernel_mf, kernel_fm, bias_mf, bias_fm, field_group):
+        tile, kernel_mf, kernel_fm, bias_mf, bias_fm = (t.contiguous() for t in (tile, kernel_mf, kernel_fm, bias_mf, bias_fm))
+        ctx.save_for_backward(tile, kernel_mf, kernel_fm)
+        ctx.field_group = field_group
+        return ops.fwbi_fwd(tile, field_group, kernel_mf, kernel_fm, bias_mf, bias_fm)
+
+    @staticmethod
+    def backward(ctx, g):
+        tile, kernel_mf, kernel_fm = ctx.saved_tensors
+        return (*ops.fwbi_bwd(tile, None, g.contiguous(), ctx.field_group, kernel_mf, kernel_fm), None)
+
+
+def fwbi(tile: torch.Tensor, field_group, kernel_mf: torch.Tensor, kernel_fm: torch.Tensor, bias_mf: torch.Tensor,
+         bias_fm: torch.Tensor) -> torch.Tensor:
+    """FLEN field-wise bi-interaction of a (B,F,D) tile -> h (B,D) (see lookup_fwbi)."""
+    return _FwBI.apply(tile, kernel_mf, kernel_fm, bias_mf, bias_fm, tuple(field_group))
+
+
 class _FwFM(torch.autograd.Function):
     @staticmethod
     def forward(ctx, tile, r):

@@ -30,12 +30,6 @@ struct PeerTables {
 // NFM/nfm.py:155-168) instead of its sum over D.
 // IdT: int64 ids (TF's sparse ids) or int32 ids (half the PCIe / HBM bytes of the id matrix; `ids64_out`, when given,
 // receives the widened copy that IndexedSlices consumers downstream expect).
-__device__ __forceinline__ long long load_id(const long long* p) { return ldg_stream_i64(p); }
-__device__ __forceinline__ long long load_id(const int* p) {
-  int r;
-  asm volatile("ld.global.nc.L1::no_allocate.s32 %0, [%1];" : "=r"(r) : "l"(p));
-  return (long long)r;
-}
 // rows of a peer shard: plain (L1-allocating) loads -- measured 650 GB/s over NVLink against 622 GB/s for
 // .nc.L1::no_allocate (tools/peerbench.cu); peer lines bypass the local L2 either way
 __device__ __forceinline__ float4 ld_peer_f4(const float4* p) {
@@ -321,16 +315,6 @@ static int launch_fwd_bi(const float* table, const int64_t* off, const int64_t* 
                          reinterpret_cast<const float4*>(table), PeerTables{}, reinterpret_cast<const long long*>(off),
                          reinterpret_cast<const long long*>(ids), (int)B, (int)F, reinterpret_cast<float4*>(tile), bi, nullptr,
                          nullptr, nullptr);
-}
-
-static int check_bfd(const char* fn, int64_t B, int64_t F, int64_t D) {
-  CTR_REQUIRE(B >= 0 && F >= 1 && D >= 1, "%s: bad sizes B=%lld F=%lld D=%lld", fn, (long long)B, (long long)F,
-              (long long)D);
-  CTR_REQUIRE(B <= 0x7fffffffLL / 8 && F <= 65536, "%s: B=%lld / F=%lld too large", fn, (long long)B, (long long)F);
-  CTR_UNSUPPORTED(D % 4 != 0 || D > 128 || (D & (D - 1)) != 0,
-                  "%s: D=%lld unsupported by the fused 128-bit path (need a power of two in 4..128); "
-                  "use ctr_bag_lookup_* for other widths", fn, (long long)D);
-  return CTR_OK;
 }
 
 template <typename IdT>

@@ -13,6 +13,14 @@ namespace ctr {
 
 __device__ __forceinline__ float4 f4_zero() { return make_float4(0.f, 0.f, 0.f, 0.f); }
 
+// A per-field id of the fused lookups: int64 (TF's sparse ids) or int32 (half the bytes of the id matrix), read once.
+__device__ __forceinline__ long long load_id(const long long* p) { return ldg_stream_i64(p); }
+__device__ __forceinline__ long long load_id(const int* p) {
+  int r;
+  asm volatile("ld.global.nc.L1::no_allocate.s32 %0, [%1];" : "=r"(r) : "l"(p));
+  return (long long)r;
+}
+
 // completes a per-lane partial sum over the lanes that hold the same chunk
 template <int LPR>
 __device__ __forceinline__ void lane_group_sum(float4& v) {
@@ -150,6 +158,17 @@ __device__ __forceinline__ void lookup_bwd_sample(const float4* __restrict__ e_r
       sink(0, j, fm2_row_grad(head.at(j, dt), g, S, v));
     }
   }
+}
+
+// Host side: the (B, F, D) bounds of the fused 128-bit row kernels, checked by every entry point `fn` that launches one.
+static int check_bfd(const char* fn, int64_t B, int64_t F, int64_t D) {
+  CTR_REQUIRE(B >= 0 && F >= 1 && D >= 1, "%s: bad sizes B=%lld F=%lld D=%lld", fn, (long long)B, (long long)F,
+              (long long)D);
+  CTR_REQUIRE(B <= 0x7fffffffLL / 8 && F <= 65536, "%s: B=%lld / F=%lld too large", fn, (long long)B, (long long)F);
+  CTR_UNSUPPORTED(D % 4 != 0 || D > 128 || (D & (D - 1)) != 0,
+                  "%s: D=%lld unsupported by the fused 128-bit path (need a power of two in 4..128); "
+                  "use ctr_bag_lookup_* for other widths", fn, (long long)D);
+  return CTR_OK;
 }
 
 // Host side: the HOLD of a sample of F fields of LPR chunks, from its ceil(F*LPR/32) chunks per lane: 4, 8 or 12.  Above

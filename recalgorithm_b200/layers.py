@@ -211,6 +211,48 @@ def fwfm_second_order(fields_embeddings: torch.Tensor) -> torch.Tensor:
     return autograd.fwfm(fields_embeddings, r)
 
 
+FWBI_MAX_GROUPS = 8
+
+
+def _fwbi_variables(field_groups, F: int, D: int):
+    """Numbers the group keys by first appearance and creates ``field_wise_bi_interaction/{kernel_mf, kernel_fm, bias_mf,
+    bias_fm}`` in the caller's scope."""
+    keys = list(field_groups)
+    if len(keys) != F:
+        raise ValueError(f"field_groups has {len(keys)} entries but there are {F} fields")
+    number = {}
+    groups = tuple(number.setdefault(k, len(number)) for k in keys)
+    M = len(number)
+    if M > FWBI_MAX_GROUPS:
+        raise ValueError(f"field_groups has {M} distinct groups; the field-wise bi-interaction supports at most "
+                         f"{FWBI_MAX_GROUPS}")
+    with variable_scope("field_wise_bi_interaction"):
+        kmf = get_variable("kernel_mf", (M * (M - 1) // 2,), initializer=lambda s: torch.ones(s))
+        kfm = get_variable("kernel_fm", (M,), initializer=lambda s: torch.full(s, 0.5))
+        bmf = get_variable("bias_mf", (D,), initializer=lambda s: torch.zeros(s))
+        bfm = get_variable("bias_fm", (D,), initializer=lambda s: torch.zeros(s))
+    return groups, (kmf, kfm, bmf, bfm)
+
+
+def field_wise_bi_interaction(fields_embeddings: torch.Tensor, field_groups) -> torch.Tensor:
+    """FLEN field-wise bi-interaction (Chen et al., arXiv:1911.04690) of the (B,F,D) field embeddings -> h (B,D).
+
+    ``field_groups`` gives each field's group key; group m is the m-th distinct key in order of first appearance (at most
+    8).  h = sum_{i<j} kernel_mf[pair(i,j)] p_i p_j + bias_mf + sum_m kernel_fm[m] (p_m^2 - q_m) + bias_fm, p_m / q_m the
+    sums of the group's embeddings / squared embeddings.  The reference tree has no FLEN file, so the variable names are
+    this project's choice: ``field_wise_bi_interaction/kernel_mf`` (M(M-1)/2,) ones, ``kernel_fm`` (M,) 0.5, ``bias_mf`` and
+    ``bias_fm`` (D,) zeros, in the caller's scope."""
+    groups, w = _fwbi_variables(field_groups, int(fields_embeddings.shape[1]), int(fields_embeddings.shape[2]))
+    return autograd.fwbi(fields_embeddings, groups, *w)
+
+
+def field_wise_bi_interaction_lookup(tables: autograd.EmbeddingTables, ids: torch.Tensor, field_groups):
+    """The lookup and field_wise_bi_interaction in one kernel each way: per-field ids (B,F) -> (fields_embeddings (B,F,D),
+    h (B,D)); same variables as field_wise_bi_interaction."""
+    groups, w = _fwbi_variables(field_groups, int(ids.shape[1]), tables.dim)
+    return autograd.lookup_fwbi(tables, ids, groups, *w)
+
+
 def afm_attention(fields_embeddings: torch.Tensor, embedding_dim: int, attention_factor: int) -> torch.Tensor:
     """AFM/afm.py:152-186: attention-weighted sum of the pairwise hadamard products, (B,K).  Creates
     ``attention_part/attention_{w,b,h}`` with the reference's shapes; ``p`` and the final matmul (afm.py:187-188) stay

@@ -514,6 +514,67 @@ def embed_bi_bwd(tile: torch.Tensor, d_tile: Optional[torch.Tensor], d_bi: torch
     return row_grads
 
 
+def _fwbi_args(field_group, F: int, D: int, kernel_mf, kernel_fm, bias_mf=None, bias_fm=None):
+    """The host int32 group map (kept alive by the caller while the entry reads it) and M = len(kernel_fm)."""
+    M = int(kernel_fm.shape[0]) if kernel_fm.dim() == 1 else -1
+    _chk(kernel_fm, F32, "kernel_fm", (M,)); _chk(kernel_mf, F32, "kernel_mf", (M * (M - 1) // 2,))
+    _chk(bias_mf, F32, "bias_mf", (D,)); _chk(bias_fm, F32, "bias_fm", (D,))
+    groups = [int(g) for g in (field_group.tolist() if torch.is_tensor(field_group) else field_group)]
+    if len(groups) != F:
+        raise ValueError(f"field_group: expected {F} entries (one per field), got {len(groups)}")
+    arr = (ctypes.c_int32 * F)(*groups)
+    return arr, M
+
+
+def embed_fwbi_fwd(table: torch.Tensor, field_row_offset: torch.Tensor, ids: torch.Tensor, field_group, kernel_mf: torch.Tensor,
+                   kernel_fm: torch.Tensor, bias_mf: torch.Tensor, bias_fm: torch.Tensor, want_tile: bool = True,
+                   ids64_out: Optional[torch.Tensor] = None):
+    """Fused lookup + FLEN field-wise bi-interaction.  ids (B,F) int64, or int32 (``ids64_out`` (B,F) i64 then receives the
+    widened copy); field_group: F group indices in [0, M), M = len(kernel_fm); kernel_mf (M(M-1)/2,).
+    Returns (tile (B,F,D) | None, h (B,D))."""
+    B, F = ids.shape
+    D = table.shape[1]
+    _chk(table, F32, "table"); _chk(field_row_offset, I64, "field_row_offset", (F + 1,))
+    i32 = ids.dtype == I32
+    _chk(ids, I32 if i32 else I64, "ids"); _chk(ids64_out, I64, "ids64_out", (B, F))
+    groups, M = _fwbi_args(field_group, F, D, kernel_mf, kernel_fm, bias_mf, bias_fm)
+    tile = torch.empty((B, F, D), dtype=F32, device=table.device) if want_tile else None
+    h = torch.empty((B, D), dtype=F32, device=table.device)
+    _lib.check(_lib.lib().ctr_embed_fwbi_fwd(_ptr(table), _ptr(field_row_offset), _ptr(ids), int(i32), B, F, D,
+                                             ctypes.addressof(groups), M, _ptr(kernel_mf), _ptr(kernel_fm), _ptr(bias_mf),
+                                             _ptr(bias_fm), _ptr(tile), _ptr(h), _ptr(ids64_out), _stream()))
+    return tile, h
+
+
+def fwbi_fwd(tile: torch.Tensor, field_group, kernel_mf: torch.Tensor, kernel_fm: torch.Tensor, bias_mf: torch.Tensor,
+             bias_fm: torch.Tensor) -> torch.Tensor:
+    """FLEN field-wise bi-interaction of a (B,F,D) tile -> h (B,D) (see embed_fwbi_fwd)."""
+    _chk(tile, F32, "tile")
+    B, F, D = tile.shape
+    groups, M = _fwbi_args(field_group, F, D, kernel_mf, kernel_fm, bias_mf, bias_fm)
+    h = torch.empty((B, D), dtype=F32, device=tile.device)
+    _lib.check(_lib.lib().ctr_fwbi_fwd(_ptr(tile), B, F, D, ctypes.addressof(groups), M, _ptr(kernel_mf), _ptr(kernel_fm),
+                                       _ptr(bias_mf), _ptr(bias_fm), _ptr(h), _stream()))
+    return h
+
+
+def fwbi_bwd(tile: torch.Tensor, d_tile: Optional[torch.Tensor], d_h: torch.Tensor, field_group, kernel_mf: torch.Tensor,
+             kernel_fm: torch.Tensor):
+    """Backward of both FwBI forms: (row_grads (B,F,D) = d_tile + the layer's term -- the IndexedSlices values of the fused
+    form --, d_kernel_mf, d_kernel_fm, d_bias_mf, d_bias_fm)."""
+    _chk(tile, F32, "tile")
+    B, F, D = tile.shape
+    _chk(d_tile, F32, "d_tile", (B, F, D)); _chk(d_h, F32, "d_h", (B, D))
+    groups, M = _fwbi_args(field_group, F, D, kernel_mf, kernel_fm)
+    row_grads = torch.empty_like(tile)
+    d_kmf, d_kfm = torch.empty_like(kernel_mf), torch.empty_like(kernel_fm)
+    d_bmf, d_bfm = (torch.empty((D,), dtype=F32, device=tile.device) for _ in range(2))
+    _lib.check(_lib.lib().ctr_fwbi_bwd(_ptr(tile), _ptr(d_tile), _ptr(d_h), B, F, D, ctypes.addressof(groups), M, _ptr(kernel_mf),
+                                       _ptr(kernel_fm), _ptr(row_grads), _ptr(d_kmf), _ptr(d_kfm), _ptr(d_bmf), _ptr(d_bfm),
+                                       _stream()))
+    return row_grads, d_kmf, d_kfm, d_bmf, d_bfm
+
+
 def fwfm_fwd(tile: torch.Tensor, r: torch.Tensor) -> torch.Tensor:
     """FwFM second-order logit (B,1).  tile (B,F,K); r (F(F-1)/2,) pair strengths in utils.index_from_upper_triangular order."""
     B, F, K = tile.shape

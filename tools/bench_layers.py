@@ -4,7 +4,7 @@
 Each kernel is timed alone with CUDA events; an L2 flush (a 256 MB write) runs between timed iterations because these
 working sets are flushed from the 50 MB L2.  Prints one JSON line per measurement.
 
-    python tools/bench_layers.py [--iters 20] [--only cin,dcn,din,fibinet]     (also: pairwise, bst, adam, pnn, dien, deepcrossing, mmoe, ple, wide, autoint)
+    python tools/bench_layers.py [--iters 20] [--only cin,dcn,din,fibinet]     (also: pairwise, bst, adam, pnn, dien, deepcrossing, mmoe, ple, wide, autoint, flen)
 """
 import argparse
 import json
@@ -541,6 +541,74 @@ def autoint_rows(iters, flush, rn):
         torch.backends.cuda.matmul.allow_tf32 = prev_tf32
 
 
+def flen_rows(iters, flush, rn, gen):
+    """FLEN field-wise bi-interaction (ctr_embed_fwbi_fwd / ctr_fwbi_fwd / ctr_fwbi_bwd) at the config-5 tile shape F = 40,
+    D = 32 with M = 3 and 8 groups, B = 4 096 and 65 536, over a 40 x 250 000-row table (1.28 GB, far above the 50 MB L2).
+    Beside each row, in the same run: ops.embed_bi_fwd / _bwd at the same (B, F, D) (NFM's fused lookup, the same bytes), and
+    plain fp32 torch doing the same layer (gather, group sums by einsum, autograd for the backward).  Algorithmic bytes:
+    forward ids + rows (+ tile when written) + h; tile-input forward tile + h; backward tile (+ d_tile) + d_h + row_grads.
+    The HBM floor is those bytes over the 3.35 TB/s data-sheet figure (H100 SXM, 700 W), not measured."""
+    print(json.dumps({"flen_card": card()}), flush=True)
+    F, D, rows = 40, 32, 250_000
+    table = rn(F * rows, D, std=0.2)
+    off = torch.arange(F + 1, dtype=torch.int64, device="cuda") * rows
+
+    def torch_form(e, oh, iu, kmf, kfm, bmf, bfm):
+        p, q = torch.einsum("bfd,fm->bmd", e, oh), torch.einsum("bfd,fm->bmd", e * e, oh)
+        h = bmf + bfm + torch.einsum("m,bmd->bd", kfm, p * p - q)
+        return h + torch.einsum("k,bkd->bd", kmf, p[:, iu[0]] * p[:, iu[1]])
+
+    for M in (3, 8):
+        group = [f % M for f in range(F)]
+        # the one-hot group matrix and the pair indices are built once, outside the timed calls
+        oh = torch.zeros(F, M, device="cuda")
+        oh[torch.arange(F), torch.tensor(group)] = 1.0
+        iu = torch.triu_indices(M, M, 1, device="cuda")
+        w = [rn(M * (M - 1) // 2, std=0.5), rn(M, std=0.5), rn(D, std=0.1), rn(D, std=0.1)]
+        for B in (4096, 65536):
+            ids = torch.randint(0, rows, (B, F), device="cuda", generator=gen)
+            g, dt = rn(B, D), rn(B, F, D)
+            cfg = {"B": B, "F": F, "D": D, "M": M, "rows_per_field": rows}
+            row, ids_b, h_b = B * F * D * 4, B * F * 8, B * D * 4
+            tile, h = ops.embed_fwbi_fwd(table, off, ids, group, *w)
+            e = table[off[:-1] + ids].requires_grad_(True)
+            wt = [t.clone().requires_grad_(True) for t in w]
+            ref_h = torch_form(e, oh, iu, *wt)
+            ref_g = torch.autograd.grad(ref_h, [e, *wt], g, retain_graph=True)
+            rg = ops.fwbi_bwd(tile, dt, g, group, w[0], w[1])
+            diff = {"fwd": float((ref_h.detach() - h).abs().max() / ref_h.detach().abs().max()),
+                    "bwd": float((ref_g[0] + dt - rg[0]).abs().max() / (ref_g[0] + dt).abs().max())}
+
+            def torch_fwd():
+                return torch_form(table[off[:-1] + ids], oh, iu, *w)
+            runs = [
+                ("fwbi_fwd_fused_tile", lambda: ops.embed_fwbi_fwd(table, off, ids, group, *w), ids_b + 2 * row + h_b,
+                 "embed_bi_fwd_tile", lambda: ops.embed_bi_fwd(table, off, ids), torch_fwd, "fwd"),
+                ("fwbi_fwd_fused_no_tile", lambda: ops.embed_fwbi_fwd(table, off, ids, group, *w, want_tile=False),
+                 ids_b + row + h_b, "embed_bi_fwd_no_tile", lambda: ops.embed_bi_fwd(table, off, ids, want_tile=False), None, "fwd"),
+                ("fwbi_fwd_tile_input", lambda: ops.fwbi_fwd(tile, group, *w), row + h_b, None, None, None, "fwd"),
+                ("fwbi_bwd_d_tile", lambda: ops.fwbi_bwd(tile, dt, g, group, w[0], w[1]), 3 * row + h_b,
+                 "embed_bi_bwd_d_tile", lambda: ops.embed_bi_bwd(tile, dt, g),
+                 lambda: torch.autograd.grad(ref_h, [e, *wt], g, retain_graph=True), "bwd"),
+                ("fwbi_bwd_no_d_tile", lambda: ops.fwbi_bwd(tile, None, g, group, w[0], w[1]), 2 * row + h_b,
+                 "embed_bi_bwd_no_d_tile", lambda: ops.embed_bi_bwd(tile, None, g), None, "bwd"),
+            ]
+            for name, fn, by, bi_name, bi_fn, torch_fn, way in runs:
+                m, bst = timeit(fn, iters, flush)
+                line = {"kernel": name, "config": cfg, "ms_median": m, "ms_best": bst, "algorithmic_GBps": by / (m * 1e-3) / 1e9,
+                        "floor_hbm_us": by / 3.35e12 * 1e6, "floor_over_kernel": by / 3.35e12 / (m * 1e-3),
+                        "max_norm_rel_diff_vs_torch": diff[way], "l2": "flushed between iterations",
+                        "note": "floor from the 3.35 TB/s data sheet (H100 SXM, 700 W), not measured"}
+                if bi_fn is not None:
+                    bm, _ = timeit(bi_fn, iters, flush)
+                    line.update({"embed_bi": bi_name, "embed_bi_ms_median": bm, "over_embed_bi": m / bm})
+                if torch_fn is not None:
+                    tm, _ = timeit(torch_fn, iters, flush)
+                    line.update({"torch_fp32_ms_median": tm, "speedup_vs_torch": tm / m})
+                print(json.dumps(line), flush=True)
+            del tile, h, e, wt, ref_h, ref_g, rg
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=20)
@@ -727,6 +795,8 @@ def main():
         wide_rows(args.iters, flush)
     if "autoint" in only:  # AutoInt interacting layer at the paper's setting (F = 40, H = 2, dk = 32, d = 16 and 64); not in the default list
         autoint_rows(args.iters, flush, rn)
+    if "flen" in only:  # FLEN field-wise bi-interaction at F = 40, D = 32, M = 3 / 8, beside embed_bi and plain torch; not in the default list
+        flen_rows(args.iters, flush, rn, gen)
 
 
 if __name__ == "__main__" and "--configs" not in sys.argv:

@@ -25,7 +25,7 @@
 //                                  Writes dP = dQ | dK | dV | dR (B F, 4 H dk) to the workspace.
 //   autoint_bwd_dx_wgmma_kernel    dx = dP . [Wq; Wk; Wv; Wr]^T: dP rows loaded straight into accumulator-layout A fragments,
 //                                  the weights streamed as a hidden operand (perm8 order, tc_ptx.cuh rows::).
-//   autoint_bwd_dw_wgmma_kernel    dW_p = x^T dP_p over the B F rows: tc_ptx.cuh's batch_reduce.
+//   dW                             dW_p = x^T dP_p over the B F rows: tc_ptx.cuh's weight_grad_wgmma_kernel (DwRows).
 // Rows of x, out and g_out are d or H dk floats (not 16-byte multiples in general), so they move with ordinary loads.
 //
 // Bounds: 1 <= F <= 64, 1 <= d <= 128, 1 <= dk <= 64, 1 <= H <= 8, H dk <= 128, B >= 0; CTR_ERR_UNSUPPORTED otherwise.
@@ -41,9 +41,6 @@ constexpr int TP = FP + 8;                   // pitch of the transpose buffer: c
 
 struct W4 {
   const float* p[4];                         // w_query, w_key, w_value, w_res (d, HD)
-};
-struct DW4 {
-  float* p[4];
 };
 
 // position of column u inside its group of 8 in a B tile fed by rows::acc_to_a fragments (the inverse of perm8)
@@ -516,58 +513,18 @@ autoint_bwd_dx_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_w, const fl
 }
 
 // ================================================================================================= backward: dW
-__host__ __device__ constexpr int dw_smem_bytes(int DP, int SB) { return SB * (2 * DP * 128 + DW_BC * DW_NC * 4 + 16); }
-
-// dW_p[i][col] = sum_rows x[row][i] dP[row][p HD + col]: A = dP^T chunks (TMA), B = x^T generated on chip.
-template <int DP>
-__global__ void __launch_bounds__(NTHREADS, 1)
-autoint_bwd_dw_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_dp, const float* __restrict__ x, DW4 dw,
-                            int rows_total, int d, int HD, int ngroups, int nslices, int SB) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = align_1024(smem_raw);
-  constexpr int qt_bytes = 2 * DP * 128;
-  constexpr int p_floats = DW_BC * DW_NC;
-  uint8_t* qts = smem;
-  float* ps = reinterpret_cast<float*>(smem + SB * qt_bytes);
-  Ring ring(smem_u32(ps + SB * p_floats), SB);
-
-  const int warp = warp_uniform(threadIdx.x >> 5), lane = threadIdx.x & 31;
-  const int group = blockIdx.x % ngroups;
-  int c_beg, c_end;
-  batch_slice(blockIdx.x / ngroups, nslices, (rows_total + DW_BC - 1) / DW_BC, c_beg, c_end);
-  const int n0 = group * DW_NC;
-
-  ring.init();
-  if (producer_role(warp, lane, [&] {
-        for (int c = c_beg; c < c_end; ++c) {
-          const Ring::Slot slot = ring.acquire(p_floats * 4);
-          tma_load_2d(smem_u32(ps + (size_t)slot.stage * p_floats), &tmap_dp, n0, c * DW_BC, slot.full);
-        }
-      }))
-    return;
-
-  const int wg = warp >> 2, w = warp & 3, g = lane >> 2, t = lane & 3;
-  const int nl0 = wg * WG_M + w * 16 + g;
-  float acc[DP / 2];
-  batch_reduce<DP>(
-      acc, ring, qts, c_beg, c_end, rows_total, lane, nl0, [](int) {},
-      [&](int k, int b0, int b) { return k < d ? __ldg(x + (size_t)(b0 + b) * d + k) : 0.f; },
-      [&](int s, int b, int nl) { return ps[(size_t)s * p_floats + b * DW_NC + nl]; });
-  if (c_end <= c_beg) return;
-#pragma unroll
-  for (int cc = 0; cc < DP / 8; ++cc)
-#pragma unroll
-    for (int e = 0; e < 2; ++e) {
-      const int i = 8 * cc + 2 * t + e;
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        const int u = n0 + nl0 + 8 * r;
-        const int p = u / HD;
-        float* dst = p == 0 ? dw.p[0] : p == 1 ? dw.p[1] : p == 2 ? dw.p[2] : dw.p[3];
-        if (i < d && u < 4 * HD) atomicAdd(dst + (size_t)i * HD + u % HD, acc[4 * cc + 2 * r + e]);
-      }
-    }
-}
+// Result rows of tc::weight_grad_wgmma_kernel over P = dP (B F, 4 HD), Q = x: row u is dW_p[:, u % HD] with p = u / HD.
+struct DwRows {
+  static constexpr bool row_sums = false, mask_q = false, slice_d = false;
+  float* dw[4];                              // d_w_query, d_w_key, d_w_value, d_w_res (d, HD)
+  int HD;
+  __device__ __forceinline__ GradRow row(int u) const {
+    if (u >= 4 * HD) return GradRow{};
+    const int p = u / HD;
+    float* dst = p == 0 ? dw[0] : p == 1 ? dw[1] : p == 2 ? dw[2] : dw[3];
+    return GradRow{dst + u % HD, HD};
+  }
+};
 
 }  // namespace autoint
 }  // namespace ctr
@@ -691,14 +648,11 @@ extern "C" int ctr_autoint_bwd(const float* x, const float* w_query, const float
       (rc = prep("ctr_autoint_bwd(prep)", w, wn, d, H, dk, s, 1, st)))
     return rc;
   const int64_t rows = B * F;
-  CUtensorMap mwt, mw, mdp;
-  if ((rc = encode_rows_operand(fn, &mwt, ws, s.DP, s.RU)) || (rc = encode_hidden_operand(fn, &mw, wn, s.DP, s.UP)) ||
-      (rc = encode_2d(fn, &mdp, dp, s.U, rows, DW_NC, DW_BC, CU_TENSOR_MAP_SWIZZLE_NONE)))
+  CUtensorMap mwt, mw;
+  if ((rc = encode_rows_operand(fn, &mwt, ws, s.DP, s.RU)) || (rc = encode_hidden_operand(fn, &mw, wn, s.DP, s.UP)))
     return rc;
   const int sms = sm_count();
-  const int ngroups = (int)((s.U + DW_NC - 1) / DW_NC);
-  const int nslices = batch_slices(sms, ngroups, (rows + DW_BC - 1) / DW_BC);
-  const DW4 dw = {{d_w_query, d_w_key, d_w_value, d_w_res}};
+  const DwRows dw = {{d_w_query, d_w_key, d_w_value, d_w_res}, (int)(H * dk)};
   rc = with_const<32, 64, 96, 128>(s.DP, [&](auto DP) {
     constexpr int SB = ring_depth(bwd_fixed_bytes(DP), DP);
     static_assert(SB >= 2, "attention backward shared memory");
@@ -716,8 +670,6 @@ extern "C" int ctr_autoint_bwd(const float* x, const float* w_query, const float
                        capped_grid((rows + DX_TILE - 1) / DX_TILE, sms), NTHREADS, SBX * (stage_bytes(DP) + 16) + 1024, st,
                        mw, dp, d_x, (int)rows, (int)d, (int)s.U, (int)s.UP))
       return r;
-    const int sb = stages_that_fit(1024, dw_smem_bytes(DP, 1));
-    return launch("ctr_autoint_bwd(dw, wgmma)", autoint_bwd_dw_wgmma_kernel<DP>, ngroups * nslices, NTHREADS,
-                  dw_smem_bytes(DP, sb) + 1024, st, mdp, x, dw, (int)rows, (int)d, (int)(H * dk), ngroups, nslices, sb);
+    return launch_weight_grad<DP>(fn, "ctr_autoint_bwd(dw, wgmma)", dw, dp, s.U, rows, x, nullptr, (int)d, 1, st);
   });
 }

@@ -25,9 +25,10 @@
 //                             the workspace and fed from the accumulator registers to dx += dz_e . W_e[chunk]^T (hidden
 //                             units in perm8 order).  After the last chunk: the softmax backward, dx += dlogit . G^T (one
 //                             more hidden chunk: the gate columns), dlogit written to the workspace.
-//   mmoe_bwd_dw_wgmma_kernel  one batch-sliced reduction over the workspace rows [dz_0 | .. | dz_{E-1} | dlogit] (pitch R)
-//                             with B = x^T generated on chip (tc_ptx.cuh's batch_reduce, the residual unit's dW0 / db0
-//                             mode): every dW_e with db_e as row sums, and every dG_t, one atomic per element per CTA.
+//   dW, db, dG                tc_ptx.cuh's weight_grad_wgmma_kernel (DwRows): one batch-sliced reduction over the workspace
+//                             rows [dz_0 | .. | dz_{E-1} | dlogit] (pitch R) with B = x^T generated on chip, as for the
+//                             residual unit's dW0 / db0: every dW_e with db_e as row sums, and every dG_t, one atomic per
+//                             element per CTA.
 // The rows of x, towers, gates and g are not 16-byte aligned in general (d = 82, H or E odd), so they are read and written
 // with ordinary loads and stores; only the prepped weights and the workspace's dz | dlogit rows are TMA tensors.
 //
@@ -380,80 +381,23 @@ mmoe_bwd_dx_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_rows, const __
 }
 
 // ================================================================================================= backward dW
-__host__ __device__ constexpr int dw_smem_bytes(int DP, int SB) { return SB * (2 * DP * 128 + DW_BC * DW_NC * 4 + 16); }
-
-// P = the workspace rows [dz_0 | .. | dz_{E-1} | dlogit] (B, R), Q = x: row n < E HP of the result is dW_e[:, h]
-// (n = e HP + h) with db_e[h] its sum over the batch, row E HP + t E + e is dG_t[:, e].
-template <int DP>
-__global__ void __launch_bounds__(NTHREADS, 1)
-mmoe_bwd_dw_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_p, const float* __restrict__ x, float* __restrict__ d_we,
-                         float* __restrict__ d_be, float* __restrict__ d_wg, int B, int d, int E, int H, int T, int HP,
-                         int ngroups, int nslices, int SB) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = align_1024(smem_raw);
-  constexpr int qt_bytes = 2 * DP * 128;                    // Q^T tiles [DP x 32 samples] (hi | lo), 128B-swizzled
-  constexpr int p_floats = DW_BC * DW_NC;                   // one P chunk [32 samples x 128 units]
-  uint8_t* qts = smem;
-  float* ps = reinterpret_cast<float*>(smem + SB * qt_bytes);
-  Ring ring(smem_u32(ps + SB * p_floats), SB);
-
-  const int warp = warp_uniform(threadIdx.x >> 5), lane = threadIdx.x & 31;
-  const int group = blockIdx.x % ngroups;
-  int c_beg, c_end;
-  batch_slice(blockIdx.x / ngroups, nslices, (B + DW_BC - 1) / DW_BC, c_beg, c_end);
-  const int n0 = group * DW_NC;
-
-  ring.init();
-  // ============================ TMA producer: P chunks [32 samples x 128 units] ============================
-  if (producer_role(warp, lane, [&] {
-        for (int c = c_beg; c < c_end; ++c) {
-          const Ring::Slot slot = ring.acquire(p_floats * 4);
-          tma_load_2d(smem_u32(ps + (size_t)slot.stage * p_floats), &tmap_p, n0, c * DW_BC, slot.full);
-        }
-      }))
-    return;
-
-  // ============================ consumers: B = x^T generated on chip, A = P^T ============================
-  const int wg = warp >> 2, w = warp & 3, g = lane >> 2, t = lane & 3;
-  float rsum[2] = {0.f, 0.f};                               // sum_b of this thread's two rows (db_e for expert units)
-  const int nl0 = wg * WG_M + w * 16 + g;                   // this thread's A rows: units n0 + nl0 (+8)
-  float acc[DP / 2];
-  batch_reduce<DP>(
-      acc, ring, qts, c_beg, c_end, B, lane, nl0, [](int) {},
-      [&](int k, int b0, int b) { return k < d ? __ldg(x + (size_t)(b0 + b) * d + k) : 0.f; },
-      [&](int s, int b, int nl) {
-        const float v = ps[(size_t)s * p_floats + b * DW_NC + nl];
-        rsum[nl == nl0 ? 0 : 1] += v;
-        return v;
-      });
-  if (c_end <= c_beg) return;
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const int n = n0 + nl0 + 8 * r;
-    float* dst = nullptr;                                   // element k of this row: dst[k * stride]
-    size_t stride = 0;
+// Result rows of tc::weight_grad_wgmma_kernel over P = the workspace rows [dz_0 | .. | dz_{E-1} | dlogit] (B, R), Q = x:
+// row n < E HP is dW_e[:, h] (n = e HP + h) with db_e[h] its batch sum, row E HP + t E + e is dG_t[:, e].
+struct DwRows {
+  static constexpr bool row_sums = true, mask_q = false, slice_d = false;
+  float* d_we;
+  float* d_be;
+  float* d_wg;
+  int d, E, H, T, HP;
+  __device__ __forceinline__ GradRow row(int n) const {
     if (n < E * HP) {
       const int e = n / HP, h = n % HP;
-      if (h < H) { dst = d_we + (size_t)e * d * H + h; stride = H; }
-    } else if (n - E * HP < T * E) {
-      const int c = n - E * HP;
-      dst = d_wg + (size_t)(c / E) * d * E + c % E;
-      stride = E;
+      return h < H ? GradRow{d_we + (size_t)e * d * H + h, H, d_be + (size_t)e * H + h} : GradRow{};
     }
-#pragma unroll
-    for (int cc = 0; cc < DP / 8; ++cc) {
-#pragma unroll
-      for (int xx = 0; xx < 2; ++xx) {
-        const int k = 8 * cc + 2 * t + xx;
-        if (dst != nullptr && k < d) atomicAdd(dst + (size_t)k * stride, acc[4 * cc + 2 * r + xx]);
-      }
-    }
-    float v = rsum[r];
-    v += __shfl_xor_sync(0xffffffffu, v, 1);
-    v += __shfl_xor_sync(0xffffffffu, v, 2);
-    if (t == 0 && n < E * HP && n % HP < H) atomicAdd(d_be + (size_t)(n / HP) * H + n % HP, v);
+    const int c = n - E * HP;
+    return c < T * E ? GradRow{d_wg + (size_t)(c / E) * d * E + c % E, E} : GradRow{};
   }
-}
+};
 
 }  // namespace mmoe
 }  // namespace ctr
@@ -563,15 +507,11 @@ extern "C" int ctr_mmoe_bwd(const float* x, const float* w_experts, const float*
   float* ws = static_cast<float*>(workspace);
   float* dzbuf = reinterpret_cast<float*>(static_cast<uint8_t*>(workspace) + s.dz_offset);
   if ((rc = prep("ctr_mmoe_bwd(prep)", w_experts, w_gates, ws, d, E, H, T, s, 2, st))) return rc;
-  CUtensorMap mr, mh, mdz;
+  CUtensorMap mr, mh;
   if ((rc = encode_rows_operand(fn, &mr, ws, s.DP, s.R)) ||
-      (rc = encode_hidden_operand(fn, &mh, ws + s.slot_floats, s.DP, s.R)) ||
-      (rc = encode_2d(fn, &mdz, dzbuf, s.R, B, DW_NC, DW_BC, CU_TENSOR_MAP_SWIZZLE_NONE)))
+      (rc = encode_hidden_operand(fn, &mh, ws + s.slot_floats, s.DP, s.R)))
     return rc;
-  const int sms = sm_count();
-  const int grid = capped_grid((B + TILE - 1) / TILE, sms);
-  const int ngroups = (int)((s.R + DW_NC - 1) / DW_NC);
-  const int nslices = batch_slices(sms, ngroups, (B + DW_BC - 1) / DW_BC);
+  const int grid = capped_grid((B + TILE - 1) / TILE, sm_count());
   return with_const<32, 64, 96, 128>(s.DP, [&](auto DP) {
     constexpr int SB = DP == 128 ? 3 : 4;
     static_assert(dx_smem_bytes(DP, SB) + 1024 <= SMEM_CAP, "dx shared memory");
@@ -579,9 +519,7 @@ extern "C" int ctr_mmoe_bwd(const float* x, const float* w_experts, const float*
                        dx_smem_bytes(DP, SB) + 1024, st, mr, mh, x, b_experts, gates, g_towers, d_x, dzbuf, (int)B, (int)d,
                        (int)E, (int)H, (int)T, (int)s.HP))
       return r;
-    const int sb = stages_that_fit(1024, dw_smem_bytes(DP, 1));
-    return launch("ctr_mmoe_bwd(dw, wgmma)", mmoe_bwd_dw_wgmma_kernel<DP>, ngroups * nslices, NTHREADS,
-                  dw_smem_bytes(DP, sb) + 1024, st, mdz, x, d_w_experts, d_b_experts, d_w_gates, (int)B, (int)d, (int)E,
-                  (int)H, (int)T, (int)s.HP, ngroups, nslices, sb);
+    const DwRows rows = {d_w_experts, d_b_experts, d_w_gates, (int)d, (int)E, (int)H, (int)T, (int)s.HP};
+    return launch_weight_grad<DP>(fn, "ctr_mmoe_bwd(dw, wgmma)", rows, dzbuf, s.R, B, x, nullptr, (int)d, 1, st);
   });
 }

@@ -27,8 +27,9 @@
 //                            backward, dlogit written to the workspace next to dz: rows [dz_0 | .. | dz_{E-1} | dlogit].
 //   ple_bwd_dx_wgmma_kernel  dx = [dz | dlogit] . [W | Gcat]^T: per 128-sample tile and N-wide slice of d, a K-sliced GEMM
 //                            over the R units, both operands TMA-staged (the workspace rows and the hidden-layout prep).
-//   ple_bwd_dw_wgmma_kernel  one batch-sliced reduction over the workspace rows with x^T generated on chip (tc_ptx.cuh's
-//                            batch_reduce), one grid dimension per N-wide slice of d: every dW_e with db_e, and dGcat.
+//   dW, db, dGcat            tc_ptx.cuh's weight_grad_wgmma_kernel (DwRows): one batch-sliced reduction over the workspace
+//                            rows with x^T generated on chip, one grid row per N-wide slice of d: every dW_e with db_e,
+//                            and dGcat.
 // x, out, gates and g are read and written with ordinary loads and stores (d, H and GC are arbitrary); the prepped weights
 // and the workspace rows are TMA tensors.
 //
@@ -479,80 +480,24 @@ ple_bwd_dx_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_dz, const __gri
 }
 
 // ================================================================================================= backward dW
-__host__ __device__ constexpr int dw_smem_bytes(int N, int SB) { return SB * (2 * N * 128 + DW_BC * DW_NC * 4 + 16); }
-
-// P = the workspace rows [dz_0 | .. | dz_{E-1} | dlogit] (B, R), Q = x[:, ds N ..]: row n < E HP of the result is
-// dW_e[ds N .., h] (n = e HP + h) with db_e[h] its sum over the batch (added by the ds = 0 slice), row E HP + c is
-// dGcat[ds N .., c].
-template <int N>
-__global__ void __launch_bounds__(NTHREADS, 1)
-ple_bwd_dw_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_p, const float* __restrict__ x, float* __restrict__ d_we,
-                        float* __restrict__ d_be, float* __restrict__ d_wg, int B, int d, int E, int H, int GC, int HP,
-                        int ngroups, int nslices, int SB) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = align_1024(smem_raw);
-  constexpr int qt_bytes = 2 * N * 128;                     // Q^T tiles [N x 32 samples] (hi | lo), 128B-swizzled
-  constexpr int p_floats = DW_BC * DW_NC;                   // one P chunk [32 samples x 128 units]
-  uint8_t* qts = smem;
-  float* ps = reinterpret_cast<float*>(smem + SB * qt_bytes);
-  Ring ring(smem_u32(ps + SB * p_floats), SB);
-
-  const int warp = warp_uniform(threadIdx.x >> 5), lane = threadIdx.x & 31;
-  const int group = blockIdx.x % ngroups, ds = blockIdx.y, k0 = ds * N;
-  int c_beg, c_end;
-  batch_slice(blockIdx.x / ngroups, nslices, (B + DW_BC - 1) / DW_BC, c_beg, c_end);
-  const int n0 = group * DW_NC;
-
-  ring.init();
-  // ============================ TMA producer: P chunks [32 samples x 128 units] ============================
-  if (producer_role(warp, lane, [&] {
-        for (int c = c_beg; c < c_end; ++c) {
-          const Ring::Slot slot = ring.acquire(p_floats * 4);
-          tma_load_2d(smem_u32(ps + (size_t)slot.stage * p_floats), &tmap_p, n0, c * DW_BC, slot.full);
-        }
-      }))
-    return;
-
-  // ============================ consumers: B = x^T generated on chip, A = P^T ============================
-  const int wg = warp >> 2, w = warp & 3, g = lane >> 2, t = lane & 3;
-  float rsum[2] = {0.f, 0.f};                               // sum_b of this thread's two rows (db_e for expert units)
-  const int nl0 = wg * WG_M + w * 16 + g;                   // this thread's A rows: units n0 + nl0 (+8)
-  float acc[N / 2];
-  batch_reduce<N>(
-      acc, ring, qts, c_beg, c_end, B, lane, nl0, [](int) {},
-      [&](int k, int b0, int b) { return k0 + k < d ? __ldg(x + (size_t)(b0 + b) * d + k0 + k) : 0.f; },
-      [&](int s, int b, int nl) {
-        const float v = ps[(size_t)s * p_floats + b * DW_NC + nl];
-        rsum[nl == nl0 ? 0 : 1] += v;
-        return v;
-      });
-  if (c_end <= c_beg) return;
-#pragma unroll
-  for (int r = 0; r < 2; ++r) {
-    const int n = n0 + nl0 + 8 * r;
-    float* dst = nullptr;                                   // element k of this row: dst[k * stride]
-    size_t stride = 0;
+// Result rows of tc::weight_grad_wgmma_kernel over P = the workspace rows [dz_0 | .. | dz_{E-1} | dlogit] (B, R), Q = x,
+// one grid row per N-wide slice of d: row n < E HP is dW_e[:, h] (n = e HP + h) with db_e[h] its batch sum, row E HP + c
+// is dGcat[:, c].
+struct DwRows {
+  static constexpr bool row_sums = true, mask_q = false, slice_d = true;
+  float* d_we;
+  float* d_be;
+  float* d_wg;
+  int d, E, H, GC, HP;
+  __device__ __forceinline__ GradRow row(int n) const {
     if (n < E * HP) {
       const int e = n / HP, h = n % HP;
-      if (h < H) { dst = d_we + (size_t)e * d * H + h; stride = H; }
-    } else if (n - E * HP < GC) {
-      dst = d_wg + (n - E * HP);
-      stride = GC;
+      return h < H ? GradRow{d_we + (size_t)e * d * H + h, H, d_be + (size_t)e * H + h} : GradRow{};
     }
-#pragma unroll
-    for (int cc = 0; cc < N / 8; ++cc) {
-#pragma unroll
-      for (int xx = 0; xx < 2; ++xx) {
-        const int k = k0 + 8 * cc + 2 * t + xx;
-        if (dst != nullptr && k < d) atomicAdd(dst + (size_t)k * stride, acc[4 * cc + 2 * r + xx]);
-      }
-    }
-    float v = rsum[r];
-    v += __shfl_xor_sync(0xffffffffu, v, 1);
-    v += __shfl_xor_sync(0xffffffffu, v, 2);
-    if (ds == 0 && t == 0 && n < E * HP && n % HP < H) atomicAdd(d_be + (size_t)(n / HP) * H + n % HP, v);
+    const int c = n - E * HP;
+    return c < GC ? GradRow{d_wg + c, GC} : GradRow{};
   }
-}
+};
 
 }  // namespace ple
 }  // namespace ctr
@@ -702,12 +647,11 @@ extern "C" int ctr_ple_bwd(const float* x, const float* w_experts, const float* 
   if (B == 0) return CTR_OK;
   float* dzbuf = reinterpret_cast<float*>(static_cast<uint8_t*>(workspace) + s.dz_offset);
   if ((rc = prep("ctr_ple_bwd(prep)", w_experts, w_gates, workspace, d, H, s, 2, st))) return rc;
-  CUtensorMap mr, mh, mdx, mdw;
+  CUtensorMap mr, mh, mdx;
   if ((rc = encode_2d(fn, &mr, workspace, s.DP, 2 * s.R, KB, PC, CU_TENSOR_MAP_SWIZZLE_128B)) ||
       (rc = encode_2d(fn, &mh, static_cast<uint8_t*>(workspace) + s.hidden_offset, s.R, 2 * s.DH, KB, s.N,
                       CU_TENSOR_MAP_SWIZZLE_128B)) ||
-      (rc = encode_2d(fn, &mdx, dzbuf, s.R, B, KB, DX_TILE, CU_TENSOR_MAP_SWIZZLE_128B)) ||
-      (rc = encode_2d(fn, &mdw, dzbuf, s.R, B, DW_NC, DW_BC, CU_TENSOR_MAP_SWIZZLE_NONE)))
+      (rc = encode_2d(fn, &mdx, dzbuf, s.R, B, KB, DX_TILE, CU_TENSOR_MAP_SWIZZLE_128B)))
     return rc;
   const int sms = sm_count();
   const int sb = tile_stages(s);
@@ -717,8 +661,6 @@ extern "C" int ctr_ple_bwd(const float* x, const float* w_experts, const float* 
     return rc;
   const int n_ds = s.DH / s.N;
   const int64_t n_dx = (B + DX_TILE - 1) / DX_TILE * n_ds;
-  const int ngroups = (int)((s.R + DW_NC - 1) / DW_NC);
-  const int nslices = batch_slices(sms / n_ds > 0 ? sms / n_ds : 1, ngroups, (B + DW_BC - 1) / DW_BC);
   return with_const<32, 64, 128>(s.N, [&](auto N) {
     constexpr int dx_sb = (int)((SMEM_CAP - 1024) / dx_stage_bytes(N)) < 4 ? (int)((SMEM_CAP - 1024) / dx_stage_bytes(N)) : 4;
     static_assert(dx_sb * (dx_stage_bytes(N) + 16) + 1024 <= (int)SMEM_CAP, "dx shared memory");
@@ -726,9 +668,7 @@ extern "C" int ctr_ple_bwd(const float* x, const float* w_experts, const float* 
                        dx_sb * (dx_stage_bytes(N) + 16) + 1024, st, mdx, mh, d_x, (int)B, (int)d, s.DH, (int)s.R, n_ds,
                        dx_sb))
       return r;
-    const int dw_sb = stages_that_fit(1024, dw_smem_bytes(N, 1));
-    return launch("ctr_ple_bwd(dw, wgmma)", ple_bwd_dw_wgmma_kernel<N>, dim3(ngroups * nslices, n_ds), NTHREADS,
-                  dw_smem_bytes(N, dw_sb) + 1024, st, mdw, x, d_w_experts, d_b_experts, d_w_gates, (int)B, (int)d, s.q.E,
-                  (int)H, s.q.GC, (int)s.HP, ngroups, nslices, dw_sb);
+    const DwRows rows = {d_w_experts, d_b_experts, d_w_gates, (int)d, s.q.E, (int)H, s.q.GC, (int)s.HP};
+    return launch_weight_grad<N>(fn, "ctr_ple_bwd(dw, wgmma)", rows, dzbuf, s.R, B, x, nullptr, (int)d, n_ds, st);
   });
 }

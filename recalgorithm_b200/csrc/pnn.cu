@@ -24,7 +24,7 @@
 //   pnn_bwd_dw_tc_kernel  A = G^T (rows = n, K = samples) from TMA-staged g_out / out chunks of 32 samples;
 //                         B = xt^T [WP x 32 samples], generated on chip into 128B-swizzled shared memory.
 //                         A CTA owns 128 n and a batch slice; one atomic add per element at the end.  The consumer
-//                         loop is tc_ptx.cuh's batch_reduce, shared with the residual unit's weight gradients.
+//                         loop is tc_ptx.cuh's batch_reduce, shared with the dense layers' weight_grad_wgmma_kernel.
 // Tensor path: WX = FK + Q + 1 <= 128 (WP = WX padded to 32 / 64 / 128) and N % 4 == 0 (the TMA row pitch of g_out / out).
 // That holds the reference defaults (F = K = 8: WX = 101, N = 1024) for both methods.  Other shapes run the CUDA-core
 // kernels below (chosen by shape only).

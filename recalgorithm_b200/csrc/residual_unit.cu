@@ -17,11 +17,11 @@
 //   resunit_bwd_dx_wgmma_kernel  per chunk: a recomputed as in the forward, t = gy . W1^T[:, chunk] (B = W1 chunk),
 //                                gh = t [a > 0], dx += gh . W0[chunk]^T (B = W0 chunk).  Writes h and gh (B, HP) to the
 //                                workspace for the weight gradients; sums gy over its rows for db1.
-//   resunit_bwd_dw_wgmma_kernel  dW1 = h^T . gy and dW0^T = gh^T . x, with sum_b gh = db0 alongside: A = h^T or gh^T (rows =
-//                                hidden units, K = samples) from TMA-staged [32 samples x 128 units] chunks, B = gy^T or x^T
-//                                [DP x 32 samples] generated on chip into 128B-swizzled shared memory.  A CTA owns 128 hidden
-//                                units and a batch slice, and issues one atomic add per element at the end.  The
-//                                consumer loop is tc_ptx.cuh's batch_reduce, shared with the PNN weight gradients.
+//   dW1, dW0                     tc_ptx.cuh's weight_grad_wgmma_kernel, once per gradient: dW1 = h^T . gy (Dw1Rows, Q masked
+//                                to gy = g [out > 0] on chip) and dW0^T = gh^T . x with sum_b gh = db0 alongside (Dw0Rows).
+//                                A = h^T or gh^T (rows = hidden units, K = samples) from TMA-staged [32 samples x 128 units]
+//                                chunks, B = gy^T or x^T [DP x 32 samples] generated on chip.  A CTA owns 128 hidden units and
+//                                a batch slice, and issues one atomic add per element at the end.
 // The rows of x, out and g are d floats (328 B at the reference d = 82), not a multiple of 16 bytes, so they are staged with
 // ordinary loads; only the prepped weights and the workspace's h / gh (pitch HP) are TMA tensors.
 //
@@ -245,79 +245,22 @@ resunit_bwd_dx_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_w0t, const 
 }
 
 // ================================================================================================= backward dW
-__host__ __device__ constexpr int dw_smem_bytes(int DP, int SB) { return SB * (2 * DP * 128 + DW_BC * DW_NC * 4 + 16); }
-
-// MODE 0: P = h, Q = gy = g [out > 0]: dw = dW1 (H,d).   MODE 1: P = gh, Q = x: dw = dW0 (d,H), db = db0 (H).
-template <int DP, int MODE>
-__global__ void __launch_bounds__(NTHREADS, 1)
-resunit_bwd_dw_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_p, const float* __restrict__ q,
-                            const float* __restrict__ qmask, float* __restrict__ dw, float* __restrict__ db, int B, int d,
-                            int H, int ngroups, int nslices, int SB) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  uint8_t* smem = align_1024(smem_raw);
-  constexpr int qt_bytes = 2 * DP * 128;                    // Q^T tiles [DP x 32 samples] (hi | lo), 128B-swizzled
-  constexpr int p_floats = DW_BC * DW_NC;                   // one P chunk [32 samples x 128 units]
-  uint8_t* qts = smem;
-  float* ps = reinterpret_cast<float*>(smem + SB * qt_bytes);
-  Ring ring(smem_u32(ps + SB * p_floats), SB);
-
-  const int warp = warp_uniform(threadIdx.x >> 5), lane = threadIdx.x & 31;
-  const int group = blockIdx.x % ngroups;
-  int c_beg, c_end;
-  batch_slice(blockIdx.x / ngroups, nslices, (B + DW_BC - 1) / DW_BC, c_beg, c_end);
-  const int n0 = group * DW_NC;
-
-  ring.init();
-  // ============================ TMA producer: P chunks [32 samples x 128 units] ============================
-  if (producer_role(warp, lane, [&] {
-        for (int c = c_beg; c < c_end; ++c) {
-          const Ring::Slot slot = ring.acquire(p_floats * 4);
-          tma_load_2d(smem_u32(ps + (size_t)slot.stage * p_floats), &tmap_p, n0, c * DW_BC, slot.full);
-        }
-      }))
-    return;
-
-  // ============================ consumers: B = Q^T generated from q, A = P^T ============================
-  const int wg = warp >> 2, w = warp & 3, g = lane >> 2, t = lane & 3;
-  float rsum[2] = {0.f, 0.f};                               // MODE 1: sum_b gh of this thread's two units
-  const int nl0 = wg * WG_M + w * 16 + g;                   // this thread's A rows: units n0 + nl0 (+8)
-  float acc[DP / 2];
-  batch_reduce<DP>(
-      acc, ring, qts, c_beg, c_end, B, lane, nl0, [](int) {},
-      [&](int k, int b0, int b) {
-        if (k >= d) return 0.f;
-        const size_t o = (size_t)(b0 + b) * d + k;
-        return (MODE == 1 || __ldg(qmask + o) > 0.f) ? __ldg(q + o) : 0.f;
-      },
-      [&](int s, int b, int nl) {
-        const float v = ps[(size_t)s * p_floats + b * DW_NC + nl];
-        if (MODE == 1) rsum[nl == nl0 ? 0 : 1] += v;
-        return v;
-      });
-  if (c_end <= c_beg) return;
-#pragma unroll
-  for (int cc = 0; cc < DP / 8; ++cc) {
-#pragma unroll
-    for (int x = 0; x < 2; ++x) {
-      const int i = 8 * cc + 2 * t + x;
-#pragma unroll
-      for (int r = 0; r < 2; ++r) {
-        const int j = n0 + nl0 + 8 * r;
-        if (i < d && j < H) atomicAdd(MODE == 0 ? dw + (size_t)j * d + i : dw + (size_t)i * H + j, acc[4 * cc + 2 * r + x]);
-      }
-    }
-  }
-  if (MODE == 1) {
-#pragma unroll
-    for (int r = 0; r < 2; ++r) {
-      float v = rsum[r];
-      v += __shfl_xor_sync(0xffffffffu, v, 1);
-      v += __shfl_xor_sync(0xffffffffu, v, 2);
-      const int j = n0 + nl0 + 8 * r;
-      if (t == 0 && j < H) atomicAdd(db + j, v);
-    }
-  }
-}
+// Result rows of tc::weight_grad_wgmma_kernel, one per hidden unit j.
+// dW1 = h^T . gy: P = h, Q = gy = g [out > 0]; row j is dW1[j, :].
+struct Dw1Rows {
+  static constexpr bool row_sums = false, mask_q = true, slice_d = false;
+  float* dw;
+  int d, H;
+  __device__ __forceinline__ GradRow row(int j) const { return j < H ? GradRow{dw + (size_t)j * d, 1} : GradRow{}; }
+};
+// dW0 = x^T . gh: P = gh, Q = x; row j is dW0[:, j], its batch sum db0[j].
+struct Dw0Rows {
+  static constexpr bool row_sums = true, mask_q = false, slice_d = false;
+  float* dw;
+  float* db;
+  int H;
+  __device__ __forceinline__ GradRow row(int j) const { return j < H ? GradRow{dw + j, H, db + j} : GradRow{}; }
+};
 
 }  // namespace resunit
 }  // namespace ctr
@@ -428,16 +371,11 @@ extern "C" int ctr_residual_unit_bwd(const float* x, const float* w0, const floa
   float* ghbuf = reinterpret_cast<float*>(static_cast<uint8_t*>(workspace) + s.gh_offset);
   rc = prep("ctr_residual_unit_bwd(prep)", w0, w1, ws, d, H, s, 3, make_int4(0, 2, 3, 0), st);
   if (rc) return rc;
-  CUtensorMap m0, m2, m3, mh, mgh;
+  CUtensorMap m0, m2, m3;
   if ((rc = encode_weights(fn, &m0, ws, s, 0, true)) || (rc = encode_weights(fn, &m2, ws, s, 1, true)) ||
-      (rc = encode_weights(fn, &m3, ws, s, 2, false)) ||
-      (rc = encode_2d(fn, &mh, hbuf, s.HP, B, DW_NC, DW_BC, CU_TENSOR_MAP_SWIZZLE_NONE)) ||
-      (rc = encode_2d(fn, &mgh, ghbuf, s.HP, B, DW_NC, DW_BC, CU_TENSOR_MAP_SWIZZLE_NONE)))
+      (rc = encode_weights(fn, &m3, ws, s, 2, false)))
     return rc;
-  const int sms = sm_count();
-  const int grid = capped_grid((B + TILE - 1) / TILE, sms);
-  const int ngroups = (int)((s.HP + DW_NC - 1) / DW_NC);
-  const int nslices = batch_slices(sms, ngroups, (B + DW_BC - 1) / DW_BC);
+  const int grid = capped_grid((B + TILE - 1) / TILE, sm_count());
   return with_const<32, 64, 96, 128>(s.DP, [&](auto DP) {
     constexpr int SB = DP == 128 ? 2 : 4;
     static_assert(dx_smem_bytes(DP, SB) + 1024 <= SMEM_CAP, "dx shared memory");
@@ -445,12 +383,10 @@ extern "C" int ctr_residual_unit_bwd(const float* x, const float* w0, const floa
                        dx_smem_bytes(DP, SB) + 1024, st, m0, m2, m3, x, b0, out, g_out, d_x, hbuf, ghbuf, d_b1, (int)B,
                        (int)d, (int)H, (int)s.HP))
       return r;
-    const int sb = stages_that_fit(1024, dw_smem_bytes(DP, 1));
-    const size_t smem = dw_smem_bytes(DP, sb) + 1024;
-    if (int r = launch("ctr_residual_unit_bwd(dw1, wgmma)", resunit_bwd_dw_wgmma_kernel<DP, 0>, ngroups * nslices, NTHREADS,
-                       smem, st, mh, g_out, out, d_w1, nullptr, (int)B, (int)d, (int)H, ngroups, nslices, sb))
+    if (int r = launch_weight_grad<DP>(fn, "ctr_residual_unit_bwd(dw1, wgmma)", Dw1Rows{d_w1, (int)d, (int)H}, hbuf, s.HP,
+                                       B, g_out, out, (int)d, 1, st))
       return r;
-    return launch("ctr_residual_unit_bwd(dw0, wgmma)", resunit_bwd_dw_wgmma_kernel<DP, 1>, ngroups * nslices, NTHREADS, smem,
-                  st, mgh, x, nullptr, d_w0, d_b0, (int)B, (int)d, (int)H, ngroups, nslices, sb);
+    return launch_weight_grad<DP>(fn, "ctr_residual_unit_bwd(dw0, wgmma)", Dw0Rows{d_w0, d_b0, (int)H}, ghbuf, s.HP, B, x,
+                                  nullptr, (int)d, 1, st);
   });
 }

@@ -1,8 +1,8 @@
 // wgmma / TMA / mbarrier PTX wrappers shared by the tensor-core kernels (sm_90a), the pipeline mechanics built on them
 // (shared-memory alignment, the mbarrier ring, the producer / consumer role split, the 3xTF32 k-step, accumulation chains,
-// the consumer loop of the batch-reduction weight-gradient GEMMs, the row-chunk GEMMs of the dense-layer kernels) and the
-// host side of a tensor-core launch (workspace check, tensor-map encoding, batch slices and ring depth of the weight-gradient
-// kernels).
+// the consumer loop of the batch-reduction weight-gradient GEMMs, the one weight-gradient kernel of the dense layers built
+// on it, the row-chunk GEMMs of the dense-layer kernels) and the host side of a tensor-core launch (workspace check,
+// tensor-map encoding, batch slices, ring depth and launch of the weight-gradient kernels).
 #pragma once
 #include <cuda.h>
 
@@ -322,6 +322,97 @@ __device__ __forceinline__ void batch_reduce(float (&acc)[N / 2], Ring& ring, ui
   }
 }
 
+// The weight-gradient kernel of the dense layers (residual unit, MMoE, PLE, AutoInt) around batch_reduce: result row n,
+// input k0 + k = sum over b < rows_total of P[b, n] Q[b, k0 + k].  P is a [rows_total x units] workspace tensor streamed by
+// TMA in [DW_BC samples x DW_NC units] chunks (no swizzle); Q is q (rows_total, d), or q [qmask > 0] with Rows::mask_q.
+// CTA (x, y) owns the DW_NC units x % ngroups, the batch slice x / ngroups of nslices and the N inputs from k0 = y N, and
+// adds its partial result with one atomic per element into rows.row(n).  Each layer's Rows type, small and trivially
+// copyable, gives `GradRow row(int n) const` and three compile-time flags: row_sums (also sum each row over the samples
+// into its bias; the y = 0 CTAs only), mask_q, and slice_d (the grid's y dimension slices the inputs; without it k0 = 0).
+// Being compile-time, they cost the layers that do not use them nothing in the per-element loops: a run-time k0, for one,
+// is rematerialised from blockIdx.y for every element at this register budget.
+struct GradRow {
+  float* dst = nullptr;                      // element k of the row at dst[k * stride]; null for padding rows
+  int stride = 0;
+  float* bias = nullptr;                     // the row's batch sum (Rows::row_sums), or null
+};
+
+// atomicAdd(p, v) with the result unused, p in global memory: the compiler cannot always tell that a pointer taken from a
+// Rows value is global, and a generic atomic tests every address for the shared window first.
+__device__ __forceinline__ void red_add_global(float* p, float v) {
+  asm volatile("red.global.add.f32 [%0], %1;" ::"l"(__cvta_generic_to_global(p)), "f"(v) : "memory");
+}
+
+// shared memory of weight_grad_wgmma_kernel: per stage the Q^T tiles, one P chunk and the two ring barriers
+__host__ __device__ constexpr int dw_smem_bytes(int N, int SB) { return SB * (2 * N * 128 + DW_BC * DW_NC * 4 + 16); }
+
+template <int N, class Rows>
+__global__ void __launch_bounds__(NTHREADS, 1)
+weight_grad_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_p, const float* __restrict__ q,
+                         const float* __restrict__ qmask, const Rows rows, int rows_total, int d, int ngroups, int nslices,
+                         int SB) {
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = align_1024(smem_raw);
+  constexpr int qt_bytes = 2 * N * 128;                     // Q^T tiles [N x 32 samples] (hi | lo), 128B-swizzled
+  constexpr int p_floats = DW_BC * DW_NC;                   // one P chunk [32 samples x 128 units]
+  uint8_t* qts = smem;
+  float* ps = reinterpret_cast<float*>(smem + SB * qt_bytes);
+  Ring ring(smem_u32(ps + SB * p_floats), SB);
+
+  const int warp = warp_uniform(threadIdx.x >> 5), lane = threadIdx.x & 31;
+  const int group = blockIdx.x % ngroups, k0 = Rows::slice_d ? blockIdx.y * N : 0;
+  int c_beg, c_end;
+  batch_slice(blockIdx.x / ngroups, nslices, (rows_total + DW_BC - 1) / DW_BC, c_beg, c_end);
+  const int n0 = group * DW_NC;
+
+  ring.init();
+  // ============================ TMA producer: P chunks [32 samples x 128 units] ============================
+  if (producer_role(warp, lane, [&] {
+        for (int c = c_beg; c < c_end; ++c) {
+          const Ring::Slot slot = ring.acquire(p_floats * 4);
+          tma_load_2d(smem_u32(ps + (size_t)slot.stage * p_floats), &tmap_p, n0, c * DW_BC, slot.full);
+        }
+      }))
+    return;
+
+  // ============================ consumers: B = Q^T generated on chip, A = P^T ============================
+  const int wg = warp >> 2, w = warp & 3, g = lane >> 2, t = lane & 3;
+  float rsum[2] = {0.f, 0.f};                               // Rows::row_sums: sum_b of this thread's two rows
+  const int nl0 = wg * WG_M + w * 16 + g;                   // this thread's A rows: units n0 + nl0 (+8)
+  float acc[N / 2];
+  batch_reduce<N>(
+      acc, ring, qts, c_beg, c_end, rows_total, lane, nl0, [](int) {},
+      [&](int k, int b0, int b) {
+        if (k0 + k >= d) return 0.f;
+        const size_t o = (size_t)(b0 + b) * d + k0 + k;
+        return (!Rows::mask_q || __ldg(qmask + o) > 0.f) ? __ldg(q + o) : 0.f;
+      },
+      [&](int s, int b, int nl) {
+        const float v = ps[(size_t)s * p_floats + b * DW_NC + nl];
+        if (Rows::row_sums) rsum[nl == nl0 ? 0 : 1] += v;
+        return v;
+      });
+  if (c_end <= c_beg) return;
+#pragma unroll
+  for (int r = 0; r < 2; ++r) {
+    const GradRow row = rows.row(n0 + nl0 + 8 * r);
+#pragma unroll
+    for (int cc = 0; cc < N / 8; ++cc) {
+#pragma unroll
+      for (int x = 0; x < 2; ++x) {
+        const int k = k0 + 8 * cc + 2 * t + x;
+        if (row.dst != nullptr && k < d) red_add_global(row.dst + (size_t)k * row.stride, acc[4 * cc + 2 * r + x]);
+      }
+    }
+    if (Rows::row_sums) {
+      float v = rsum[r];
+      v += __shfl_xor_sync(0xffffffffu, v, 1);
+      v += __shfl_xor_sync(0xffffffffu, v, 2);
+      if (blockIdx.y == 0 && t == 0 && row.bias != nullptr) red_add_global(row.bias, v);
+    }
+  }
+}
+
 // Row-chunk GEMMs of the dense-layer kernels (residual unit, MMoE): 64 staged rows of an input of width DP (32 / 64 / 96 /
 // 128) times a chunk of HC hidden units, whose result stays in registers and feeds the next GEMM as A fragments.
 //   rows operand    [HC units x DP] K-major, streamed from a [2 R][DP] map (hi copy, then the lo copy R rows on);
@@ -489,6 +580,21 @@ static inline int batch_slices(int sms, int64_t ngroups, int64_t n_units) {
 static inline int stages_that_fit(size_t fixed, size_t stage) {
   const size_t sb = (SMEM_CAP - fixed) / stage;
   return (int)(sb < 4 ? sb : 4);
+}
+// Launches weight_grad_wgmma_kernel<N, Rows> over P = p (rows_total rows of `units` floats) and Q = q (rows_total rows of
+// d floats, masked by qmask with Rows::mask_q) for n_ds slices of N inputs: the batch slices of each input slice share
+// one wave over the SMs (n_ds > 1 needs Rows::slice_d); `what` names the launch in error messages, `fn` the entry.
+template <int N, class Rows>
+static inline int launch_weight_grad(const char* fn, const char* what, const Rows& rows, const float* p, int64_t units,
+                                     int64_t rows_total, const float* q, const float* qmask, int d, int n_ds,
+                                     cudaStream_t st) {
+  CUtensorMap map;
+  if (int rc = encode_2d(fn, &map, p, units, rows_total, DW_NC, DW_BC, CU_TENSOR_MAP_SWIZZLE_NONE)) return rc;
+  const int ngroups = (int)((units + DW_NC - 1) / DW_NC);
+  const int nslices = batch_slices(sm_count() / n_ds, ngroups, (rows_total + DW_BC - 1) / DW_BC);
+  const int sb = stages_that_fit(1024, dw_smem_bytes(N, 1));
+  return launch(what, weight_grad_wgmma_kernel<N, Rows>, dim3(ngroups * nslices, n_ds), NTHREADS, dw_smem_bytes(N, sb) + 1024,
+                st, map, q, qmask, rows, (int)rows_total, d, ngroups, nslices, sb);
 }
 
 namespace rows {

@@ -907,7 +907,7 @@ def chunked_reference(B, fn):
 
 def check_reduced(got, ref_mag, what):
     """Batch-reduced gradient against float64: |got - R| <= TOL max(|R| + rms(R), M) element-wise (see chunked_reference);
-    a gradient whose every chunk is exactly zero must be exactly zero."""
+    a gradient whose every chunk is exactly zero must be exactly zero.  Returns the worst |got - R| / bound."""
     ref, mag = ref_mag
     got = got.detach().cpu().double().numpy() if isinstance(got, torch.Tensor) else np.asarray(got, np.float64)
     got = got.reshape(ref.shape)
@@ -916,10 +916,12 @@ def check_reduced(got, ref_mag, what):
     err = np.abs(got - ref)
     zero = bound == 0
     assert np.all(got[zero] == 0), f"{what}: {int(np.count_nonzero(got[zero]))} elements must be exactly zero"
+    worst = 0.0
     if (~zero).any():
         worst = float((err[~zero] / bound[~zero]).max())
         assert worst <= 1.0, (f"{what}: element-wise error is {worst:.2f}x the bound TOL max(|ref| + rms(ref), "
                               f"sum over 64-sample chunks |chunk ref|) (max error {float(err.max()):.3e})")
+    return worst
 
 
 def _f64(*arrays):

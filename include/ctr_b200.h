@@ -404,6 +404,47 @@ int ctr_ple_bwd(const float* x, const float* w_experts, const float* b_experts, 
                 int64_t extraction, float* d_x, float* d_w_experts, float* d_b_experts, float* d_w_gates, void* workspace,
                 int64_t workspace_bytes, void* stream);
 
+/* ---- Row MTL: multi-task loss balancing (uncertainty weighting, GradNorm, PCGrad) -------------------------
+ * The reference sums its per-task losses (MMOE/mmoe.py:261-263, PLE/ple.py:251-254: tf.add_n); its README lists
+ * "Uncertainty, GradNorm, PCGrad" as a to-do, so no reference code exists and these definitions are the contract.
+ * T tasks, 1 <= T <= 8; B (samples) and P (shared-parameter floats) in 0..2^31-1; CTR_ERR_UNSUPPORTED naming the bound
+ * otherwise.  L_t = mean_b sigmoid_ce(logit[t,b], label[t,b]) in TF's stable form (as ctr_sigmoid_ce).
+ *   method 0, sum:         total = sum_t L_t                                   (the reference's add_n)
+ *   method 1, weights:     total = sum_t w_t L_t                               (GradNorm's network loss; task_param = w)
+ *   method 2, uncertainty: total = sum_t exp(-s_t) L_t + s_t / 2               (Kendall et al. 2018, eq. 10; task_param = s
+ *                          = log sigma_t^2);  d total / d s_t = -exp(-s_t) L_t + 1/2
+ * ctr_multitask_sigmoid_ce: logits, labels (T,B); task_param (T) (unused, may be NULL, for method 0).  Writes task_loss (T),
+ * unweighted, and total_loss (1).  d_logits (T,B) (nullable) receives the UNWEIGHTED (sigmoid(x) - z) / B, so that it serves
+ * the total (times 1, w_t or exp(-s_t)) and each L_t alone; d_task_param (T) (nullable) receives d total / d task_param
+ * (L_t for method 1, zeros for method 0).  Deterministic: one cluster of 8 CTAs with a fixed partition and summation order
+ * in float64, so the same inputs give the same bits.  B = 0 gives zero task losses.
+ * Per-task gradients: grads holds T rows of P floats, row t = d L_t / d W over the shared parameters W (flattened), row
+ * pitch ld >= P floats, any alignment.
+ * ctr_multitask_gram: gram (T,T) float64 = grads . grads^T, one streaming pass over the T*P floats and a second one-CTA
+ * pass over the per-CTA partials; deterministic.  workspace: at least ctr_multitask_gram_workspace_bytes(T, P) bytes,
+ * 8-byte aligned.
+ * ctr_pcgrad_combine (Yu et al. 2020, Algorithm 1): g_i' = g_i; for j in order (a permutation of 0..T-1, int32, device;
+ * other entries are skipped), j != i: if g_i'.g_j < 0 then g_i' -= (g_i'.g_j / |g_j|^2) g_j; out (P) = sum_i g_i'.  Solved
+ * in coefficient space from gram (C = I; dot = sum_k C_ik gram_kj; C_ij -= dot / gram_jj when dot < 0 and gram_jj > 0),
+ * then out = sum_k (sum_i C_ik) g_k accumulated in float64.  coef (T, float64, nullable) receives sum_i C_ik.  A zero row
+ * never triggers a projection; at T = 1 out equals the row bit for bit.
+ * ctr_gradnorm_update (Chen et al. 2018, Algorithm 1), one small CTA in float64: n_t = sqrt(gram_tt) (gram of the
+ * unweighted d L_t / d W), G_t = w_t n_t, Gbar = mean_t G_t, r_t = (L_t / L0_t) / mean_k (L_k / L0_k),
+ * grad_loss (1) = sum_t |G_t - Gbar r_t^alpha| (the target is a constant), d_weights (T, nullable) = sign(G_t - Gbar
+ * r_t^alpha) n_t with sign(0) = 0; then weights (T, in place) <- w - lr d_weights, renormalised to sum T.  No clamp: a large
+ * lr can drive a weight negative.  initial_loss (L0) must be positive.  When every current loss is 0 (B = 0, or a batch
+ * fitted exactly) r_t is undefined: weights are left unchanged, d_weights and grad_loss are 0. */
+int ctr_multitask_sigmoid_ce(const float* logits, const float* labels, int64_t T, int64_t B, int method,
+                             const float* task_param, float* task_loss, float* total_loss, float* d_logits,
+                             float* d_task_param, void* stream);
+int ctr_multitask_gram_workspace_bytes(int64_t T, int64_t P, int64_t* bytes);
+int ctr_multitask_gram(const float* grads, int64_t T, int64_t P, int64_t ld, double* gram, void* workspace,
+                       int64_t workspace_bytes, void* stream);
+int ctr_pcgrad_combine(const float* grads, int64_t T, int64_t P, int64_t ld, const double* gram, const int32_t* order,
+                       float* out, double* coef, void* stream);
+int ctr_gradnorm_update(const double* gram, const float* task_loss, const float* initial_loss, int64_t T, float alpha,
+                        float lr, float* weights, float* grad_loss, float* d_weights, void* stream);
+
 /* ---- Row DIN-ATT: DIN attention unit -----------------------------------------------------------------
  * Replaces din_attention(query, keys, keys_length, is_softmax) (DIN/din_attention.py:17-43).
  * query (B,H); keys (B,T,H); keys_length int64 (B); dense layers f1_att (4H->64, relu), f2_att (64->32,

@@ -111,6 +111,11 @@ SIGNATURES = {
     "ctr_autoint_workspace_bytes": (c_int, [_I, _I, _I, _I, _I, POINTER(c_int64)]),
     "ctr_autoint_fwd": (c_int, [_P] * 5 + [_I] * 5 + [_P, _P, _I, _P]),
     "ctr_autoint_bwd": (c_int, [_P] * 7 + [_I] * 5 + [_P] * 6 + [_I, _P]),
+    "ctr_multitask_sigmoid_ce": (c_int, [_P, _P, _I, _I, c_int] + [_P] * 6),
+    "ctr_multitask_gram_workspace_bytes": (c_int, [_I, _I, POINTER(c_int64)]),
+    "ctr_multitask_gram": (c_int, [_P, _I, _I, _I, _P, _P, _I, _P]),
+    "ctr_pcgrad_combine": (c_int, [_P, _I, _I, _I, _P, _P, _P, _P, _P]),
+    "ctr_gradnorm_update": (c_int, [_P, _P, _P, _I, ctypes.c_float, ctypes.c_float, _P, _P, _P, _P]),
 }
 
 

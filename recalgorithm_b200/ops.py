@@ -1010,3 +1010,82 @@ def ple_bwd(x, w_experts, b_experts, w_gates, gates, g_out, experts_per_task, nu
                                       H, len(n), arr, S, ext, _ptr(d_x), _ptr(d_we), _ptr(d_be), _ptr(d_wg), _ptr(ws),
                                       ws.numel(), _stream()))
     return d_x, d_we, d_be, d_wg
+
+
+# ------------------------------------------------------------------------------------ Row MTL: multi-task loss balancing
+MTL_METHODS = {"sum": 0, "gradnorm": 1, "uncertainty": 2}   # 1: task_param holds GradNorm's weights w; 2: s = log sigma^2
+MTL_MAX_TASKS = 8
+F64 = torch.float64
+
+
+def multitask_sigmoid_ce(logits: torch.Tensor, labels: torch.Tensor, method: int, task_param: Optional[torch.Tensor] = None,
+                         want_grad: bool = True):
+    """Per-task mean sigmoid cross-entropies of logits / labels (T,B) and the method's total (include/ctr_b200.h, Row MTL):
+    (task_loss (T,), total (1,), d_logits (T,B) | None, d_task_param (T,) | None).  d_logits is the unweighted
+    (sigmoid(x) - z) / B; d_task_param is d total / d task_param (None for method 0)."""
+    T, B = logits.shape
+    _chk(logits, F32, "logits"); _chk(labels, F32, "labels", (T, B))
+    if method != 0:
+        _chk(task_param, F32, "task_param", (T,))
+    task_loss = torch.empty((T,), dtype=F32, device=logits.device)
+    total = torch.empty((1,), dtype=F32, device=logits.device)
+    d_logits = torch.empty((T, B), dtype=F32, device=logits.device) if want_grad else None
+    d_param = torch.empty((T,), dtype=F32, device=logits.device) if want_grad and method != 0 else None
+    _lib.check(_lib.lib().ctr_multitask_sigmoid_ce(_ptr(logits), _ptr(labels), T, B, int(method),
+                                                   _ptr(task_param) if method != 0 else None, _ptr(task_loss), _ptr(total),
+                                                   _ptr(d_logits), _ptr(d_param), _stream()))
+    return task_loss, total, d_logits, d_param
+
+
+def _task_rows(grads: torch.Tensor):
+    """(T, P, ld) of a (T,P) float32 view whose rows are contiguous (row pitch ld >= P, e.g. a column slice)."""
+    if grads.dim() != 2:
+        raise ValueError(f"grads: expected (T,P), got shape {tuple(grads.shape)}")
+    T, P = grads.shape
+    if not (grads.is_cuda and grads.device.index == torch.cuda.current_device() and grads.dtype == F32):
+        _chk(grads.contiguous(), F32, "grads")                         # raises the device / dtype error
+    ld = grads.stride(0) if T > 1 else P
+    if (P > 1 and grads.stride(1) != 1) or ld < P:
+        raise ValueError(f"grads: rows must be contiguous with a row pitch >= P, got strides {grads.stride()}")
+    return T, P, ld
+
+
+def multitask_gram(grads: torch.Tensor, gram: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """gram (T,T) float64 = grads . grads^T of the per-task gradient rows grads (T,P), deterministic."""
+    T, P, ld = _task_rows(grads)
+    nbytes = ctypes.c_int64(0)
+    _lib.check(_lib.lib().ctr_multitask_gram_workspace_bytes(T, P, ctypes.byref(nbytes)))
+    ws = torch.empty((max(int(nbytes.value) // 8, 1),), dtype=F64, device=grads.device)
+    if gram is None:
+        gram = torch.empty((T, T), dtype=F64, device=grads.device)
+    _chk(gram, F64, "gram", (T, T))
+    _lib.check(_lib.lib().ctr_multitask_gram(_ptr(grads), T, P, ld, _ptr(gram), _ptr(ws), ws.numel() * 8, _stream()))
+    return gram
+
+
+def pcgrad_combine(grads: torch.Tensor, gram: torch.Tensor, order: torch.Tensor, out: Optional[torch.Tensor] = None,
+                   want_coef: bool = False):
+    """PCGrad of the per-task gradient rows grads (T,P) given their gram (T,T) float64 and the projection order (T,) int32:
+    (out (P,), coef (T,) float64 | None), out = sum_k coef_k grads[k]."""
+    T, P, ld = _task_rows(grads)
+    _chk(gram, F64, "gram", (T, T)); _chk(order, I32, "order", (T,))
+    if out is None:
+        out = torch.empty((P,), dtype=F32, device=grads.device)
+    _chk(out, F32, "out", (P,))
+    coef = torch.empty((T,), dtype=F64, device=grads.device) if want_coef else None
+    _lib.check(_lib.lib().ctr_pcgrad_combine(_ptr(grads), T, P, ld, _ptr(gram), _ptr(order), _ptr(out), _ptr(coef), _stream()))
+    return out, coef
+
+
+def gradnorm_update(gram: torch.Tensor, task_loss: torch.Tensor, initial_loss: torch.Tensor, weights: torch.Tensor,
+                    alpha: float, lr: float, want_d_weights: bool = False):
+    """One GradNorm step on weights (T,) in place from the gram (T,T) float64 of the unweighted per-task gradients, the task
+    losses and the initial ones: (grad_loss (1,), d_weights (T,) | None)."""
+    T = weights.numel()
+    _chk(weights, F32, "weights", (T,)); _chk(gram, F64, "gram", (T, T))
+    _chk(task_loss, F32, "task_loss", (T,)); _chk(initial_loss, F32, "initial_loss", (T,))
+    grad_loss = torch.empty((1,), dtype=F32, device=weights.device)
+    d_w = torch.empty((T,), dtype=F32, device=weights.device) if want_d_weights else None
+    _lib.check(_lib.lib().ctr_gradnorm_update(_ptr(gram), _ptr(task_loss), _ptr(initial_loss), T, float(alpha), float(lr),
+                                              _ptr(weights), _ptr(grad_loss), _ptr(d_w), _stream()))
+    return grad_loss, d_w

@@ -127,19 +127,33 @@ def pnn_logit(fields_embeddings, num_fields: int, embedding_dim: int, output_dim
 
 
 def dien_logit(dense_input, category_input, target_input, sequnence_input, sequnence_length, gru_output_units=8,
-               custom_gru_type: str = "AGRU", hidden_units=(64, 32)):
-    """DIEN/dien.py:179-254 (the auxiliary loss :261-300, Dice / PReLU / batch-norm of the fcn tail left out, as for DIN).
-    Returns (logit, attention_scores (B, T, 1))."""
+               custom_gru_type: str = "AGRU", hidden_units=(64, 32), use_auxiliary_loss: bool = False,
+               neg_sequnence_input=None, negative_sample_number=3):
+    """DIEN/dien.py:179-254 (Dice / PReLU / batch-norm of the fcn tail left out, as for DIN).  Returns (logit,
+    attention_scores (B, T, 1)); with ``use_auxiliary_loss`` (:256-300), (logit, attention_scores, aux_loss), where
+    aux_loss is the paper's sign (the negative of the reference's) and the training loss is ce + aux_loss (:316-317).
+    neg_sequnence_input (B, (T-1)*negative_sample_number, na) are the caller's negatives, looked up like the history."""
+    if use_auxiliary_loss:
+        na, nh = int(sequnence_input.shape[-1]), int(gru_output_units)
+        with L.variable_scope("aux_loss"):                                                # :264, 268
+            w_aux = L.get_variable("aux_project_matrix", (na, nh))
     with L.variable_scope("seq_encoder"):                                                 # :199-229, one kernel each way
-        final_state, attention_scores = L.dien_interest_evolution(sequnence_input, sequnence_length, target_input,
-                                                                  gru_output_units, custom_gru_type=custom_gru_type,
-                                                                  return_attention_scores=True)
+        if use_auxiliary_loss:
+            final_state, attention_scores, aux_loss = L.dien_interest_evolution_aux(
+                sequnence_input, sequnence_length, target_input, neg_sequnence_input, w_aux, gru_output_units,
+                custom_gru_type=custom_gru_type, negative_sample_number=negative_sample_number, return_attention_scores=True)
+        else:
+            final_state, attention_scores = L.dien_interest_evolution(sequnence_input, sequnence_length, target_input,
+                                                                      gru_output_units, custom_gru_type=custom_gru_type,
+                                                                      return_attention_scores=True)
         concat_all = torch.cat([dense_input, category_input, target_input, final_state], dim=-1)   # :237
         with L.variable_scope("fcn"):                                                     # :240-254 (TF names dense, dense_1, ...)
             net = concat_all
             for i, unit in enumerate(hidden_units):
                 net = dense(net, unit, name=f"dense_{i}" if i else "dense")
             logit = dense(net, 1, name=f"dense_{len(hidden_units)}" if hidden_units else "dense")
+    if use_auxiliary_loss:
+        return logit, attention_scores, aux_loss
     return logit, attention_scores
 
 

@@ -489,6 +489,33 @@ int ctr_dien_bwd(const float* seq_input, const int64_t* seq_length, const float*
                  const float* g_final_state, int64_t B, int64_t T, int64_t na, int64_t nh, int cell_type, float* d_seq_input,
                  float* d_target_input, float* d_params, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* DIEN auxiliary loss (DIEN/dien.py:256-300, added to the loss at :316-317): next-behaviour supervision of the extractor
+ * states h_t of ctr_dien_fwd.  With L = clamp(seq_length, 0, T), w_aux = aux_loss/aux_project_matrix W (na, nh),
+ * neg_seq_input (B, (T-1)*T_neg, na) whose row t*T_neg + n is negative n of position t (the reshape at :279), and
+ * q_t = W h_t (na):
+ *   aux_loss = -(1/B) sum_b sum_{t < L-1} [ log sig(q_t . x_{t+1}) + sum_n log(1 - sig(q_t . neg_{t,n})) ]
+ * -- the NEGATIVE of the reference's aux_loss (which, added to the loss as written, would be minimised toward -inf), in the
+ * stable forms log sig(z) = -softplus(-z), log(1 - sig(z)) = -softplus(z).  Positions t >= L-1 are never computed.  The sum
+ * is fixed-order (float64): the same inputs give the same bits.  B = 0 gives 0.
+ * ctr_dien_aux_workspace_bytes(): the DIEN workspace plus B*(T-1) per-position terms; one such workspace serves ctr_dien_fwd,
+ * ctr_dien_aux_fwd and ctr_dien_bwd_aux.  ctr_dien_aux_fwd reads the states ctr_dien_fwd left there, so it runs after it.
+ * ctr_dien_bwd_aux: ctr_dien_bwd with the auxiliary loss's gradient added, given g_aux_loss, a DEVICE scalar (no host
+ * synchronisation: the call is graph-capturable).  With s = g_aux/B, g+_t = s (sig(z+_t) - 1), g-_{t,n} = s sig(z-_{t,n}):
+ * d_neg_seq_input (B, (T-1)*T_neg, na) is overwritten (row (t,n) = g-_{t,n} q_t, exactly 0 at t >= L-1); d_seq_input gets
+ * g+_t q_t at row t+1 on top of ctr_dien_bwd's gradient; dL/dh_t gets W^T (g+_t x_{t+1} + sum_n g-_{t,n} neg_{t,n}) on top of the
+ * attention and evolution terms; d_w_aux (na, nh) is overwritten with sum (that vector) (x) h_t.  With g_aux = 0 the outputs
+ * of ctr_dien_bwd are reproduced bit for bit.  DIEN's bounds, and T_neg >= 1 with B*(T-1)*T_neg*na < 2^31
+ * (CTR_ERR_UNSUPPORTED otherwise).  B = 0 zeroes aux_loss / d_params and d_w_aux and launches nothing else. */
+int ctr_dien_aux_workspace_bytes(int64_t B, int64_t T, int64_t na, int64_t nh, int64_t T_neg, int64_t* bytes);
+int ctr_dien_aux_fwd(const float* seq_input, const float* neg_seq_input, const int64_t* seq_length, const float* w_aux,
+                     int64_t B, int64_t T, int64_t na, int64_t nh, int64_t T_neg, float* aux_loss, void* workspace,
+                     int64_t workspace_bytes, void* stream);
+int ctr_dien_bwd_aux(const float* seq_input, const float* neg_seq_input, const int64_t* seq_length, const float* target_input,
+                     const float* params, const float* w_aux, const float* g_final_state, const float* g_aux_loss, int64_t B,
+                     int64_t T, int64_t na, int64_t nh, int64_t T_neg, int cell_type, float* d_seq_input,
+                     float* d_neg_seq_input, float* d_target_input, float* d_params, float* d_w_aux, void* workspace,
+                     int64_t workspace_bytes, void* stream);
+
 /* ---- Rows SENET / BILINEAR: FiBiNET ---------------------------------------------------------------------
  * senet(input, embedding_dim, reduction_ratio) (FiBiNET/senet.py:26-34): x (B,F,K); w1 (F,r); w2 (r,F). */
 int ctr_senet_fwd(const float* x, const float* w1, const float* w2, int64_t B, int64_t F, int64_t K, int64_t r,

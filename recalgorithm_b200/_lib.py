@@ -99,6 +99,9 @@ SIGNATURES = {
     "ctr_dien_workspace_bytes": (c_int, [_I, _I, _I, _I, POINTER(c_int64)]),
     "ctr_dien_fwd": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, c_int, _P, _P, _P, _I, _P]),
     "ctr_dien_bwd": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, c_int, _P, _P, _P, _P, _I, _P]),
+    "ctr_dien_aux_workspace_bytes": (c_int, [_I, _I, _I, _I, _I, POINTER(c_int64)]),
+    "ctr_dien_aux_fwd": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _I, _P]),
+    "ctr_dien_bwd_aux": (c_int, [_P] * 8 + [_I] * 5 + [c_int] + [_P] * 6 + [_I, _P]),
     "ctr_residual_unit_workspace_bytes": (c_int, [_I, _I, _I, POINTER(c_int64)]),
     "ctr_residual_unit_fwd": (c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _I, _P]),
     "ctr_residual_unit_bwd": (c_int, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P, _I, _P]),

@@ -489,6 +489,36 @@ def dien(seq, seq_len, target, params, nh: int, cell: int):
     return _DIEN.apply(seq, seq_len, target, nh, cell, *params)
 
 
+class _DIENAux(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, seq, seq_len, target, neg_seq, w_aux, nh, cell, T_neg, *params):
+        na = seq.shape[-1]
+        packed = ops.dien_pack_params(params, na, nh)
+        seq, target, neg_seq, w_aux = seq.contiguous(), target.contiguous(), neg_seq.contiguous(), w_aux.contiguous()
+        final, scores, aux, ws = ops.dien_fwd_aux(seq, seq_len, target, neg_seq, packed, w_aux, nh, cell, T_neg)
+        ctx.save_for_backward(seq, seq_len, target, neg_seq, packed, w_aux, ws)
+        ctx.cfg = (nh, cell, T_neg)
+        ctx.mark_non_differentiable(scores)
+        ctx.set_materialize_grads(False)            # an unused output's gradient arrives as None and goes down as zeros
+        return final, scores, aux
+
+    @staticmethod
+    def backward(ctx, g_final, _g_scores, g_aux):
+        seq, seq_len, target, neg_seq, packed, w_aux, ws = ctx.saved_tensors
+        nh, cell, T_neg = ctx.cfg
+        g_final = torch.zeros((seq.shape[0], nh), dtype=seq.dtype, device=seq.device) if g_final is None else g_final.contiguous()
+        g_aux = torch.zeros((), dtype=seq.dtype, device=seq.device) if g_aux is None else g_aux.reshape(()).contiguous()
+        d_seq, d_neg, d_tgt, d_p, d_w = ops.dien_bwd_aux(seq, seq_len, target, neg_seq, packed, w_aux, g_final, g_aux, nh, cell,
+                                                         T_neg, ws)
+        return (d_seq, None, d_tgt, d_neg, d_w, None, None, None) + tuple(ops.dien_unpack_params(d_p, seq.shape[-1], nh))
+
+
+def dien_aux(seq, seq_len, target, neg_seq, w_aux, params, nh: int, cell: int, T_neg: int):
+    """DIEN seq_encoder plus the auxiliary loss (DIEN/dien.py:198-229, 256-300, the paper's sign): (final_state (B,nh),
+    attention scores (B,T), forward only, aux_loss ()); one backward serves both differentiable outputs."""
+    return _DIENAux.apply(seq, seq_len, target, neg_seq, w_aux, nh, cell, T_neg, *params)
+
+
 class _ResidualUnit(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x, w0, b0, w1, b1):

@@ -11,6 +11,10 @@
 // the backward reads them, runs BPTT through the evolution cell, the softmax and the extractor, and accumulates the nine
 // weight gradients in shared memory (one global atomic per element per CTA at the end).
 //
+// The auxiliary loss (DIEN/dien.py:256-300, the paper's sign) reads H from the same workspace: dien_aux_fwd_kernel and
+// dien_aux_sum_kernel give the loss, dien_aux_bwd_kernel its row gradients and dL/dh_t, which dien_bwd_aux_kernel -- the
+// backward above with the extra terms added instead of overwritten -- carries through BPTT.
+//
 // Forward weights: the nine recurrent blocks (the extractor's state rows, the evolution cell's input and state rows) are
 // held per lane in registers at nh_pad = 8 and staged by the CTA, zero padded, in shared memory above it; the extractor's
 // input rows W_x are read through the read-only cache in the projection, which runs outside the recurrent part.  Input rows
@@ -485,12 +489,18 @@ __global__ void __launch_bounds__(DIEN_WARPS * 32, 1) dien_fwd_kernel(
 }
 
 // ------------------------------------------------------------------------------------------------------------ backward
-template <int NHP, int AUGRU>
-__global__ void __launch_bounds__(DIEN_WARPS * 32, 1) dien_bwd_kernel(
-    const float* __restrict__ x, const long long* __restrict__ len, const float* __restrict__ tgt,
-    const float* __restrict__ P, const float* __restrict__ g_final, int B, int T, int na, int nh,
-    const float* __restrict__ wsH, const float* __restrict__ wsS, const float* __restrict__ wsA, float* __restrict__ wsDH,
-    float* __restrict__ wsDA, float* __restrict__ d_x, float* __restrict__ d_tgt, float* __restrict__ d_P) {
+// AUX: the auxiliary loss's backward (dien_aux_bwd_kernel) has already seeded dL/dh_t into wsDH and its positive-row term
+// into d_x; the evolution pass and the extractor pass then add to them instead of overwriting.
+#define DIEN_BWD_PARAMS                                                                                                  \
+  const float* __restrict__ x, const long long* __restrict__ len, const float* __restrict__ tgt,                        \
+      const float* __restrict__ P, const float* __restrict__ g_final, int B, int T, int na, int nh,                     \
+      const float* __restrict__ wsH, const float* __restrict__ wsS, const float* __restrict__ wsA,                      \
+      float* __restrict__ wsDH, float* __restrict__ wsDA, float* __restrict__ d_x, float* __restrict__ d_tgt,           \
+      float* __restrict__ d_P
+#define DIEN_BWD_ARGS x, len, tgt, P, g_final, B, T, na, nh, wsH, wsS, wsA, wsDH, wsDA, d_x, d_tgt, d_P
+
+template <int NHP, int AUGRU, bool AUX>
+__device__ __forceinline__ void dien_bwd_body(DIEN_BWD_PARAMS) {
   using LN = Lane<NHP>;
   constexpr int G = LN::G, U = LN::U, RMAX = (64 + G - 1) / G;
   extern __shared__ float acc[];                              // d_P, packed like P, summed over this CTA's samples
@@ -614,7 +624,8 @@ __global__ void __launch_bounds__(DIEN_WARPS * 32, 1) dien_bwd_kernel(
           atomicAdd(acc + o.egb + j, dzr[u]);
           if (AUGRU) atomicAdd(acc + o.egb + nh + j, dzu[u]);
           atomicAdd(acc + o.ecb + j, dzc[u]);
-          wsDH[(row + t) * nh + j] = dxe[u];
+          if constexpr (AUX) wsDH[(row + t) * nh + j] += dxe[u];
+          else wsDH[(row + t) * nh + j] = dxe[u];
         }
         if (act) ds[u] = ln.live[u] ? dsp[u] : 0.f;
       }
@@ -698,7 +709,10 @@ __global__ void __launch_bounds__(DIEN_WARPS * 32, 1) dien_bwd_kernel(
 #pragma unroll
         for (int q = 0; q < RMAX; ++q) {
           const int i = ln.gl + q * G;
-          if (i < na) d_x[(row + t) * na + i] = dxr[q];
+          if (i < na) {
+            if constexpr (AUX) d_x[(row + t) * na + i] += dxr[q];
+            else d_x[(row + t) * na + i] = dxr[q];
+          }
         }
       }
       // weight gradients of the extractor
@@ -776,6 +790,181 @@ __global__ void __launch_bounds__(DIEN_WARPS * 32, 1) dien_bwd_kernel(
   for (int i = threadIdx.x; i < o.total; i += blockDim.x) atomicAdd(d_P + i, acc[i]);
 }
 
+template <int NHP, int AUGRU>
+__global__ void __launch_bounds__(DIEN_WARPS * 32, 1) dien_bwd_kernel(DIEN_BWD_PARAMS) {
+  dien_bwd_body<NHP, AUGRU, false>(DIEN_BWD_ARGS);
+}
+template <int NHP, int AUGRU>
+__global__ void __launch_bounds__(DIEN_WARPS * 32, 1) dien_bwd_aux_kernel(DIEN_BWD_PARAMS) {
+  dien_bwd_body<NHP, AUGRU, true>(DIEN_BWD_ARGS);
+}
+
+// ------------------------------------------------------------------------------------------------------------ auxiliary loss
+// DIEN/dien.py:256-300 with the paper's sign: for every position t < L - 1 of a sample, q_t = W h_t (na), z+ = q_t . x_{t+1},
+// z-_n = q_t . neg_{t,n}, and the sample's term softplus(-z+) + sum_n softplus(z-_n) = -[log sig(z+) + sum_n log(1 - sig(z-_n))].
+// One warp per position (b, t) (persistent CTAs): the positions are independent, and a warp per sample would walk its
+// positions one after another, bound by the latency of the dependent loads and warp sums.  Lane l owns the input elements
+// i = l and l + 32 (na <= 64), so every row read is coalesced and every dot product is one warp sum.  W (na, nh) is staged
+// in shared memory twice: transposed for q = W h (lane i reads its row across j) and as is for the backward's W^T dq (lane j
+// reads its column across i).
+constexpr int AUX_WARPS = 8;
+
+__device__ __forceinline__ float softplus(float z) { return fmaxf(z, 0.f) + log1pf(expf(-fabsf(z))); }
+
+__device__ __forceinline__ int clamp_len(long long l, int T) { return l <= 0 ? 0 : (l >= T ? T : (int)l); }
+
+// Stages W into wt[j * na + i] (and, if w_rm, into w_rm[i * nh + j] as well).
+__device__ __forceinline__ void aux_stage_w(const float* __restrict__ W, int na, int nh, float* wt, float* w_rm) {
+  for (int idx = threadIdx.x; idx < na * nh; idx += blockDim.x) {
+    const float w = __ldg(W + idx);
+    wt[(idx % nh) * na + idx / nh] = w;
+    if (w_rm) w_rm[idx] = w;
+  }
+}
+
+// q = W h for the lane's two rows (0 past na); h0 / h1: the lane's elements j = lane, lane + 32 of h (0 past nh).
+__device__ __forceinline__ void aux_q(const float* wt, int na, int nh, float h0, float h1, float& q0, float& q1) {
+  const int lane = threadIdx.x & 31;
+  q0 = q1 = 0.f;
+  for (int j = 0; j < nh; ++j) {
+    const float hj = __shfl_sync(FULL, j < 32 ? h0 : h1, j & 31);
+    if (lane < na) q0 = fmaf(wt[j * na + lane], hj, q0);
+    if (lane + 32 < na) q1 = fmaf(wt[j * na + lane + 32], hj, q1);
+  }
+}
+
+struct AuxRow {
+  float v0, v1;
+  __device__ __forceinline__ void load(const float* __restrict__ r, int na) {
+    const int lane = threadIdx.x & 31;
+    v0 = lane < na ? __ldg(r + lane) : 0.f;
+    v1 = lane + 32 < na ? __ldg(r + lane + 32) : 0.f;
+  }
+  __device__ __forceinline__ float dot(float q0, float q1) const { return warp_sum(fmaf(q1, v1, q0 * v0)); }
+};
+
+__device__ __forceinline__ void aux_store(float* __restrict__ r, int na, float v0, float v1) {
+  const int lane = threadIdx.x & 31;
+  if (lane < na) r[lane] = v0;
+  if (lane + 32 < na) r[lane + 32] = v1;
+}
+
+// part[b * (T - 1) + t] = the term of position t of sample b, 0 where it does not count.
+__global__ void __launch_bounds__(AUX_WARPS * 32) dien_aux_fwd_kernel(
+    const float* __restrict__ x, const float* __restrict__ neg, const long long* __restrict__ len,
+    const float* __restrict__ W, int B, int T, int na, int nh, int T_neg, const float* __restrict__ wsH,
+    float* __restrict__ part) {
+  extern __shared__ float wt[];
+  aux_stage_w(W, na, nh, wt, nullptr);
+  __syncthreads();
+  const int lane = threadIdx.x & 31, n = B * (T - 1);
+  for (int p = blockIdx.x * AUX_WARPS + threadIdx.x / 32; p < n; p += gridDim.x * AUX_WARPS) {
+    const int b = p / (T - 1), t = p % (T - 1);
+    float term = 0.f;
+    if (t + 1 < clamp_len(len[b], T)) {
+      const float* h = wsH + ((size_t)b * T + t) * nh;
+      float q0, q1;
+      aux_q(wt, na, nh, lane < nh ? h[lane] : 0.f, lane + 32 < nh ? h[lane + 32] : 0.f, q0, q1);
+      AuxRow r;
+      r.load(x + ((size_t)b * T + t + 1) * na, na);
+      term = softplus(-r.dot(q0, q1));
+      const float* nr = neg + (size_t)p * T_neg * na;
+      for (int k = 0; k < T_neg; ++k) {
+        r.load(nr + (size_t)k * na, na);
+        term += softplus(r.dot(q0, q1));
+      }
+    }
+    if (lane == 0) part[p] = term;
+  }
+}
+
+// aux_loss = (sum of the n terms) / B in float64: one CTA, strided partial sums then a fixed tree, so the bits do not depend
+// on timing.
+constexpr int AUX_SUM_THREADS = 1024;
+__global__ void __launch_bounds__(AUX_SUM_THREADS) dien_aux_sum_kernel(const float* __restrict__ part, int n, int B,
+                                                                       float* __restrict__ aux_loss) {
+  __shared__ double s[AUX_SUM_THREADS];
+  double v = 0.0;
+  for (int p = threadIdx.x; p < n; p += AUX_SUM_THREADS) v += part[p];
+  s[threadIdx.x] = v;
+  __syncthreads();
+  for (int o = AUX_SUM_THREADS / 2; o > 0; o >>= 1) {
+    if (threadIdx.x < o) s[threadIdx.x] += s[threadIdx.x + o];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) *aux_loss = (float)(s[0] / B);
+}
+
+// Backward given g = *g_aux (scale g / B): recomputes q_t and z, writes d_neg (every row, exact zeros at t >= L - 1), the
+// positive-row term of d_x (row t + 1 gets g+ q_t; rows 0 and >= L exactly 0), dL/dh_t = W^T dq_t into wsDH (0 at t = L - 1)
+// for dien_bwd_aux_kernel, and d_W = sum dq_t (x) h_t (shared-memory sums, one global atomic per element per CTA).
+__global__ void __launch_bounds__(AUX_WARPS * 32) dien_aux_bwd_kernel(
+    const float* __restrict__ x, const float* __restrict__ neg, const long long* __restrict__ len,
+    const float* __restrict__ W, const float* __restrict__ g_aux, int B, int T, int na, int nh, int T_neg,
+    const float* __restrict__ wsH, float* __restrict__ wsDH, float* __restrict__ d_x, float* __restrict__ d_neg,
+    float* __restrict__ d_W) {
+  extern __shared__ float sm[];
+  const int nw = na * nh;
+  float *wt = sm, *w_rm = sm + nw, *acc = sm + 2 * nw;
+  aux_stage_w(W, na, nh, wt, w_rm);
+  for (int i = threadIdx.x; i < nw; i += blockDim.x) acc[i] = 0.f;
+  __syncthreads();
+  const int lane = threadIdx.x & 31;
+  const float gs = __ldg(g_aux) / (float)B;
+  const int n = B * T;
+  for (int p = blockIdx.x * AUX_WARPS + threadIdx.x / 32; p < n; p += gridDim.x * AUX_WARPS) {
+    const int b = p / T, t = p % T, L = clamp_len(len[b], T);
+    const size_t row = (size_t)b * T;
+    if (t == 0) aux_store(d_x + row * na, na, 0.f, 0.f);             // row 0 has no positive term
+    if (t == L - 1) {                                                // the last state feeds no aux term
+      if (lane < nh) wsDH[(row + t) * nh + lane] = 0.f;
+      if (lane + 32 < nh) wsDH[(row + t) * nh + lane + 32] = 0.f;
+    }
+    if (t + 1 >= T) continue;
+    float* dn = d_neg + (((size_t)b * (T - 1) + t) * T_neg) * na;
+    if (t + 1 >= L) {                                                // not counted: exact zeros
+      for (int k = 0; k < T_neg; ++k) aux_store(dn + (size_t)k * na, na, 0.f, 0.f);
+      aux_store(d_x + (row + t + 1) * na, na, 0.f, 0.f);
+      continue;
+    }
+    const float* h = wsH + (row + t) * nh;
+    const float h0 = lane < nh ? h[lane] : 0.f, h1 = lane + 32 < nh ? h[lane + 32] : 0.f;
+    float q0, q1;
+    aux_q(wt, na, nh, h0, h1, q0, q1);
+    AuxRow r;
+    r.load(x + (row + t + 1) * na, na);
+    const float gp = gs * (sigm(r.dot(q0, q1)) - 1.f);
+    float dq0 = gp * r.v0, dq1 = gp * r.v1;
+    aux_store(d_x + (row + t + 1) * na, na, gp * q0, gp * q1);
+    const float* nr = neg + (((size_t)b * (T - 1) + t) * T_neg) * na;
+    for (int k = 0; k < T_neg; ++k) {
+      r.load(nr + (size_t)k * na, na);
+      const float gn = gs * sigm(r.dot(q0, q1));
+      aux_store(dn + (size_t)k * na, na, gn * q0, gn * q1);
+      dq0 = fmaf(gn, r.v0, dq0);
+      dq1 = fmaf(gn, r.v1, dq1);
+    }
+    // dh_j = sum_i W[i, j] dq_i for the lane's j = lane, lane + 32
+    float dh0 = 0.f, dh1 = 0.f;
+    for (int i = 0; i < na; ++i) {
+      const float dqi = __shfl_sync(FULL, i < 32 ? dq0 : dq1, i & 31);
+      if (lane < nh) dh0 = fmaf(w_rm[i * nh + lane], dqi, dh0);
+      if (lane + 32 < nh) dh1 = fmaf(w_rm[i * nh + lane + 32], dqi, dh1);
+    }
+    if (lane < nh) wsDH[(row + t) * nh + lane] = dh0;
+    if (lane + 32 < nh) wsDH[(row + t) * nh + lane + 32] = dh1;
+    // d_W[i, j] += dq_i h_j
+    for (int base = 0; base < nw; base += 32) {
+      const int idx = base + lane, i = idx / nh, j = idx % nh;
+      const float a0 = __shfl_sync(FULL, dq0, i & 31), a1 = __shfl_sync(FULL, dq1, i & 31);
+      const float c0 = __shfl_sync(FULL, h0, j & 31), c1 = __shfl_sync(FULL, h1, j & 31);
+      if (idx < nw) atomicAdd(acc + idx, (i < 32 ? a0 : a1) * (j < 32 ? c0 : c1));
+    }
+  }
+  __syncthreads();
+  for (int i = threadIdx.x; i < nw; i += blockDim.x) atomicAdd(d_W + i, acc[i]);
+}
+
 // ------------------------------------------------------------------------------------------------------------ host
 struct DienWs {
   float *H, *S, *A, *DH, *DA;
@@ -803,6 +992,22 @@ int check_dien(const char* fn, int64_t B, int64_t T, int64_t na, int64_t nh) {
 }
 
 int dien_nhp(int64_t nh) { return nh <= 8 ? 8 : nh <= 16 ? 16 : nh <= 32 ? 32 : 64; }
+
+// The auxiliary loss's workspace: the DIEN workspace, then one float per position t < T - 1 of every sample.
+int64_t dien_aux_ws_bytes(int64_t B, int64_t T, int64_t nh) { return (int64_t)sizeof(float) * (dien_ws_floats(B, T, nh) + B * (T - 1)); }
+
+int check_dien_aux(const char* fn, int64_t B, int64_t T, int64_t na, int64_t nh, int64_t T_neg) {
+  int rc = check_dien(fn, B, T, na, nh);
+  if (rc) return rc;
+  CTR_REQUIRE(T_neg >= 1, "%s: T_neg=%lld must be >= 1", fn, (long long)T_neg);
+  CTR_UNSUPPORTED(T_neg >= (1ll << 31) || B * (T - 1) * T_neg * na >= (1ll << 31),
+                  "%s: B=%lld T=%lld T_neg=%lld na=%lld: more than 2^31 - 1 negative-row elements", fn, (long long)B,
+                  (long long)T, (long long)T_neg, (long long)na);
+  return CTR_OK;
+}
+
+// Persistent grid of warps, one position each, over n positions.
+long long dien_aux_ctas(int64_t n) { return (n + AUX_WARPS - 1) / AUX_WARPS; }
 
 }  // namespace
 }  // namespace ctr
@@ -862,6 +1067,76 @@ extern "C" int ctr_dien_bwd(const float* seq_input, const int64_t* seq_length, c
   return with_const<8, 16, 32, 64>(nhp, [&](auto NHP) {
     return with_const<0, 1>(cell_type, [&](auto CELL) {
       return launch_resident("ctr_dien_bwd", dien_bwd_kernel<NHP, CELL>, need, DIEN_WARPS * 32, smem, st, seq_input,
+                             reinterpret_cast<const long long*>(seq_length), target_input, params, g_final_state, (int)B,
+                             (int)T, (int)na, (int)nh, w.H, w.S, w.A, w.DH, w.DA, d_seq_input, d_target_input, d_params);
+    });
+  });
+}
+
+extern "C" int ctr_dien_aux_workspace_bytes(int64_t B, int64_t T, int64_t na, int64_t nh, int64_t T_neg, int64_t* bytes) {
+  int rc = check_dien_aux("ctr_dien_aux_workspace_bytes", B, T, na, nh, T_neg);
+  if (rc) return rc;
+  CTR_REQUIRE(bytes, "ctr_dien_aux_workspace_bytes: null argument");
+  *bytes = dien_aux_ws_bytes(B, T, nh);
+  return CTR_OK;
+}
+
+extern "C" int ctr_dien_aux_fwd(const float* seq_input, const float* neg_seq_input, const int64_t* seq_length,
+                                const float* w_aux, int64_t B, int64_t T, int64_t na, int64_t nh, int64_t T_neg,
+                                float* aux_loss, void* workspace, int64_t workspace_bytes, void* stream) {
+  int rc = check_dien_aux("ctr_dien_aux_fwd", B, T, na, nh, T_neg);
+  if (rc) return rc;
+  CTR_REQUIRE(seq_input && neg_seq_input && seq_length && w_aux && aux_loss && workspace, "ctr_dien_aux_fwd: null argument");
+  CTR_REQUIRE(workspace_bytes >= dien_aux_ws_bytes(B, T, nh),
+              "ctr_dien_aux_fwd: workspace_bytes=%lld < ctr_dien_aux_workspace_bytes()", (long long)workspace_bytes);
+  cudaStream_t st = as_stream(stream);
+  if (B == 0) {
+    CTR_CUDA(cudaMemsetAsync(aux_loss, 0, sizeof(float), st));
+    return CTR_OK;
+  }
+  const DienWs w = dien_ws(workspace, B, T, nh);
+  float* part = static_cast<float*>(workspace) + dien_ws_floats(B, T, nh);
+  const int n = (int)(B * (T - 1));
+  if (n > 0)
+    rc = launch_resident("ctr_dien_aux_fwd", dien_aux_fwd_kernel, dien_aux_ctas(n), AUX_WARPS * 32,
+                       sizeof(float) * (size_t)(na * nh), st, seq_input, neg_seq_input,
+                       reinterpret_cast<const long long*>(seq_length), w_aux, (int)B, (int)T, (int)na, (int)nh, (int)T_neg,
+                       (const float*)w.H, part);
+  if (rc) return rc;
+  return launch("ctr_dien_aux_fwd", dien_aux_sum_kernel, dim3(1), dim3(AUX_SUM_THREADS), 0, st, (const float*)part, n, (int)B,
+                aux_loss);
+}
+
+extern "C" int ctr_dien_bwd_aux(const float* seq_input, const float* neg_seq_input, const int64_t* seq_length,
+                                const float* target_input, const float* params, const float* w_aux, const float* g_final_state,
+                                const float* g_aux_loss, int64_t B, int64_t T, int64_t na, int64_t nh, int64_t T_neg,
+                                int cell_type, float* d_seq_input, float* d_neg_seq_input, float* d_target_input,
+                                float* d_params, float* d_w_aux, void* workspace, int64_t workspace_bytes, void* stream) {
+  int rc = check_dien_aux("ctr_dien_bwd_aux", B, T, na, nh, T_neg);
+  if (rc) return rc;
+  CTR_REQUIRE(cell_type == 0 || cell_type == 1, "ctr_dien_bwd_aux: cell_type=%d (0 = AGRU, 1 = AUGRU)", cell_type);
+  CTR_REQUIRE(seq_input && neg_seq_input && seq_length && target_input && params && w_aux && g_final_state && g_aux_loss &&
+                  d_seq_input && d_neg_seq_input && d_target_input && d_params && d_w_aux && workspace,
+              "ctr_dien_bwd_aux: null argument");
+  CTR_REQUIRE(workspace_bytes >= (int64_t)sizeof(float) * dien_ws_floats(B, T, nh),
+              "ctr_dien_bwd_aux: workspace_bytes=%lld < ctr_dien_workspace_bytes()", (long long)workspace_bytes);
+  const DienParams o = dien_params((int)na, (int)nh);
+  cudaStream_t st = as_stream(stream);
+  CTR_CUDA(cudaMemsetAsync(d_params, 0, sizeof(float) * o.total, st));
+  CTR_CUDA(cudaMemsetAsync(d_w_aux, 0, sizeof(float) * (size_t)(na * nh), st));
+  if (B == 0) return CTR_OK;
+  const DienWs w = dien_ws(workspace, B, T, nh);
+  rc = launch_resident("ctr_dien_bwd_aux", dien_aux_bwd_kernel, dien_aux_ctas(B * T), AUX_WARPS * 32,
+                       3 * sizeof(float) * (size_t)(na * nh), st, seq_input, neg_seq_input,
+                       reinterpret_cast<const long long*>(seq_length), w_aux, g_aux_loss, (int)B, (int)T, (int)na, (int)nh,
+                       (int)T_neg, (const float*)w.H, w.DH, d_seq_input, d_neg_seq_input, d_w_aux);
+  if (rc) return rc;
+  const int nhp = dien_nhp(nh), spw = 32 / (nhp < 32 ? nhp : 32);
+  const long long need = ((B + spw - 1) / spw + DIEN_WARPS - 1) / DIEN_WARPS;
+  const size_t smem = sizeof(float) * (size_t)o.total;
+  return with_const<8, 16, 32, 64>(nhp, [&](auto NHP) {
+    return with_const<0, 1>(cell_type, [&](auto CELL) {
+      return launch_resident("ctr_dien_bwd_aux", dien_bwd_aux_kernel<NHP, CELL>, need, DIEN_WARPS * 32, smem, st, seq_input,
                              reinterpret_cast<const long long*>(seq_length), target_input, params, g_final_state, (int)B,
                              (int)T, (int)na, (int)nh, w.H, w.S, w.A, w.DH, w.DA, d_seq_input, d_target_input, d_params);
     });

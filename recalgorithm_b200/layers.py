@@ -326,6 +326,15 @@ def dien_interest_evolution(sequnence_input: torch.Tensor, sequnence_length: tor
     ``attention_project_matrix`` (nh, na), and the custom cell's ``rnn/{gates,candidate}/{kernel,bias}`` (gate bias ones,
     custom_grucell.py:66-68).  Kernels are glorot-uniform.  ``custom_gru_type == "AUGRU"`` selects AUGRU; ANY other value
     selects AGRU (dien.py:220-223).  ``gru_output_units`` may arrive as a string."""
+    nh, na, cell, params = _dien_variables(sequnence_input, gru_output_units, custom_gru_type)
+    final_state, scores = autograd.dien(sequnence_input, sequnence_length.to(torch.int64), target_input, params, nh, cell)
+    if return_attention_scores:
+        return final_state, scores.unsqueeze(-1)
+    return final_state
+
+
+def _dien_variables(sequnence_input, gru_output_units, custom_gru_type):
+    """The nine variables of the seq_encoder block in the caller's scope (ops.DIEN_PARAM_ORDER) -> (nh, na, cell, params)."""
     nh = int(gru_output_units)
     na = int(sequnence_input.shape[-1])
     cell = 1 if custom_gru_type == "AUGRU" else 0
@@ -342,11 +351,38 @@ def dien_interest_evolution(sequnence_input: torch.Tensor, sequnence_length: tor
             egk = get_variable("kernel", (2 * nh, 2 * nh)); egb = get_variable("bias", (2 * nh,), initializer=ones)
         with variable_scope("candidate"):
             eck = get_variable("kernel", (2 * nh, nh)); ecb = get_variable("bias", (nh,), initializer=zeros)
-    final_state, scores = autograd.dien(sequnence_input, sequnence_length.to(torch.int64), target_input,
-                                        (gk, gb, ck, cb, att, egk, egb, eck, ecb), nh, cell)
+    return nh, na, cell, (gk, gb, ck, cb, att, egk, egb, eck, ecb)
+
+
+def dien_interest_evolution_aux(sequnence_input: torch.Tensor, sequnence_length: torch.Tensor, target_input: torch.Tensor,
+                                neg_sequnence_input: torch.Tensor, aux_project_matrix: torch.Tensor, gru_output_units,
+                                custom_gru_type: str = "AGRU", negative_sample_number=3,
+                                return_attention_scores: bool = False):
+    """dien_interest_evolution plus DIEN's auxiliary loss (DIEN/dien.py:256-300) over the same extractor states h_t, one
+    kernel set each way.  Returns ``(final_state, aux_loss)``, or ``(final_state, attention_scores (B, T, 1), aux_loss)``
+    when ``return_attention_scores``.
+
+    ``aux_loss = -(1/B) sum_b sum_{t < len-1} [log sig(h_t . W^T x_{t+1}) + sum_n log(1 - sig(h_t . W^T neg_{t,n}))]`` with
+    W = ``aux_project_matrix`` (na, nh): the paper's next-behaviour loss, i.e. the negative of the reference's aux_loss, in
+    the numerically stable softplus form.  ``neg_sequnence_input`` (B, (T-1)*negative_sample_number, na) holds the
+    negatives of position t in rows t*T_neg .. t*T_neg + T_neg - 1 (the reshape at :279); the caller samples them, e.g.
+    through the shared ``feedid`` table.  ``aux_project_matrix`` is an argument because the reference creates it in
+    model_fn's own ``aux_loss`` scope; the nine seq_encoder variables are created in the caller's scope exactly as by
+    dien_interest_evolution.  ``negative_sample_number`` may arrive as a string, like ``gru_output_units``."""
+    T_neg = int(negative_sample_number)
+    nh, na, cell, params = _dien_variables(sequnence_input, gru_output_units, custom_gru_type)
+    B, T = sequnence_input.shape[:2]
+    want = (B, (T - 1) * T_neg, na)
+    if tuple(neg_sequnence_input.shape) != want:
+        raise ValueError(f"neg_sequnence_input: expected shape {want} ((B, (T-1)*negative_sample_number, na)), "
+                         f"got {tuple(neg_sequnence_input.shape)}")
+    if tuple(aux_project_matrix.shape) != (na, nh):
+        raise ValueError(f"aux_project_matrix: expected shape {(na, nh)}, got {tuple(aux_project_matrix.shape)}")
+    final_state, scores, aux_loss = autograd.dien_aux(sequnence_input, sequnence_length.to(torch.int64), target_input,
+                                                      neg_sequnence_input, aux_project_matrix, params, nh, cell, T_neg)
     if return_attention_scores:
-        return final_state, scores.unsqueeze(-1)
-    return final_state
+        return final_state, scores.unsqueeze(-1), aux_loss
+    return final_state, aux_loss
 
 
 # --------------------------------------------------------------------------------------------------- DeepCrossing

@@ -818,6 +818,61 @@ def dien_bwd(seq, seq_len, target, packed, g_final, nh: int, cell: int, ws):
     return d_seq, d_tgt, d_p
 
 
+def _dien_aux_args(seq, neg_seq, w_aux, nh, T_neg):
+    B, T, na = seq.shape
+    if int(T_neg) < 1:
+        raise ValueError(f"negative_sample_number must be >= 1, got {T_neg!r}")
+    _chk(neg_seq, F32, "neg_sequnence_input", (B, (T - 1) * int(T_neg), na))
+    _chk(w_aux, F32, "aux_project_matrix", (na, nh))
+
+
+def dien_aux_workspace(B: int, T: int, na: int, nh: int, T_neg: int, device) -> torch.Tensor:
+    """One workspace for dien_fwd, dien_aux_fwd and dien_bwd_aux: the DIEN workspace plus per-sample partials."""
+    nbytes = ctypes.c_int64(0)
+    _lib.check(_lib.lib().ctr_dien_aux_workspace_bytes(B, T, na, nh, T_neg, ctypes.byref(nbytes)))
+    return torch.empty((int(nbytes.value),), dtype=torch.uint8, device=device)
+
+
+def dien_fwd_aux(seq, seq_len, target, neg_seq, packed, w_aux, nh: int, cell: int, T_neg: int):
+    """DIEN/dien.py:198-229 and the auxiliary loss :256-300 with the paper's sign: (final_state (B,nh), attention scores
+    (B,T), aux_loss (), workspace for dien_bwd_aux)."""
+    B, T, na = _dien_args(seq, seq_len, target, packed, nh, cell)
+    _dien_aux_args(seq, neg_seq, w_aux, nh, T_neg)
+    final = torch.empty((B, nh), dtype=F32, device=seq.device)
+    scores = torch.empty((B, T), dtype=F32, device=seq.device)
+    ws = dien_aux_workspace(B, T, na, nh, T_neg, seq.device)
+    _lib.check(_lib.lib().ctr_dien_fwd(_ptr(seq), _ptr(seq_len), _ptr(target), _ptr(packed), B, T, na, nh, cell, _ptr(final),
+                                       _ptr(scores), _ptr(ws), ws.numel(), _stream()))
+    aux = dien_aux_fwd(seq, neg_seq, seq_len, w_aux, nh, T_neg, ws)
+    return final, scores, aux, ws
+
+
+def dien_aux_fwd(seq, neg_seq, seq_len, w_aux, nh: int, T_neg: int, ws):
+    """The auxiliary loss () of the states dien_fwd_aux (or ctr_dien_fwd on this dien_aux_workspace) left in ws."""
+    B, T, na = seq.shape
+    _chk(seq, F32, "sequnence_input"); _chk(seq_len, I64, "sequnence_length", (B,))
+    _dien_aux_args(seq, neg_seq, w_aux, nh, T_neg)
+    aux = torch.empty((), dtype=F32, device=seq.device)
+    _lib.check(_lib.lib().ctr_dien_aux_fwd(_ptr(seq), _ptr(neg_seq), _ptr(seq_len), _ptr(w_aux), B, T, na, nh, int(T_neg),
+                                           _ptr(aux), _ptr(ws), ws.numel(), _stream()))
+    return aux
+
+
+def dien_bwd_aux(seq, seq_len, target, neg_seq, packed, w_aux, g_final, g_aux, nh: int, cell: int, T_neg: int, ws):
+    """Gradients of dien_fwd_aux given d final_state (B,nh) and d aux_loss (a device scalar): (d_seq (B,T,na), d_neg_seq,
+    d_target (B,na), d_packed, d_w_aux (na,nh))."""
+    B, T, na = _dien_args(seq, seq_len, target, packed, nh, cell)
+    _dien_aux_args(seq, neg_seq, w_aux, nh, T_neg)
+    _chk(g_final, F32, "g_final_state", (B, nh))
+    _chk(g_aux, F32, "g_aux_loss", ())
+    d_seq, d_neg, d_tgt = torch.empty_like(seq), torch.empty_like(neg_seq), torch.empty_like(target)
+    d_p, d_w = torch.empty_like(packed), torch.empty_like(w_aux)
+    _lib.check(_lib.lib().ctr_dien_bwd_aux(_ptr(seq), _ptr(neg_seq), _ptr(seq_len), _ptr(target), _ptr(packed), _ptr(w_aux),
+                                           _ptr(g_final), _ptr(g_aux), B, T, na, nh, int(T_neg), cell, _ptr(d_seq), _ptr(d_neg),
+                                           _ptr(d_tgt), _ptr(d_p), _ptr(d_w), _ptr(ws), ws.numel(), _stream()))
+    return d_seq, d_neg, d_tgt, d_p, d_w
+
+
 # ------------------------------------------------------------------------------------ DeepCrossing residual unit
 def residual_unit_workspace(B: int, d: int, H: int, device) -> torch.Tensor:
     """Caller-owned workspace: the prepped weights (B = 0, what the forward needs) plus, for the backward, h and its gradient."""

@@ -4,7 +4,7 @@
 Each kernel is timed alone with CUDA events; an L2 flush (a 256 MB write) runs between timed iterations because these
 working sets are flushed from the 50 MB L2.  Prints one JSON line per measurement.
 
-    python tools/bench_layers.py [--iters 20] [--only cin,dcn,din,fibinet]     (also: pairwise, bst, adam, pnn, dien, deepcrossing, mmoe, ple, wide, autoint, flen)
+    python tools/bench_layers.py [--iters 20] [--only cin,dcn,din,fibinet]     (also: pairwise, bst, adam, pnn, dien, dien_aux, deepcrossing, mmoe, ple, wide, autoint, flen)
 """
 import argparse
 import json
@@ -207,6 +207,64 @@ def dien_rows(iters, flush, hbm):
                                   "note": "autograd of the same torch form (backward only), fp32, TF32 disabled"}), flush=True)
     finally:
         torch.backends.cuda.matmul.allow_tf32 = prev_tf32
+
+
+def dien_aux_rows(iters, flush, hbm):
+    """DIEN auxiliary loss at DIEN's reference shape (T = 50, na = 16, nh = 8, lengths uniform in {0..50}) with T_neg = 3, B =
+    4096 and 65 536, both cells: ctr_dien_aux_fwd alone, ctr_dien_bwd_aux next to the plain ctr_dien_bwd, and the whole step
+    (forward, aux forward, backward) with and without the loss.  HBM floors from shapes: the aux forward reads, per counted
+    position (t < len - 1), the positive row, T_neg negative rows and h_t; the aux backward reads the same, writes every
+    negative-row gradient (zeros included), the positive-row term of d_seq_input (all B*T rows) and dL/dh_t, and
+    ctr_dien_bwd_aux reads that d_seq_input and dL/dh back."""
+    import subprocess
+    T, na, nh, T_neg = 50, 16, 8, 3
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.sm,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                       capture_output=True, text=True)
+    print(json.dumps({"dien_aux_card": {"device": torch.cuda.get_device_name(0),
+                                        "name, power.limit, clocks.sm, clocks.max.sm": q.stdout.strip() or q.stderr.strip()}}),
+          flush=True)
+    gen = torch.Generator(device="cuda").manual_seed(50)
+    for B in (4096, 65536):
+        L = torch.randint(0, T + 1, (B,), device="cuda", generator=gen)
+        seq = torch.randn((B, T, na), device="cuda", generator=gen) * 0.7
+        seq[torch.arange(T, device="cuda")[None, :] >= L[:, None]] = 0
+        neg = torch.randn((B, (T - 1) * T_neg, na), device="cuda", generator=gen) * 0.7
+        tgt = torch.randn((B, na), device="cuda", generator=gen) * 0.7
+        g = torch.randn((B, nh), device="cuda", generator=gen)
+        g_aux = torch.ones((), device="cuda")
+        params = [(torch.rand(s, device="cuda", generator=gen) * 2 - 1) * (0.5 if len(s) == 1 else (6.0 / sum(s)) ** 0.5)
+                  for s in ops.dien_param_shapes(na, nh)]
+        w = (torch.rand((na, nh), device="cuda", generator=gen) * 2 - 1) * (6.0 / (na + nh)) ** 0.5
+        packed = ops.dien_pack_params(params, na, nh)
+        P = int((L - 1).clamp(min=0).sum())                         # counted positions
+        fwd_bytes = 4 * P * (na * (1 + T_neg) + nh) + 8 * B + 8 * B + 8 * B
+        bwd_bytes = 4 * (P * (na * (1 + T_neg) + 2 * nh) + B * (T - 1) * T_neg * na + B * T * na) + 8 * B
+        extra_bytes = 4 * (B * T * na + P * nh)                     # ctr_dien_bwd_aux re-reads the seeds it adds to
+        for cell, tag in ((0, "agru"), (1, "augru")):
+            cfg = {"cell": tag.upper(), "B": B, "T": T, "na": na, "nh": nh, "T_neg": T_neg, "lengths": "uniform 0..50",
+                   "counted_positions": P}
+            _, _, _, ws = ops.dien_fwd_aux(seq, L, tgt, neg, packed, w, nh, cell, T_neg)
+            rows = (("dien_aux_fwd", lambda: ops.dien_aux_fwd(seq, neg, L, w, nh, T_neg, ws), fwd_bytes),
+                    ("dien_bwd", lambda: ops.dien_bwd(seq, L, tgt, packed, g, nh, cell, ws), None),
+                    ("dien_bwd_aux", lambda: ops.dien_bwd_aux(seq, L, tgt, neg, packed, w, g, g_aux, nh, cell, T_neg, ws),
+                     bwd_bytes + extra_bytes),
+                    ("step_plain", lambda: ops.dien_bwd(seq, L, tgt, packed, g, nh, cell,
+                                                        ops.dien_fwd(seq, L, tgt, packed, nh, cell)[2]), None),
+                    ("step_aux", lambda: ops.dien_bwd_aux(seq, L, tgt, neg, packed, w, g, g_aux, nh, cell, T_neg,
+                                                          ops.dien_fwd_aux(seq, L, tgt, neg, packed, w, nh, cell, T_neg)[3]),
+                     None))
+            ms = {}
+            for name, fn, nbytes in rows:
+                m, bst = timeit(fn, iters, flush)
+                ms[name] = m
+                line = {"kernel": f"{name}_{tag}", "config": cfg, "ms_median": m, "ms_best": bst, "iters": iters,
+                        "l2": "flushed between iterations"}
+                if nbytes is not None:
+                    line.update(hbm_floor_ms=nbytes / (hbm * 1e9) * 1e3, algorithmic_bytes=nbytes)
+                print(json.dumps(line), flush=True)
+            print(json.dumps({"kernel": f"dien_aux_overhead_{tag}", "config": cfg,
+                              "bwd_aux_over_bwd": ms["dien_bwd_aux"] / ms["dien_bwd"] - 1,
+                              "step_aux_over_step_plain": ms["step_aux"] / ms["step_plain"] - 1}), flush=True)
 
 
 def deepcrossing_rows(iters, flush, rn):
@@ -785,6 +843,8 @@ def main():
         pnn_rows(args.iters, flush, rn, hbm)
     if "dien" in only:  # DIEN seq_encoder at the reference shape (na = 16, nh = 8) with config 4's T and lengths; not in the default list
         dien_rows(args.iters, flush, hbm)
+    if "dien_aux" in only:  # DIEN's auxiliary loss at the same shape with T_neg = 3; not in the default list
+        dien_aux_rows(args.iters, flush, hbm)
     if "deepcrossing" in only:  # DeepCrossing residual unit at the reference width (d = 82) and both result.md H; not in the default list
         deepcrossing_rows(args.iters, flush, rn)
     if "mmoe" in only:  # MMoE expert-gate layer at the reference shape (d = 82, E = 3, H = 512, T = 3); not in the default list

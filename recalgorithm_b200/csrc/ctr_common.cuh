@@ -65,6 +65,13 @@ __device__ __forceinline__ float4 ldg_stream_f4(const float4* p) {
                : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "l"(p));
   return r;
 }
+// 128-bit load through the L1 path.  The config-5 streams (the lookup backward's tile and d_tile rows, the gather's random
+// 128-byte table rows) measured about 3 % faster this way than with ldg_stream_f4 (H100 SXM, 700 W).
+__device__ __forceinline__ float4 ldg_f4(const float4* p) {
+  float4 r;
+  asm volatile("ld.global.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "l"(p));
+  return r;
+}
 // write-once 128-bit store, evict-first in L2 (keeps hot table rows resident)
 __device__ __forceinline__ void stg_stream_f4(float4* p, const float4& v) {
   asm volatile("st.global.cs.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w)

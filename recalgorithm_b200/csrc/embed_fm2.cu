@@ -13,7 +13,8 @@
 //   row addresses of a sample are known before the first row load issues -> up to 8 independent
 //   128-bit loads in flight per lane (enough outstanding bytes per SM to cover HBM latency).
 //   S = sum_f e and Q = sum_f e^2 accumulate in registers; the FM2 logit is a shuffle reduction.
-//   The (B,F,D) tile is written with evict-first stores so it does not displace hot table rows in L2.
+//   The (B,F,D) tile is written with plain stores: its last-written rows are still in L2 when the backward, which walks the
+//   samples from the last one down, reads them first.
 #include "lookup_bwd.cuh"
 
 namespace ctr {
@@ -83,7 +84,7 @@ embed_fm2_fwd_kernel(const float4* __restrict__ table, const PeerTables peers, c
           v[u] = f4_zero();
           if (in[u] && r >= 0) {
             if (SH) v[u] = ld_peer_f4(peers.base[r & (peers.G - 1)] + (size_t)(r >> peers.logG) * LPR + c);
-            else v[u] = ldg_stream_f4(table + (size_t)r * LPR + c);
+            else v[u] = ldg_f4(table + (size_t)r * LPR + c);
           }
         }
 #pragma unroll
@@ -94,7 +95,7 @@ embed_fm2_fwd_kernel(const float4* __restrict__ table, const PeerTables peers, c
           Q.z = __fadd_rn(Q.z, __fmul_rn(v[u].z, v[u].z)); Q.w = __fadd_rn(Q.w, __fmul_rn(v[u].w, v[u].w));
           if (tile != nullptr && in[u]) {
             const int fs = (it0 + u) * RPW + sub;
-            stg_stream_f4(tile + ((size_t)b * F + f0 + fs) * LPR + c, v[u]);
+            tile[((size_t)b * F + f0 + fs) * LPR + c] = v[u];
           }
           if (LIN && in[u]) {
             const float4 w = __ldg(wlin + (size_t)(f0 + (it0 + u) * RPW + sub) * LPR + c);
@@ -159,7 +160,8 @@ embed_fm2_bwd_kernel(const float4* __restrict__ tile, const float4* __restrict__
   const int n4 = F * LPR;
   LinHead<MODE == FM2_LIN ? HOLD : 1> lin;
   if (MODE == FM2_LIN) lin.stage(s_lin, d_tile, n4);
-  for (int b = warp0; b < B; b += nwarps) {
+  for (int w = warp0; w < B; w += nwarps) {
+    const int b = B - 1 - w;   // last sample first: the forward wrote it last, so its tile row is the likeliest L2 hit
     StoreRow sink{row_grads + (size_t)b * n4};
     RowGrad rows{d_tile ? d_tile + (size_t)b * n4 : nullptr};   // not read in LIN mode
     float4 g4;
@@ -285,25 +287,37 @@ static int launch_fwd(const float* table, const PeerTables* peers, const int64_t
   PeerTables none = {};
   // 4 CTAs/SM (64 registers) measured 0.80 of HBM peak vs 0.71-0.80 uncapped; a next-sample id prefetch variant measured
   // neutral-to-negative (it costs spills) and was removed.  The sharded (peer-pull) variant keeps the register budget open.
-  const PeerTables& pt = peers ? *peers : none;
-  auto go = [&](auto k) {
-    return launch_resident("ctr_embed_fm2_fwd", k, (B + 7) / 8, 256, 0, st, reinterpret_cast<const float4*>(table), pt,
-                           reinterpret_cast<const long long*>(off), ids, (int)B, (int)F, reinterpret_cast<float4*>(tile), fm2,
-                           reinterpret_cast<long long*>(ids64_out), nullptr, nullptr);
-  };
-  return peers != nullptr ? go(embed_fm2_fwd_kernel<LPR, true, 1, false, IdT>) : go(embed_fm2_fwd_kernel<LPR, false, 4, false, IdT>);
+  // The local gather runs one CTA per 8 samples instead of a resident grid: CTAs start in order, so the tile rows being
+  // written at any moment stay in a narrow, advancing address range (1 % faster at config 5 on H100 SXM).
+  const float4* table4 = reinterpret_cast<const float4*>(table);
+  const long long* off64 = reinterpret_cast<const long long*>(off);
+  float4* tile4 = reinterpret_cast<float4*>(tile);
+  long long* ids64 = reinterpret_cast<long long*>(ids64_out);
+  if (peers != nullptr)
+    return launch_resident("ctr_embed_fm2_fwd", embed_fm2_fwd_kernel<LPR, true, 1, false, IdT>, (B + 7) / 8, 256, 0, st, table4,
+                           *peers, off64, ids, (int)B, (int)F, tile4, fm2, ids64, nullptr, nullptr);
+  return launch("ctr_embed_fm2_fwd", embed_fm2_fwd_kernel<LPR, false, 4, false, IdT>, (unsigned)((B + 7) / 8), 256, 0, st, table4,
+                none, off64, ids, (int)B, (int)F, tile4, fm2, ids64, nullptr, nullptr);
 }
 
 // FM2_LIN has no two-pass form: wider rows fail in with_hold with `what` in the message.
+// The plain and BI forms run one CTA per 8 samples (one sample per warp) instead of a resident grid: CTAs start in order, so
+// the rows in flight stay in a narrow, advancing address range, which measured 2.5 % faster at config 5 on H100 SXM.  The LIN
+// form stays resident: each CTA stages wlin and reduces its d_wlin once.
 template <int MODE>
 static int launch_bwd(const char* what, const float* tile, const float* d_tile, const float* d_fm2, const float* d_lin, int64_t B,
                       int64_t F, int64_t D, float* row_grads, float* d_wlin, cudaStream_t st) {
   return with_lpr(D, [&](auto LPR) {
     return with_hold<MODE != FM2_LIN>(F, LPR, [&](auto HOLD) {
-      return launch_resident(what, embed_fm2_bwd_kernel<LPR, HOLD, MODE>, (B + 7) / 8, 256,
-                             MODE == FM2_LIN ? sizeof(float4) * 2 * (size_t)F * LPR : 0, st, reinterpret_cast<const float4*>(tile),
-                             reinterpret_cast<const float4*>(d_tile), d_fm2, d_lin, (int)B, (int)F,
-                             reinterpret_cast<float4*>(row_grads), reinterpret_cast<float4*>(d_wlin));
+      const auto k = embed_fm2_bwd_kernel<LPR, HOLD, MODE>;
+      const float4* tile4 = reinterpret_cast<const float4*>(tile);
+      const float4* d_tile4 = reinterpret_cast<const float4*>(d_tile);
+      float4* row_grads4 = reinterpret_cast<float4*>(row_grads);
+      float4* d_wlin4 = reinterpret_cast<float4*>(d_wlin);
+      if (MODE != FM2_LIN)
+        return launch(what, k, (unsigned)((B + 7) / 8), 256, 0, st, tile4, d_tile4, d_fm2, d_lin, (int)B, (int)F, row_grads4, d_wlin4);
+      return launch_resident(what, k, (B + 7) / 8, 256, sizeof(float4) * 2 * (size_t)F * LPR, st, tile4, d_tile4, d_fm2, d_lin, (int)B,
+                             (int)F, row_grads4, d_wlin4);
     }, what);
   });
 }

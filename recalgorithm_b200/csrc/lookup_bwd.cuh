@@ -48,7 +48,7 @@ __device__ __forceinline__ void load_tile_row(float4 (&e)[HOLD], const float4* _
     const int j = k * 32 + lane;
     e[k] = f4_zero();
     if (j < n4) {
-      e[k] = ldg_stream_f4(e_row + j);
+      e[k] = ldg_f4(e_row + j);
       chunk(k, j);
     }
   }
@@ -70,7 +70,7 @@ __device__ __forceinline__ float4 tile_row_sum(const float4 (&e)[HOLD]) {
 struct RowGrad {
   const float4* __restrict__ row;
   __device__ __forceinline__ void load(float4& d, int j) const {
-    if (row != nullptr) d = ldg_stream_f4(row + j);
+    if (row != nullptr) d = ldg_f4(row + j);
   }
   __device__ __forceinline__ float4 at(int, const float4& d) const { return d; }
   __device__ __forceinline__ void add(int, const float4&) {}

@@ -53,6 +53,25 @@ def dcn_logit(dense_input: torch.Tensor, category_input: torch.Tensor, num_cross
         return dense(torch.cat([cross_vec, dnn_vec], dim=-1), 1)
 
 
+def dcn_v2_logit(dense_input: torch.Tensor, category_input: torch.Tensor, num_cross_layer: int = 3, projection_dim=None,
+                 structure: str = "stacked", hidden_units=(64, 32)):
+    """DCN-V2 (Wang et al., WWW 2021, arXiv:2008.13535) in dcn_logit's scopes: the cross network (layers.cross_network_v2,
+    full rank or rank projection_dim) in cross_part.  ``structure="stacked"`` feeds the cross output to the deep part and
+    the logit reads the deep output (the paper's Figure 1b); ``"parallel"`` runs the deep part on concat_all and the logit
+    reads both, concatenated, like DCN/dcn.py:167-169 (Figure 1a)."""
+    if structure not in ("stacked", "parallel"):
+        raise ValueError(f"structure must be 'stacked' or 'parallel', got {structure!r}")
+    concat_all = torch.cat([dense_input, category_input], dim=-1)
+    with L.variable_scope("cross_part"):
+        cross_vec = L.cross_network_v2(concat_all, num_cross_layer, projection_dim)
+    with L.variable_scope("dnn_part"):
+        dnn_vec = cross_vec if structure == "stacked" else concat_all
+        for i, unit in enumerate(hidden_units):
+            dnn_vec = dense(dnn_vec, unit, activation=torch.relu, name=f"dnn_dense_{i}")
+    with L.variable_scope("output_part"):
+        return dense(dnn_vec if structure == "stacked" else torch.cat([cross_vec, dnn_vec], dim=-1), 1)
+
+
 def xdeepfm_logit(dense_input: torch.Tensor, x0: torch.Tensor, cin_layer_feature_maps=("16", "16"), hidden_units=(64, 32)):
     """xDeepFM/xdeepfm.py:152-185.  x0: (B, m, D) tile; layer widths arrive as strings like in the reference (:253)."""
     B = x0.shape[0]

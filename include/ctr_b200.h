@@ -276,6 +276,33 @@ int ctr_embed_cross_fwd(const float* table, const int64_t* field_row_offset, con
                         int64_t B, int64_t F, int64_t D, const float* w, const float* b, int64_t L, float* x0, float* out,
                         void* stream);
 
+/* ---- Row CROSS-V2: DCN-V2 cross network ----------------------------------------------------------------
+ * The cross network of DCN-V2 (Wang et al., WWW 2021, arXiv:2008.13535, eq. 1-2).  The reference tree has no DCN-V2 code,
+ * so this row follows the paper and is checked against a float64 restatement of it.  Row-vector form, l = 0 .. L-1:
+ *   x_{l+1} = x0 * z_l + x_l,  z_l = x_l . W_l + b_l    x0 (B,d); x_0 = xl_in (B,d), or x0 when xl_in == NULL;
+ *   full rank (rank == 0):  W_l = w[l]          w (L,d,d); u is not read and may be NULL;
+ *   low rank (rank >= 1):   W_l = w[l] . u[l]   w (L,d,rank), u (L,rank,d) (the paper's V_l and U_l^T);
+ *   b (L,d); out (B,d) = x_L.
+ * fp32-class accuracy (3xTF32 on the tensor cores).  1 <= d <= 512, 1 <= L <= 8, 0 <= rank <= 128 (CTR_ERR_UNSUPPORTED
+ * otherwise); rows need no alignment; B = 0 launches nothing.  The entries never allocate or synchronise.
+ * saved: caller-owned, ctr_cross_v2_workspace_bytes' saved_bytes = B * ((2L - 1) d + L rank) * 4 bytes: the layer inputs
+ *   x_1 .. x_{L-1} (L-1, B, d), then z_0 .. z_{L-1} (L, B, d), then at low rank t_l = x_l . w[l] (L, B, rank).  The forward
+ *   writes it and the backward reads it.  A forward-only caller may pass saved = NULL (the layers then run in place in out).
+ * workspace: 128-byte aligned, at least the workspace_bytes of ctr_cross_v2_workspace_bytes(0, ..) for the forward (the
+ *   prepped tf32 weight copies) and of ctr_cross_v2_workspace_bytes(B, ..) for the backward (also dz, dt at low rank and
+ *   up to two dx_l, (B, d rounded up to 32), (B, rank rounded up to 32) and (B, d) each).
+ * The backward takes g_out = dL/dout (B,d).  dx0 (B,d) receives every use of x0 (and x_0 itself when xl_in == NULL);
+ * dxl_in (B,d) is written when xl_in != NULL.  dw, du (not touched at rank 0, may be NULL) and db are overwritten (zeros
+ * at B = 0; batch-reduced with fp32 atomics). */
+int ctr_cross_v2_workspace_bytes(int64_t B, int64_t d, int64_t L, int64_t rank, int64_t* workspace_bytes,
+                                 int64_t* saved_bytes);
+int ctr_cross_v2_fwd(const float* x0, const float* xl_in, const float* w, const float* u, const float* b, int64_t B,
+                     int64_t d, int64_t L, int64_t rank, float* out, void* saved, void* workspace, int64_t workspace_bytes,
+                     void* stream);
+int ctr_cross_v2_bwd(const float* x0, const float* xl_in, const float* w, const float* u, const float* b, const void* saved,
+                     const float* g_out, int64_t B, int64_t d, int64_t L, int64_t rank, float* dx0, float* dxl_in,
+                     float* dw, float* du, float* db, void* workspace, int64_t workspace_bytes, void* stream);
+
 /* ---- Row CIN: xDeepFM compressed-interaction layer -------------------------------------------------
  * Replaces cin_layer(x0, xk, hk_1, index) (xDeepFM/cin_layer.py:17-30):
  *   out[b,n,d] = sum_{i,j} xk[b,i,d] * x0[b,j,d] * filter[i*m + j, n]

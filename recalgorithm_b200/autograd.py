@@ -174,6 +174,31 @@ def cross_stack(x0: torch.Tensor, w: torch.Tensor, b: torch.Tensor, xl: Optional
     return _CrossStack.apply(x0, xl, w, b)
 
 
+class _CrossV2(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x0, xl, w, u, b, rank):
+        x0, w, b = (t.contiguous() for t in (x0, w, b))
+        u = u.contiguous() if rank else None
+        xl = None if xl is None else xl.contiguous()
+        out, saved = ops.cross_v2_fwd(x0, w, u, b, rank, xl_in=xl)
+        ctx.save_for_backward(x0, xl, w, u, b, saved)          # saved: the layer inputs x_1 .. x_{L-1}, z_l and t_l
+        ctx.rank = rank
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        x0, xl, w, u, b, saved = ctx.saved_tensors
+        dx0, dxl, dw, du, db = ops.cross_v2_bwd(x0, w, u, b, ctx.rank, saved, g.contiguous(), xl_in=xl)
+        return dx0, dxl, dw, du, db, None
+
+
+def cross_v2(x0: torch.Tensor, w: torch.Tensor, u: Optional[torch.Tensor], b: torch.Tensor, rank: int,
+             xl: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """All L DCN-V2 cross layers in one forward and one backward call: w (L,d,d) at rank 0, else w (L,d,rank) and
+    u (L,rank,d); b (L,d); xl the optional start vector (default x0)."""
+    return _CrossV2.apply(x0, xl, w, u, b, int(rank))
+
+
 class _LookupCross(torch.autograd.Function):
     @staticmethod
     def forward(ctx, anchor, tables: EmbeddingTables, ids, w, b):

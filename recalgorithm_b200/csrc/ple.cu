@@ -48,13 +48,12 @@ using namespace ctr::tc::rows;
 
 constexpr int TM = WG_M;                     // samples per forward / dz tile: both warpgroups share the tile's rows
 constexpr int PC = 2 * HC;                   // units per ring stage: one 32-unit half per warpgroup
-constexpr int SBYTES = 2 * PC * KB * 4;      // one stage: [64 units x 32 inputs], hi then lo
+constexpr int SBYTES = ks_stage_bytes<HC>(); // one stage: [64 units x 32 inputs], hi then lo
 constexpr int MAX_D = 512, MAX_H = 512, MAX_T = 4, MAX_E = 64, MAX_GC = 160;
 constexpr int DX_TILE = NWG * WG_M;          // samples per dx tile
-// 32-input slices per accumulation chain (4 k-steps x 3 = 12 MMAs each).  The tensor core truncates as it accumulates; with
-// 96-MMA chains the widest inputs missed the fp32 bars by up to 1.2x (the softmax turns a gate logit's absolute error into
-// the gate's relative error).  The row GEMMs drain every slice, the dx GEMM every two (its drain is 64 adds per thread).
-constexpr int KCHAIN = 1, DX_KCHAIN = 2;
+// 32-input slices per accumulation chain of the dx GEMM (4 k-steps x 3 = 12 MMAs each): it drains every two slices (its
+// drain is 64 adds per thread), the row GEMMs (rows::gemm_ks) every slice.
+constexpr int DX_KCHAIN = 2;
 
 // The gate structure of one call.  Experts: task t's at e0[t] .. e0[t] + n[t], the shared ones at ES .. ES + S.  Gate
 // g < T has columns c0[g] .. c0[g] + n[g] + S over [task g's experts, shared]; gate T (extraction network only) has
@@ -121,41 +120,6 @@ __global__ void ple_prep_kernel(const float* __restrict__ we, const float* __res
 }
 
 // ------------------------------------------------------------------------------------------------ shared device pieces
-// TMA loads of one stage: units u0 .. u0 + 63, inputs 32 kb .. 32 kb + 31, hi then lo, from the [2 R][DP] rows map.
-__device__ __forceinline__ void load_stage(uint32_t dst, const CUtensorMap* map, int u0, int kb, int R, uint32_t bar) {
-  tma_load_2d(dst, map, kb * KB, u0, bar);
-  tma_load_2d(dst + PC * 128, map, kb * KB, R + u0, bar);
-}
-
-// D[64 x HC] = X[64 x DP] . B over the next nk ring stages: X = the tile's staged rows (pitch ldx), B = this warpgroup's
-// 32-unit half of each stage.  One 32-input slice (4 k-steps) per stage; chains of KCHAIN slices drained into d.
-__device__ __forceinline__ void gemm_ks(float (&d)[HC / 2], const float* xs, int ldx, int nk, int r0, int t, int lane,
-                                        int wg, Ring& ring, uint32_t sbase) {
-  float dacc[HC / 2];
-#pragma unroll
-  for (int q = 0; q < HC / 2; ++q) { d[q] = 0.f; dacc[q] = 0.f; }
-  for (int kb = 0; kb < nk; ++kb) {
-    const uint32_t st = sbase + ring.wait() * SBYTES + wg * HC * 128;
-    const uint64_t bhi = gmma_desc_kmajor(st, 128), blo = gmma_desc_kmajor(st + PC * 128, 128);
-    uint32_t ah[4][4], al[4][4];
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) {
-      float a[4];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) a[q] = xs[(r0 + 8 * (q & 1)) * ldx + kb * KB + 8 * ks + t + 4 * (q >> 1)];
-      tf32_split(a, ah[ks], al[ks]);
-    }
-    const bool start = chain_first(kb, KCHAIN);
-    wgmma_fence();
-#pragma unroll
-    for (int ks = 0; ks < 4; ++ks) mma_3xtf32<HC>(dacc, ah[ks], al[ks], bhi, blo, (uint64_t)(2 * ks), (start && ks == 0) ? 0 : 1);
-    wgmma_commit();
-    wgmma_wait_keep(ah, al);
-    ring.release(lane);
-    if (chain_last(kb, nk, KCHAIN)) chain_drain(d, dacc);
-  }
-}
-
 // Stages the tile's 64 rows of x (B,d), zero padded to DP columns and past B, with all 256 consumer threads.
 __device__ __forceinline__ void stage_tile(float* xs, int ldx, const float* __restrict__ x, long long base, int B, int d,
                                            int DP) {
@@ -193,13 +157,13 @@ ple_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_rows, const __grid
           for (int gp = 0; gp < GP / PC; ++gp)
             for (int kb = 0; kb < nk; ++kb) {
               const Ring::Slot slot = ring.acquire(SBYTES);
-              load_stage(sbase + slot.stage * SBYTES, &tmap_rows, q.E * HP + gp * PC, kb, R, slot.full);
+              load_ks_stage<HC>(sbase + slot.stage * SBYTES, &tmap_rows, q.E * HP + gp * PC, kb, R, slot.full);
             }
           for (int j = j_beg; j < j_end; ++j)
             for (int e = 0; e < q.E; ++e)
               for (int kb = 0; kb < nk; ++kb) {
                 const Ring::Slot slot = ring.acquire(SBYTES);
-                load_stage(sbase + slot.stage * SBYTES, &tmap_rows, e * HP + j * PC, kb, R, slot.full);
+                load_ks_stage<HC>(sbase + slot.stage * SBYTES, &tmap_rows, e * HP + j * PC, kb, R, slot.full);
               }
         }
       }))
@@ -218,7 +182,7 @@ ple_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_rows, const __grid
     consumers_bar();
     for (int gp = 0; gp < GP / PC; ++gp) {
       float z[HC / 2];
-      gemm_ks(z, xs, ldx, nk, r0, t, lane, wg, ring, sbase);
+      gemm_ks<HC>(z, xs, ldx, nk, r0, t, lane, wg, ring, sbase);
 #pragma unroll
       for (int k = 0; k < HC / 2; ++k) {
         const int col = gp * PC + wg * HC + 8 * (k >> 2) + 2 * t + (k & 1), r = r0 + 8 * ((k >> 1) & 1);
@@ -246,7 +210,7 @@ ple_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_rows, const __grid
         for (int k = 0; k < HC / 2; ++k) acc[o][k] = 0.f;
       for (int e = 0; e < q.E; ++e) {
         float a[HC / 2];
-        gemm_ks(a, xs, ldx, nk, r0, t, lane, wg, ring, sbase);
+        gemm_ks<HC>(a, xs, ldx, nk, r0, t, lane, wg, ring, sbase);
         float pe[MAX_T][2];
 #pragma unroll
         for (int o = 0; o < MAX_T; ++o) {
@@ -301,7 +265,7 @@ ple_bwd_dz_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_rows, const __g
             for (int j = 0; j < NJ; ++j)
               for (int kb = 0; kb < nk; ++kb) {
                 const Ring::Slot slot = ring.acquire(SBYTES);
-                load_stage(sbase + slot.stage * SBYTES, &tmap_rows, e * HP + j * PC, kb, R, slot.full);
+                load_ks_stage<HC>(sbase + slot.stage * SBYTES, &tmap_rows, e * HP + j * PC, kb, R, slot.full);
               }
       }))
     return;
@@ -327,7 +291,7 @@ ple_bwd_dz_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_rows, const __g
       }
       for (int j = 0; j < NJ; ++j) {
         float a[HC / 2];
-        gemm_ks(a, xs, ldx, nk, r0, t, lane, wg, ring, sbase);
+        gemm_ks<HC>(a, xs, ldx, nk, r0, t, lane, wg, ring, sbase);
         float gh[HC / 2];
 #pragma unroll
         for (int k = 0; k < HC / 2; ++k) {    // h_e, and h_e > 0 exactly where a_e > 0

@@ -1,7 +1,7 @@
 // wgmma / TMA / mbarrier PTX wrappers shared by the tensor-core kernels (sm_90a), the pipeline mechanics built on them
 // (shared-memory alignment, the mbarrier ring, the producer / consumer role split, the 3xTF32 k-step, accumulation chains,
 // the consumer loop of the batch-reduction weight-gradient GEMMs, the one weight-gradient kernel of the dense layers built
-// on it, the row-chunk GEMMs of the dense-layer kernels) and the host side of a tensor-core launch (workspace check,
+// on it, the row-chunk and K-sliced row GEMMs of the dense-layer kernels) and the host side of a tensor-core launch (workspace check,
 // tensor-map encoding, batch slices, ring depth and launch of the weight-gradient kernels).
 #pragma once
 #include <cuda.h>
@@ -513,6 +513,51 @@ __device__ __forceinline__ void stage_rows(float* dst, const float* __restrict__
       v = (mask == nullptr || __ldg(mask + o) > 0.f) ? __ldg(src + o) : 0.f;
     }
     dst[r * LD + c] = v;
+  }
+}
+
+// K-sliced row GEMMs over inputs up to 512 wide (PLE, DCN-V2): both warpgroups read the same staged rows, and a ring stage
+// holds [2 NW units x 32 inputs] (hi tile, then lo tile), of which warpgroup wg takes units wg NW .. wg NW + NW - 1.  The
+// ring depth does not depend on the input width.
+template <int NW>
+__host__ __device__ constexpr int ks_stage_bytes() { return 2 * 2 * NW * KB * 4; }
+
+// TMA loads of one stage: units u0 .. u0 + 2 NW - 1, inputs 32 kb .., hi then lo, from a [2 NP][KP] map (boxes of
+// [2 NW x 32]; the lo copy starts NP rows on).
+template <int NW>
+__device__ __forceinline__ void load_ks_stage(uint32_t dst, const CUtensorMap* map, int u0, int kb, int NP, uint32_t bar) {
+  tma_load_2d(dst, map, kb * KB, u0, bar);
+  tma_load_2d(dst + 2 * NW * 128, map, kb * KB, NP + u0, bar);
+}
+
+// D[64 x NW] = X[64 x 32 nk] . B over the next nk ring stages: X = the tile's staged rows (pitch ldx), B = this warpgroup's
+// NW-unit half of each stage.  One 32-input slice (4 k-steps) per stage, each drained into d on its own: the tensor core
+// truncates as it accumulates, and with 96-MMA chains PLE's widest inputs missed the fp32 bars by up to 1.2x (the softmax
+// turns a gate logit's absolute error into the gate's relative error).
+template <int NW>
+__device__ __forceinline__ void gemm_ks(float (&d)[NW / 2], const float* xs, int ldx, int nk, int r0, int t, int lane,
+                                        int wg, Ring& ring, uint32_t sbase) {
+  float dacc[NW / 2];
+#pragma unroll
+  for (int q = 0; q < NW / 2; ++q) { d[q] = 0.f; dacc[q] = 0.f; }
+  for (int kb = 0; kb < nk; ++kb) {
+    const uint32_t st = sbase + ring.wait() * ks_stage_bytes<NW>() + wg * NW * 128;
+    const uint64_t bhi = gmma_desc_kmajor(st, 128), blo = gmma_desc_kmajor(st + 2 * NW * 128, 128);
+    uint32_t ah[4][4], al[4][4];
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) {
+      float a[4];
+#pragma unroll
+      for (int q = 0; q < 4; ++q) a[q] = xs[(r0 + 8 * (q & 1)) * ldx + kb * KB + 8 * ks + t + 4 * (q >> 1)];
+      tf32_split(a, ah[ks], al[ks]);
+    }
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) mma_3xtf32<NW>(dacc, ah[ks], al[ks], bhi, blo, (uint64_t)(2 * ks), ks == 0 ? 0 : 1);
+    wgmma_commit();
+    wgmma_wait_keep(ah, al);
+    ring.release(lane);
+    chain_drain(d, dacc);
   }
 }
 

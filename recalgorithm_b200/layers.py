@@ -135,6 +135,51 @@ def cross_network(x0: torch.Tensor, num_cross_layer: int) -> torch.Tensor:
     return autograd.cross_stack(x0, w, b)
 
 
+def _cross_v2_variables(dimension: int, index, projection_dim):
+    with variable_scope(f"cross_v2_{index}"):
+        if projection_dim is None:
+            w, u = get_variable("kernel", (dimension, dimension)), None
+        else:
+            w = get_variable("kernel_v", (dimension, projection_dim))
+            u = get_variable("kernel_u", (projection_dim, dimension))
+        b = get_variable("bias", (dimension,), initializer=lambda s: torch.zeros(s))
+    return w, u, b
+
+
+def _projection_dim(projection_dim):
+    if projection_dim is None:
+        return None
+    r = int(projection_dim)
+    if r < 1:
+        raise ValueError(f"projection_dim must be at least 1 (None selects the full-rank layer), got {projection_dim!r}")
+    return r
+
+
+def cross_layer_v2(x0: torch.Tensor, xl: torch.Tensor, index: int, projection_dim=None) -> torch.Tensor:
+    """One DCN-V2 cross layer (Wang et al., WWW 2021, arXiv:2008.13535, eq. 1-2), same call shape as cross_layer:
+    ``x0 * (xl . W + bias) + xl`` with W = ``kernel`` (d, d), or at low rank W = ``kernel_v . kernel_u``.
+
+    The reference tree has no DCN-V2 code, so the variable names are this project's choice: in the caller's scope, a scope
+    ``cross_v2_{index}`` holding ``kernel`` (d, d) -- or, when ``projection_dim`` r is given, ``kernel_v`` (d, r) and
+    ``kernel_u`` (r, d), the paper's V and U^T -- all glorot-uniform, and ``bias`` (d,) zeros.  ``projection_dim`` goes
+    through ``int()`` (a string width works)."""
+    r = _projection_dim(projection_dim)
+    w, u, b = _cross_v2_variables(int(x0.shape[-1]), index, r)
+    return autograd.cross_v2(x0, w[None], None if u is None else u[None], b[None], r or 0, xl=None if xl is x0 else xl)
+
+
+def cross_network_v2(x0: torch.Tensor, num_cross_layer, projection_dim=None) -> torch.Tensor:
+    """``for i: x = cross_layer_v2(x0, x, i, projection_dim)`` over ``num_cross_layer`` layers in one call each way; creates
+    exactly the variables the loop would create.  ``num_cross_layer = 0`` returns x0 and launches nothing."""
+    n, r = int(num_cross_layer), _projection_dim(projection_dim)
+    if n == 0:
+        return x0
+    vs = [_cross_v2_variables(int(x0.shape[-1]), i, r) for i in range(n)]
+    w = torch.stack([v[0] for v in vs])
+    u = None if r is None else torch.stack([v[1] for v in vs])
+    return autograd.cross_v2(x0, w, u, torch.stack([v[2] for v in vs]), r or 0)
+
+
 # --------------------------------------------------------------------------------------------------- xDeepFM
 def cin_layer(x0: torch.Tensor, xk: torch.Tensor, hk_1, index: int, return_pooled: bool = False):
     """xdeepfm CIN layer -- same signature as xDeepFM/cin_layer.py:4.  x0 (B,m,D), xk (B,hk,D) -> (B,hk_1,D).

@@ -321,6 +321,73 @@ def cross_bwd(x0, w, b, g_out, xl_in=None):
     return dx0, dxl, dw, db
 
 
+# ------------------------------------------------------------------ Row CROSS-V2
+def _cross_v2_bytes(B: int, d: int, L: int, rank: int) -> Tuple[int, int]:
+    ws, sv = ctypes.c_int64(0), ctypes.c_int64(0)
+    _lib.check(_lib.lib().ctr_cross_v2_workspace_bytes(B, d, L, rank, ctypes.byref(ws), ctypes.byref(sv)))
+    return int(ws.value), int(sv.value)
+
+
+def cross_v2_workspace(B: int, d: int, L: int, rank: int, device) -> Tuple[torch.Tensor, int]:
+    """(workspace, saved_bytes): the caller-owned workspace for batch B (B = 0: the prepped weights, what the forward needs;
+    B: also the backward's rows) and the bytes of the `saved` buffer the forward fills for the backward at batch B."""
+    ws, sv = _cross_v2_bytes(B, d, L, rank)
+    return torch.empty((ws,), dtype=torch.uint8, device=device), sv
+
+
+def _cross_v2_args(x0, w, u, b, rank, xl_in):
+    _chk(x0, F32, "x0")
+    if x0.dim() != 2 or w.dim() != 3:
+        raise ValueError("cross_v2: x0 (B,d) and w (L,d,d) or (L,d,rank) expected")
+    B, d = x0.shape
+    L, rank = w.shape[0], int(rank)
+    _chk(w, F32, "w", (L, d, rank if rank else d)); _chk(b, F32, "b", (L, d)); _chk(xl_in, F32, "xl_in", (B, d))
+    if rank:
+        if u is None:
+            raise ValueError("cross_v2: u (L,rank,d) is required at rank >= 1")
+        _chk(u, F32, "u", (L, rank, d))
+    return B, d, L, rank
+
+
+def _saved_check(saved, nbytes):
+    _chk(saved, torch.uint8, "saved")
+    if saved.numel() < nbytes:
+        raise ValueError(f"saved: {nbytes} bytes required, got {saved.numel()}")
+
+
+def cross_v2_fwd(x0, w, u, b, rank: int, xl_in=None, saved=None, want_saved: bool = True):
+    """DCN-V2 cross network (arXiv:2008.13535 eq. 1-2): x_{l+1} = x0 * (x_l . W_l + b_l) + x_l, W_l = w[l] (rank 0, w (L,d,d))
+    or w[l] . u[l] (w (L,d,rank), u (L,rank,d)), x_0 = xl_in or x0.  Returns (x_L (B,d), saved): `saved` (uint8, given or
+    allocated when want_saved) holds what cross_v2_bwd reads; None when not wanted."""
+    B, d, L, rank = _cross_v2_args(x0, w, u, b, rank, xl_in)
+    ws, _ = cross_v2_workspace(0, d, L, rank, x0.device)
+    nbytes = _cross_v2_bytes(B, d, L, rank)[1]
+    if saved is None and want_saved:
+        saved = torch.empty((nbytes,), dtype=torch.uint8, device=x0.device)
+    if saved is not None:
+        _saved_check(saved, nbytes)
+    out = torch.empty_like(x0)
+    _lib.check(_lib.lib().ctr_cross_v2_fwd(_ptr(x0), _ptr(xl_in), _ptr(w), _ptr(u if rank else None), _ptr(b), B, d, L, rank,
+                                           _ptr(out), _ptr(saved), _ptr(ws), ws.numel(), _stream()))
+    return out, saved
+
+
+def cross_v2_bwd(x0, w, u, b, rank: int, saved, g_out, xl_in=None):
+    """Gradients of cross_v2_fwd given its `saved` and g_out (B,d): (dx0, dxl_in | None, dw, du | None, db)."""
+    B, d, L, rank = _cross_v2_args(x0, w, u, b, rank, xl_in)
+    _chk(g_out, F32, "g_out", (B, d))
+    ws, nbytes = cross_v2_workspace(B, d, L, rank, x0.device)
+    _saved_check(saved, nbytes)
+    dx0 = torch.empty_like(x0)
+    dxl = torch.empty_like(x0) if xl_in is not None else None
+    dw, db = torch.empty_like(w), torch.empty_like(b)
+    du = torch.empty_like(u) if rank else None
+    _lib.check(_lib.lib().ctr_cross_v2_bwd(_ptr(x0), _ptr(xl_in), _ptr(w), _ptr(u if rank else None), _ptr(b), _ptr(saved),
+                                           _ptr(g_out), B, d, L, rank, _ptr(dx0), _ptr(dxl), _ptr(dw), _ptr(du), _ptr(db),
+                                           _ptr(ws), ws.numel(), _stream()))
+    return dx0, dxl, dw, du, db
+
+
 # ------------------------------------------------------------------ Row DIN-ATT
 def _din_params(H, w1, b1, w2, b2, w3, b3):
     w3 = w3.reshape(32)

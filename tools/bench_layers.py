@@ -4,7 +4,7 @@
 Each kernel is timed alone with CUDA events; an L2 flush (a 256 MB write) runs between timed iterations because these
 working sets are flushed from the 50 MB L2.  Prints one JSON line per measurement.
 
-    python tools/bench_layers.py [--iters 20] [--only cin,dcn,din,fibinet]     (also: pairwise, bst, adam, pnn, dien, dien_aux, deepcrossing, mmoe, ple, wide, autoint, flen)
+    python tools/bench_layers.py [--iters 20] [--only cin,dcn,din,fibinet]     (also: pairwise, bst, adam, pnn, dien, dien_aux, deepcrossing, mmoe, ple, wide, autoint, flen, dcnv2)
 """
 import argparse
 import json
@@ -599,6 +599,66 @@ def autoint_rows(iters, flush, rn):
         torch.backends.cuda.matmul.allow_tf32 = prev_tf32
 
 
+def dcnv2_rows(iters, flush, rn):
+    """DCN-V2 cross network (ctr_cross_v2_fwd / _bwd, L = 3) at DCN config 2's width d = 480, full rank and rank 120 and
+    64, B = 4096 and 65 536, and at the reference DCN's width d = 82.  Each row is timed next to plain torch running the
+    same stack: fp32 matmuls with TF32 off, autograd for the backward.  Algorithmic FLOPs per layer: 2 B d^2 (full rank) or
+    4 B d r (low rank) forward, twice that backward (dx and the weight gradients).  Floors from data-sheet rates of the H100
+    SXM (700 W), not measured: 3 x FLOPs (3xTF32) over 495 TFLOP/s, and bytes over 3.35 TB/s (forward x0, out and the
+    saved x_l, z_l, t_l; backward x0, g_out, the saved tensors and dx0)."""
+    print(json.dumps({"dcnv2_card": card()}), flush=True)
+    L = 3
+
+    def torch_form(x0, w, u, b):
+        x = x0
+        for l in range(L):
+            z = (x @ w[l] if u is None else (x @ w[l]) @ u[l]) + b[l]
+            x = x0 * z + x
+        return x
+
+    prev_tf32 = torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cuda.matmul.allow_tf32 = False
+    try:
+        shapes = [(480, r, B) for B in (4096, 65536) for r in (0, 120, 64)] + [(82, 0, B) for B in (4096, 65536)]
+        for d, r, B in shapes:
+            w = rn(L, d, r or d, std=(0.25 / d) ** 0.5)
+            u = rn(L, r, d, std=(0.25 / r) ** 0.5) if r else None
+            b, x0, g = rn(L, d, std=0.3), rn(B, d), rn(B, d)
+            cfg = {"B": B, "d": d, "L": L, "rank": r}
+            gemm = 2.0 * B * d * (2 * r if r else d) * L
+            saved = 4.0 * B * ((2 * L - 1) * d + L * r)
+            flops = {"fwd": gemm, "bwd": 2 * gemm}
+            hbm = {"fwd": 4.0 * B * 2 * d + saved, "bwd": 4.0 * B * 3 * d + saved}
+            out, sv = ops.cross_v2_fwd(x0, w, u, b, r)
+            ps = [t.clone().requires_grad_() for t in (x0, w, u, b) if t is not None]
+            pu = ps[2] if r else None
+            ref_out = torch_form(ps[0], ps[1], pu, ps[-1])
+            grads = [t for t in ops.cross_v2_bwd(x0, w, u, b, r, sv, g) if t is not None]
+            ref_grads = torch.autograd.grad(ref_out, ps, g, retain_graph=True)
+            diff = {"fwd": float((ref_out.detach() - out).abs().max() / ref_out.detach().abs().max()),
+                    "bwd": max(float((a - c).abs().max() / c.abs().max()) for a, c in zip(grads, ref_grads))}
+            del grads, ref_grads
+            runs = {"fwd": (lambda: ops.cross_v2_fwd(x0, w, u, b, r, saved=sv), lambda: torch_form(x0, w, u, b)),
+                    "bwd": (lambda: ops.cross_v2_bwd(x0, w, u, b, r, sv, g),
+                            lambda: torch.autograd.grad(ref_out, ps, g, retain_graph=True))}
+            for way in ("fwd", "bwd"):
+                m, bst = timeit(runs[way][0], iters, flush)
+                tm, tbst = timeit(runs[way][1], iters, flush)
+                f_tc, f_hbm = 3 * flops[way] / 495e12 * 1e6, hbm[way] / 3.35e12 * 1e6
+                print(json.dumps({
+                    "kernel": f"cross_v2_{way}", "config": cfg, "ms_median": m, "ms_best": bst,
+                    "torch_fp32_ms_median": tm, "torch_fp32_ms_best": tbst, "speedup_vs_torch": tm / m,
+                    "max_norm_rel_diff_vs_torch": diff[way], "l2": "flushed between iterations",
+                    "algorithmic_TFLOPs": flops[way] / (m * 1e-3) / 1e12, "algorithmic_GBps": hbm[way] / (m * 1e-3) / 1e9,
+                    "floor_3xtf32_us": f_tc, "floor_fp32_us": flops[way] / 67e12 * 1e6, "floor_hbm_us": f_hbm,
+                    "bound": "tensor" if f_tc >= f_hbm else "hbm", "floor_over_kernel": max(f_tc, f_hbm) / (m * 1e3),
+                    "note": "floors are data-sheet rates (H100 SXM, 700 W), not measured; torch: same stack, fp32, TF32 off"}),
+                    flush=True)
+            del out, sv, ps, ref_out
+    finally:
+        torch.backends.cuda.matmul.allow_tf32 = prev_tf32
+
+
 def flen_rows(iters, flush, rn, gen):
     """FLEN field-wise bi-interaction (ctr_embed_fwbi_fwd / ctr_fwbi_fwd / ctr_fwbi_bwd) at the config-5 tile shape F = 40,
     D = 32 with M = 3 and 8 groups, B = 4 096 and 65 536, over a 40 x 250 000-row table (1.28 GB, far above the 50 MB L2).
@@ -857,6 +917,8 @@ def main():
         autoint_rows(args.iters, flush, rn)
     if "flen" in only:  # FLEN field-wise bi-interaction at F = 40, D = 32, M = 3 / 8, beside embed_bi and plain torch; not in the default list
         flen_rows(args.iters, flush, rn, gen)
+    if "dcnv2" in only:  # DCN-V2 cross network, L = 3, at d = 480 (full rank, r = 120, 64) and d = 82; not in the default list
+        dcnv2_rows(args.iters, flush, rn)
 
 
 if __name__ == "__main__" and "--configs" not in sys.argv:

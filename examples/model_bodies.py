@@ -54,16 +54,22 @@ def dcn_logit(dense_input: torch.Tensor, category_input: torch.Tensor, num_cross
 
 
 def dcn_v2_logit(dense_input: torch.Tensor, category_input: torch.Tensor, num_cross_layer: int = 3, projection_dim=None,
-                 structure: str = "stacked", hidden_units=(64, 32)):
+                 structure: str = "stacked", hidden_units=(64, 32), num_experts=None):
     """DCN-V2 (Wang et al., WWW 2021, arXiv:2008.13535) in dcn_logit's scopes: the cross network (layers.cross_network_v2,
     full rank or rank projection_dim) in cross_part.  ``structure="stacked"`` feeds the cross output to the deep part and
     the logit reads the deep output (the paper's Figure 1b); ``"parallel"`` runs the deep part on concat_all and the logit
-    reads both, concatenated, like DCN/dcn.py:167-169 (Figure 1a)."""
+    reads both, concatenated, like DCN/dcn.py:167-169 (Figure 1a).  With ``num_experts``, the cross part is DCN-Mix
+    instead (layers.cross_network_mix, that many experts of rank projection_dim, tanh)."""
     if structure not in ("stacked", "parallel"):
         raise ValueError(f"structure must be 'stacked' or 'parallel', got {structure!r}")
+    if num_experts is not None and projection_dim is None:
+        raise ValueError("num_experts needs projection_dim, the rank of each expert")
     concat_all = torch.cat([dense_input, category_input], dim=-1)
     with L.variable_scope("cross_part"):
-        cross_vec = L.cross_network_v2(concat_all, num_cross_layer, projection_dim)
+        if num_experts is None:
+            cross_vec = L.cross_network_v2(concat_all, num_cross_layer, projection_dim)
+        else:
+            cross_vec = L.cross_network_mix(concat_all, num_cross_layer, num_experts, low_rank=projection_dim)
     with L.variable_scope("dnn_part"):
         dnn_vec = cross_vec if structure == "stacked" else concat_all
         for i, unit in enumerate(hidden_units):

@@ -303,6 +303,37 @@ int ctr_cross_v2_bwd(const float* x0, const float* xl_in, const float* w, const 
                      const float* g_out, int64_t B, int64_t d, int64_t L, int64_t rank, float* dx0, float* dxl_in,
                      float* dw, float* du, float* db, void* workspace, int64_t workspace_bytes, void* stream);
 
+/* ---- Row CROSS-MIX: DCN-Mix cross network (mixture of low-rank cross experts) ---------------------------------
+ * DCN-Mix (Wang et al., WWW 2021, arXiv:2008.13535, eq. 3-4), the paper's mixture of K low-rank experts per cross layer.
+ * The reference tree has no DCN-Mix code, so this row follows the paper and is checked against a float64 restatement of
+ * it.  Row-vector form, l = 0 .. L-1, experts i = 1 .. K, x_0 = x0, g = tanh (activation 1) or the identity (0):
+ *   q_i = x_l . v[l,i],  t_i = g(q_i),  m_i = t_i . c[l,i],  c~_i = g(m_i)     v (L,K,d,r) (the paper's V_i^l),
+ *                                                                             c (L,K,r,r) (the paper's (C_i^l)^T);
+ *   p = softmax_i(x_l . gate) (max subtracted)                                gate (d,K), no bias, shared by all layers;
+ *   z_l = sum_i p_i c~_i . u[l,i] + b[l],  x_{l+1} = x0 * z_l + x_l           u (L,K,r,d) (the paper's (U_i^l)^T), b (L,d);
+ *   out (B,d) = x_L.  The paper's sum_i p_i (x0 * (c~_i u_i + b)) is this, since sum_i p_i = 1.
+ * With K = 1, the identity and c = I, the layer is row CROSS-V2's low-rank layer (w = v[:,0], u = u[:,0]).
+ * fp32-class accuracy (3xTF32 on the tensor cores).  1 <= d <= 512, 1 <= L <= 8, 1 <= K <= 16, r >= 1, K*r <= 128
+ * (CTR_ERR_UNSUPPORTED otherwise); rows need no alignment; B = 0 launches nothing.  The entries never allocate or
+ * synchronise.
+ * saved: caller-owned, ctr_cross_mix_workspace_bytes' saved_bytes = B * ((2L - 1) d + L (2 K r + K)) * 4 bytes: the layer
+ *   inputs x_1 .. x_{L-1} (L-1, B, d), then z_0 .. z_{L-1} (L, B, d), then t (L, B, K r), c~ (L, B, K r) and p (L, B, K),
+ *   experts side by side.  The forward writes it and the backward reads it.  A forward-only caller may pass saved = NULL
+ *   (the layers then run in place in out).
+ * workspace: 128-byte aligned, at least the workspace_bytes of ctr_cross_mix_workspace_bytes(0, ..) for the forward (the
+ *   prepped tf32 weight copies) and of ctr_cross_mix_workspace_bytes(B, ..) for the backward (also its per-sample rows).
+ * The backward takes g_out = dL/dout (B,d).  dx0 (B,d) receives every use of x0.  dv, dc, du, db and dgate are
+ *   overwritten (zeros at B = 0; batch-reduced with fp32 atomics); dgate sums over the layers. */
+int ctr_cross_mix_workspace_bytes(int64_t B, int64_t d, int64_t L, int64_t K, int64_t r, int64_t* workspace_bytes,
+                                  int64_t* saved_bytes);
+int ctr_cross_mix_fwd(const float* x0, const float* v, const float* c, const float* u, const float* b, const float* gate,
+                      int64_t B, int64_t d, int64_t L, int64_t K, int64_t r, int activation, float* out, void* saved,
+                      void* workspace, int64_t workspace_bytes, void* stream);
+int ctr_cross_mix_bwd(const float* x0, const float* v, const float* c, const float* u, const float* b, const float* gate,
+                      const void* saved, const float* g_out, int64_t B, int64_t d, int64_t L, int64_t K, int64_t r,
+                      int activation, float* dx0, float* dv, float* dc, float* du, float* db, float* dgate, void* workspace,
+                      int64_t workspace_bytes, void* stream);
+
 /* ---- Row CIN: xDeepFM compressed-interaction layer -------------------------------------------------
  * Replaces cin_layer(x0, xk, hk_1, index) (xDeepFM/cin_layer.py:17-30):
  *   out[b,n,d] = sum_{i,j} xk[b,i,d] * x0[b,j,d] * filter[i*m + j, n]

@@ -85,6 +85,9 @@ SIGNATURES = {
     "ctr_cross_v2_workspace_bytes": (c_int, [_I, _I, _I, _I, POINTER(c_int64), POINTER(c_int64)]),
     "ctr_cross_v2_fwd": (c_int, [_P] * 5 + [_I] * 4 + [_P, _P, _P, _I, _P]),
     "ctr_cross_v2_bwd": (c_int, [_P] * 7 + [_I] * 4 + [_P] * 6 + [_I, _P]),
+    "ctr_cross_mix_workspace_bytes": (c_int, [_I] * 5 + [POINTER(c_int64), POINTER(c_int64)]),
+    "ctr_cross_mix_fwd": (c_int, [_P] * 6 + [_I] * 5 + [c_int, _P, _P, _P, _I, _P]),
+    "ctr_cross_mix_bwd": (c_int, [_P] * 8 + [_I] * 5 + [c_int] + [_P] * 7 + [_I, _P]),
     "ctr_cin_fwd_workspace_bytes": (c_int64, [_I, _I, _I, _I, _I]),
     "ctr_cin_fwd": (c_int, [_P, _P, _P, _I, _I, _I, _I, _I, _P, _P, c_int, _P, _I, _P]),
     "ctr_cin_bwd": (c_int, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _P, _P, _P, _P, _I, _P]),

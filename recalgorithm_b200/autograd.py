@@ -199,6 +199,28 @@ def cross_v2(x0: torch.Tensor, w: torch.Tensor, u: Optional[torch.Tensor], b: to
     return _CrossV2.apply(x0, xl, w, u, b, int(rank))
 
 
+class _CrossMix(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x0, v, c, u, b, gate, activation):
+        x0, v, c, u, b, gate = (t.contiguous() for t in (x0, v, c, u, b, gate))
+        out, saved = ops.cross_mix_fwd(x0, v, c, u, b, gate, activation)
+        ctx.save_for_backward(x0, v, c, u, b, gate, saved)    # saved: x_1 .. x_{L-1}, z_l, t, c~ and p
+        ctx.activation = activation
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        x0, v, c, u, b, gate, saved = ctx.saved_tensors
+        return (*ops.cross_mix_bwd(x0, v, c, u, b, gate, saved, g.contiguous(), ctx.activation), None)
+
+
+def cross_mix(x0: torch.Tensor, v: torch.Tensor, c: torch.Tensor, u: torch.Tensor, b: torch.Tensor, gate: torch.Tensor,
+              activation="tanh") -> torch.Tensor:
+    """All L DCN-Mix cross layers (mixtures of K low-rank experts) in one forward and one backward call: v (L,K,d,r),
+    c (L,K,r,r), u (L,K,r,d), b (L,d), gate (d,K) shared by the layers; activation "tanh" or "identity"."""
+    return _CrossMix.apply(x0, v, c, u, b, gate, activation)
+
+
 class _LookupCross(torch.autograd.Function):
     @staticmethod
     def forward(ctx, anchor, tables: EmbeddingTables, ids, w, b):

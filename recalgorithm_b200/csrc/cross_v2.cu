@@ -44,13 +44,10 @@ constexpr int SBYTES = ks_stage_bytes<NW>();
 constexpr int MAX_D = 512, MAX_L = 8, MAX_R = 128;
 constexpr int SU = 16;                       // staging: elements per thread loaded before they are stored
 
-// the epilogue of a GEMM (see the file header)
-enum Epilogue { EPI_STORE = 0, EPI_FWD = 1, EPI_BWD = 2 };
-
 // One launch: A rows (B, lda) [o a_mul], columns < ka, zero padded to the first GEMM's width, times the operand(s).  The
 // pointers x_l / out may alias (a forward without `saved` runs in place with nsplit = 1), so none is __restrict__ and the
 // rows are read with ordinary loads.
-struct Args {
+struct Args {                                // the epilogue fields as tc_ptx.cuh's cross_epilogue reads them
   const float* a;
   const float* a_mul;        // A = a o a_mul (dz = g o x0), or null
   float* a_copy;             // the staged A rows (pitch: the first GEMM's KP) written out by each tile's first CTA, or null
@@ -91,53 +88,6 @@ __global__ void cross_v2_prep_kernel(const float* __restrict__ src, float* __res
     const float hi = tf32_rna(v);
     dst[idx] = hi;                            // hi | lo, with lo rounded to tf32 too (the tensor core would truncate it)
     dst[total + idx] = tf32_rna(v - hi);
-  }
-}
-
-// The epilogue of one slice for this thread's accumulator (rows r0, r0 + 8 of the tile, columns c0 + 8 c + e).  Every
-// operand is loaded before the first store: the pointers may alias, so a load would otherwise wait for each store before
-// it, one memory latency per element.
-__device__ __forceinline__ void epilogue(const Args& p, const float (&acc)[NW / 2], long long base, int r0, int c0) {
-  if (p.epi == EPI_STORE) {
-#pragma unroll
-    for (int k = 0; k < NW / 2; ++k) {
-      const int col = c0 + 8 * (k >> 2) + (k & 1);
-      const long long row = base + r0 + 8 * ((k >> 1) & 1);
-      if (row < p.B && col < p.ldy) p.y[(size_t)row * p.ldy + col] = acc[k];
-    }
-    return;
-  }
-  const bool fwd = p.epi == EPI_FWD;
-  float u0[NW / 2], u1[NW / 2], u2[NW / 2];  // FWD: x0, x_l, b;  BWD: g, z, the old dx0
-#pragma unroll
-  for (int k = 0; k < NW / 2; ++k) {
-    const int col = c0 + 8 * (k >> 2) + (k & 1);
-    const long long row = base + r0 + 8 * ((k >> 1) & 1);
-    u0[k] = u1[k] = u2[k] = 0.f;
-    if (row < p.B && col < p.d) {
-      const size_t o = (size_t)row * p.d + col;
-      u0[k] = fwd ? p.x0[o] : p.g[o];
-      u1[k] = fwd ? p.xl[o] : p.z[o];
-      u2[k] = fwd ? __ldg(p.bias + col) : p.dx0_accumulate ? p.dx0[o] : 0.f;
-    }
-  }
-#pragma unroll
-  for (int k = 0; k < NW / 2; ++k) {
-    const int col = c0 + 8 * (k >> 2) + (k & 1);
-    const long long row = base + r0 + 8 * ((k >> 1) & 1);
-    if (row >= p.B || col >= p.d) continue;
-    const size_t o = (size_t)row * p.d + col;
-    if (fwd) {
-      const float z = acc[k] + u2[k];
-      if (p.z_out != nullptr) p.z_out[o] = z;
-      p.y[o] = u0[k] * z + u1[k];
-    } else {
-      const float dx = u0[k] + acc[k];
-      float d0 = u0[k] * u1[k];
-      if (p.dx0_add_dx) d0 += dx;
-      else if (p.y != nullptr) p.y[o] = dx;
-      p.dx0[o] = p.dx0_accumulate ? u2[k] + d0 : d0;
-    }
   }
 }
 
@@ -216,7 +166,7 @@ cross_v2_rows_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_pre, const _
     for (int s = s_beg; s < s_end; ++s) {
       float acc[NW / 2];
       gemm_ks<NW>(acc, xs, ld, p.KP / KB, r0, t, lane, wg, ring, sbase);
-      epilogue(p, acc, base, r0, s * SLICE + wg * NW + 2 * t);
+      cross_epilogue<NW>(p, acc, base, r0, s * SLICE + wg * NW + 2 * t);
     }
     consumers_bar();                          // the rows may be restaged once every thread has read them
   }

@@ -1,7 +1,7 @@
 // wgmma / TMA / mbarrier PTX wrappers shared by the tensor-core kernels (sm_90a), the pipeline mechanics built on them
 // (shared-memory alignment, the mbarrier ring, the producer / consumer role split, the 3xTF32 k-step, accumulation chains,
 // the consumer loop of the batch-reduction weight-gradient GEMMs, the one weight-gradient kernel of the dense layers built
-// on it, the row-chunk and K-sliced row GEMMs of the dense-layer kernels) and the host side of a tensor-core launch (workspace check,
+// on it, the row-chunk and K-sliced row GEMMs of the dense-layer kernels and the cross-network epilogue) and the host side of a tensor-core launch (workspace check,
 // tensor-map encoding, batch slices, ring depth and launch of the weight-gradient kernels).
 #pragma once
 #include <cuda.h>
@@ -558,6 +558,59 @@ __device__ __forceinline__ void gemm_ks(float (&d)[NW / 2], const float* xs, int
     wgmma_wait_keep(ah, al);
     ring.release(lane);
     chain_drain(d, dacc);
+  }
+}
+
+// The epilogue of a cross-network K-sliced row GEMM slice (DCN-V2, DCN-Mix) for this thread's gemm_ks<NW> accumulator
+// (rows r0, r0 + 8 of the 64-sample tile at `base`, columns c0 + 8 c + e).  The layer's Args type names the fields read here:
+//   EPI_STORE  y (B, ldy) = acc;
+//   EPI_FWD    z = acc + bias, x_{l+1} = x0 o z + xl into y, z into z_out (or not);
+//   EPI_BWD    dx_l = g + acc into y (or nothing), dx0 (+)= g o z (+ dx_l with dx0_add_dx).
+// Every operand is loaded before the first store: the pointers may alias, so a load would otherwise wait for each store
+// before it, one memory latency per element.
+enum CrossEpilogue { EPI_STORE = 0, EPI_FWD = 1, EPI_BWD = 2 };
+template <int NW, class Args>
+__device__ __forceinline__ void cross_epilogue(const Args& p, const float (&acc)[NW / 2], long long base, int r0, int c0) {
+  if (p.epi == EPI_STORE) {
+#pragma unroll
+    for (int k = 0; k < NW / 2; ++k) {
+      const int col = c0 + 8 * (k >> 2) + (k & 1);
+      const long long row = base + r0 + 8 * ((k >> 1) & 1);
+      if (row < p.B && col < p.ldy) p.y[(size_t)row * p.ldy + col] = acc[k];
+    }
+    return;
+  }
+  const bool fwd = p.epi == EPI_FWD;
+  float u0[NW / 2], u1[NW / 2], u2[NW / 2];  // FWD: x0, x_l, b;  BWD: g, z, the old dx0
+#pragma unroll
+  for (int k = 0; k < NW / 2; ++k) {
+    const int col = c0 + 8 * (k >> 2) + (k & 1);
+    const long long row = base + r0 + 8 * ((k >> 1) & 1);
+    u0[k] = u1[k] = u2[k] = 0.f;
+    if (row < p.B && col < p.d) {
+      const size_t o = (size_t)row * p.d + col;
+      u0[k] = fwd ? p.x0[o] : p.g[o];
+      u1[k] = fwd ? p.xl[o] : p.z[o];
+      u2[k] = fwd ? __ldg(p.bias + col) : p.dx0_accumulate ? p.dx0[o] : 0.f;
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < NW / 2; ++k) {
+    const int col = c0 + 8 * (k >> 2) + (k & 1);
+    const long long row = base + r0 + 8 * ((k >> 1) & 1);
+    if (row >= p.B || col >= p.d) continue;
+    const size_t o = (size_t)row * p.d + col;
+    if (fwd) {
+      const float z = acc[k] + u2[k];
+      if (p.z_out != nullptr) p.z_out[o] = z;
+      p.y[o] = u0[k] * z + u1[k];
+    } else {
+      const float dx = u0[k] + acc[k];
+      float d0 = u0[k] * u1[k];
+      if (p.dx0_add_dx) d0 += dx;
+      else if (p.y != nullptr) p.y[o] = dx;
+      p.dx0[o] = p.dx0_accumulate ? u2[k] + d0 : d0;
+    }
   }
 }
 

@@ -180,6 +180,46 @@ def cross_network_v2(x0: torch.Tensor, num_cross_layer, projection_dim=None) -> 
     return autograd.cross_v2(x0, w, u, torch.stack([v[2] for v in vs]), r or 0)
 
 
+_MIX_ACTIVATIONS = ("tanh", "identity")
+
+
+def cross_network_mix(x0: torch.Tensor, num_cross_layer, num_experts=4, low_rank=32, activation="tanh") -> torch.Tensor:
+    """DCN-Mix cross network (Wang et al., WWW 2021, arXiv:2008.13535, eq. 3-4): ``num_cross_layer`` layers, each a
+    softmax-gated mixture of ``num_experts`` low-rank experts, ``x_{l+1} = x0 * (sum_i p_i g(g(x_l V_i) C_i) U_i + bias)
+    + x_l`` with ``p = softmax(x_l gate)`` and g = tanh (``activation="tanh"``) or the identity, in one call each way.
+
+    The reference tree has no DCN-Mix code, so the variable names are this project's choice: in the caller's scope,
+    ``cross_mix_{l}/expert_{i}/kernel_v`` (d, r), ``kernel_c`` (r, r) and ``kernel_u`` (r, d) -- the paper's V_i, C_i^T and
+    U_i^T, one 2-D variable per expert matrix so that glorot-uniform sees its own fans -- and ``cross_mix_{l}/bias`` (d,)
+    zeros; the paper's gates carry no layer index, so one ``cross_mix_gates/kernel`` (d, K), glorot-uniform, serves every
+    layer.  The integer arguments go through ``int()``; ``num_cross_layer = 0`` returns x0 with no variable and no launch."""
+    n, K, r = int(num_cross_layer), int(num_experts), int(low_rank)
+    if activation not in _MIX_ACTIVATIONS:
+        raise ValueError(f"activation must be one of {_MIX_ACTIVATIONS}, got {activation!r}")
+    if n < 0:
+        raise ValueError(f"num_cross_layer must be at least 0, got {num_cross_layer!r}")
+    if K < 1 or r < 1:
+        raise ValueError(f"num_experts and low_rank must be at least 1, got {num_experts!r} and {low_rank!r}")
+    if K > 16 or K * r > 128:
+        raise ValueError(f"num_experts must be at most 16 and num_experts * low_rank at most 128, got {K} * {r}")
+    if n == 0:
+        return x0
+    d = int(x0.shape[-1])
+    vs, cs, us, bs = [], [], [], []
+    for l in range(n):
+        with variable_scope(f"cross_mix_{l}"):
+            for i in range(K):
+                with variable_scope(f"expert_{i}"):
+                    vs.append(get_variable("kernel_v", (d, r)))
+                    cs.append(get_variable("kernel_c", (r, r)))
+                    us.append(get_variable("kernel_u", (r, d)))
+            bs.append(get_variable("bias", (d,), initializer=lambda s: torch.zeros(s)))
+    with variable_scope("cross_mix_gates"):
+        gate = get_variable("kernel", (d, K))
+    stack = lambda ts, *shape: torch.stack(ts).reshape(n, K, *shape)
+    return autograd.cross_mix(x0, stack(vs, d, r), stack(cs, r, r), stack(us, r, d), torch.stack(bs), gate, activation)
+
+
 # --------------------------------------------------------------------------------------------------- xDeepFM
 def cin_layer(x0: torch.Tensor, xk: torch.Tensor, hk_1, index: int, return_pooled: bool = False):
     """xdeepfm CIN layer -- same signature as xDeepFM/cin_layer.py:4.  x0 (B,m,D), xk (B,hk,D) -> (B,hk_1,D).

@@ -388,6 +388,76 @@ def cross_v2_bwd(x0, w, u, b, rank: int, saved, g_out, xl_in=None):
     return dx0, dxl, dw, du, db
 
 
+# ------------------------------------------------------------------ Row CROSS-MIX
+_ACTIVATIONS = {"tanh": 1, "identity": 0}
+
+
+def _cross_mix_bytes(B: int, d: int, L: int, K: int, r: int) -> Tuple[int, int]:
+    ws, sv = ctypes.c_int64(0), ctypes.c_int64(0)
+    _lib.check(_lib.lib().ctr_cross_mix_workspace_bytes(B, d, L, K, r, ctypes.byref(ws), ctypes.byref(sv)))
+    return int(ws.value), int(sv.value)
+
+
+def cross_mix_workspace(B: int, d: int, L: int, K: int, r: int, device) -> Tuple[torch.Tensor, int]:
+    """(workspace, saved_bytes): the caller-owned workspace for batch B (B = 0: the prepped weights, what the forward needs;
+    B: also the backward's rows) and the bytes of the `saved` buffer the forward fills for the backward at batch B."""
+    ws, sv = _cross_mix_bytes(B, d, L, K, r)
+    return torch.empty((ws,), dtype=torch.uint8, device=device), sv
+
+
+def _activation_code(activation) -> int:
+    if activation in _ACTIVATIONS:
+        return _ACTIVATIONS[activation]
+    if activation in (0, 1) and not isinstance(activation, bool):
+        return int(activation)
+    raise ValueError(f"activation must be 'tanh' (1) or 'identity' (0), got {activation!r}")
+
+
+def _cross_mix_args(x0, v, c, u, b, gate):
+    _chk(x0, F32, "x0")
+    if x0.dim() != 2 or v.dim() != 4:
+        raise ValueError("cross_mix: x0 (B,d) and v (L,K,d,r) expected")
+    B, d = x0.shape
+    L, K, _, r = v.shape
+    _chk(v, F32, "v", (L, K, d, r)); _chk(c, F32, "c", (L, K, r, r)); _chk(u, F32, "u", (L, K, r, d))
+    _chk(b, F32, "b", (L, d)); _chk(gate, F32, "gate", (d, K))
+    return B, d, L, K, r
+
+
+def cross_mix_fwd(x0, v, c, u, b, gate, activation="tanh", saved=None, want_saved: bool = True):
+    """DCN-Mix cross network (arXiv:2008.13535 eq. 3-4): x_{l+1} = x0 * (sum_i p_i g(g(x_l . v[l,i]) . c[l,i]) . u[l,i]
+    + b[l]) + x_l with p = softmax(x_l . gate), g = tanh or the identity.  v (L,K,d,r), c (L,K,r,r), u (L,K,r,d), b (L,d),
+    gate (d,K).  Returns (x_L (B,d), saved): `saved` (uint8, given or allocated when want_saved) holds what cross_mix_bwd
+    reads; None when not wanted."""
+    B, d, L, K, r = _cross_mix_args(x0, v, c, u, b, gate)
+    act = _activation_code(activation)
+    ws, _ = cross_mix_workspace(0, d, L, K, r, x0.device)
+    nbytes = _cross_mix_bytes(B, d, L, K, r)[1]
+    if saved is None and want_saved:
+        saved = torch.empty((nbytes,), dtype=torch.uint8, device=x0.device)
+    if saved is not None:
+        _saved_check(saved, nbytes)
+    out = torch.empty_like(x0)
+    _lib.check(_lib.lib().ctr_cross_mix_fwd(_ptr(x0), _ptr(v), _ptr(c), _ptr(u), _ptr(b), _ptr(gate), B, d, L, K, r, act,
+                                            _ptr(out), _ptr(saved), _ptr(ws), ws.numel(), _stream()))
+    return out, saved
+
+
+def cross_mix_bwd(x0, v, c, u, b, gate, saved, g_out, activation="tanh"):
+    """Gradients of cross_mix_fwd given its `saved` and g_out (B,d): (dx0, dv, dc, du, db, dgate)."""
+    B, d, L, K, r = _cross_mix_args(x0, v, c, u, b, gate)
+    act = _activation_code(activation)
+    _chk(g_out, F32, "g_out", (B, d))
+    ws, nbytes = cross_mix_workspace(B, d, L, K, r, x0.device)
+    _saved_check(saved, nbytes)
+    dx0 = torch.empty_like(x0)
+    dv, dc, du, db, dgate = (torch.empty_like(t) for t in (v, c, u, b, gate))
+    _lib.check(_lib.lib().ctr_cross_mix_bwd(_ptr(x0), _ptr(v), _ptr(c), _ptr(u), _ptr(b), _ptr(gate), _ptr(saved),
+                                            _ptr(g_out), B, d, L, K, r, act, _ptr(dx0), _ptr(dv), _ptr(dc), _ptr(du),
+                                            _ptr(db), _ptr(dgate), _ptr(ws), ws.numel(), _stream()))
+    return dx0, dv, dc, du, db, dgate
+
+
 # ------------------------------------------------------------------ Row DIN-ATT
 def _din_params(H, w1, b1, w2, b2, w3, b3):
     w3 = w3.reshape(32)

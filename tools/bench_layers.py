@@ -4,7 +4,7 @@
 Each kernel is timed alone with CUDA events; an L2 flush (a 256 MB write) runs between timed iterations because these
 working sets are flushed from the 50 MB L2.  Prints one JSON line per measurement.
 
-    python tools/bench_layers.py [--iters 20] [--only cin,dcn,din,fibinet]     (also: pairwise, bst, adam, pnn, dien, dien_aux, deepcrossing, mmoe, ple, wide, autoint, flen, dcnv2)
+    python tools/bench_layers.py [--iters 20] [--only cin,dcn,din,fibinet]     (also: pairwise, bst, adam, pnn, dien, dien_aux, deepcrossing, mmoe, ple, wide, autoint, flen, dcnv2, dcnmix)
 """
 import argparse
 import json
@@ -659,6 +659,87 @@ def dcnv2_rows(iters, flush, rn):
         torch.backends.cuda.matmul.allow_tf32 = prev_tf32
 
 
+def dcnmix_rows(iters, flush, rn):
+    """DCN-Mix cross network (ctr_cross_mix_fwd / _bwd, L = 3, tanh) at DCN config 2's width d = 480 with K = 4 experts of
+    rank 32 and K = 8 of rank 16, and at the reference DCN's width d = 82 with K = 4, r = 32; B = 4096 and 65 536.  Each
+    row is timed next to plain torch running the same layers, fp32 matmuls with TF32 off and autograd for the backward, in
+    two forms: the collapsed one the kernels compute (one matmul per GEMM, the experts side by side, an einsum for c) and
+    the paper's per-expert loop.  Algorithmic FLOPs per layer forward: 2 B (2 d K r + K r^2 + d K); backward twice that.
+    Floors from data-sheet rates of the H100 SXM (700 W), not measured: 3 x FLOPs (3xTF32) over 495 TFLOP/s, FLOPs over
+    the 67 TFLOP/s FP32 rate, and bytes over 3.35 TB/s (forward x0, out and the saved x_l, z_l, t, c~, p; backward x0,
+    g_out, the saved tensors and dx0)."""
+    print(json.dumps({"dcnmix_card": card()}), flush=True)
+    L = 3
+
+    def collapsed(x0, v, c, u, b, gate):
+        _, K, d, r = v.shape
+        x = x0
+        for l in range(L):
+            p = torch.softmax(x @ gate, dim=1)
+            t = torch.tanh(x @ v[l].permute(1, 0, 2).reshape(d, K * r)).view(-1, K, r)
+            ct = torch.tanh(torch.einsum("bkr,krs->bks", t, c[l]))
+            x = x0 * ((p[:, :, None] * ct).reshape(-1, K * r) @ u[l].reshape(K * r, d) + b[l]) + x
+        return x
+
+    def per_expert(x0, v, c, u, b, gate):
+        K = v.shape[1]
+        x = x0
+        for l in range(L):
+            p = torch.softmax(x @ gate, dim=1)
+            y = x
+            for i in range(K):
+                y = y + p[:, i:i + 1] * (x0 * (torch.tanh(torch.tanh(x @ v[l, i]) @ c[l, i]) @ u[l, i] + b[l]))
+            x = y
+        return x
+
+    prev_tf32 = torch.backends.cuda.matmul.allow_tf32
+    torch.backends.cuda.matmul.allow_tf32 = False
+    try:
+        shapes = [(d, K, r, B) for d, K, r in ((480, 4, 32), (480, 8, 16), (82, 4, 32)) for B in (4096, 65536)]
+        for d, K, r, B in shapes:
+            v, c = rn(L, K, d, r, std=(1.0 / d) ** 0.5), rn(L, K, r, r, std=(1.0 / r) ** 0.5)
+            u, gate = rn(L, K, r, d, std=(0.25 / r) ** 0.5), rn(d, K, std=(1.0 / d) ** 0.5)
+            b, x0, g = rn(L, d, std=0.3), rn(B, d), rn(B, d)
+            w = (v, c, u, b, gate)
+            cfg = {"B": B, "d": d, "L": L, "K": K, "r": r, "activation": "tanh"}
+            KR = K * r
+            fwd = 2.0 * B * (2 * d * KR + K * r * r + d * K) * L
+            saved = 4.0 * B * ((2 * L - 1) * d + L * (2 * KR + K))
+            flops = {"fwd": fwd, "bwd": 2 * fwd}
+            hbm = {"fwd": 4.0 * B * 2 * d + saved, "bwd": 4.0 * B * 3 * d + saved}
+            out, sv = ops.cross_mix_fwd(x0, *w)
+            grads = ops.cross_mix_bwd(x0, *w, sv, g)
+            ps = [t.clone().requires_grad_() for t in (x0, *w)]
+            ref = {"collapsed": collapsed(*ps), "per_expert": per_expert(*ps)}
+            diff = {}
+            for form, ro in ref.items():
+                rg = torch.autograd.grad(ro, ps, g, retain_graph=True)
+                diff[form] = {"fwd": float((ro.detach() - out).abs().max() / ro.detach().abs().max()),
+                              "bwd": max(float((a - c_).abs().max() / c_.abs().max()) for a, c_ in zip(grads, rg))}
+            del grads, rg
+            for way in ("fwd", "bwd"):
+                m, bst = timeit((lambda: ops.cross_mix_fwd(x0, *w, saved=sv)) if way == "fwd" else
+                                (lambda: ops.cross_mix_bwd(x0, *w, sv, g)), iters, flush)
+                line = {"kernel": f"cross_mix_{way}", "config": cfg, "ms_median": m, "ms_best": bst}
+                for form, fn in (("collapsed", collapsed), ("per_expert", per_expert)):
+                    tfn = ((lambda: fn(x0, *w)) if way == "fwd" else
+                           (lambda: torch.autograd.grad(ref[form], ps, g, retain_graph=True)))
+                    tm, _ = timeit(tfn, iters, flush)
+                    line.update({f"torch_{form}_ms_median": tm, f"speedup_vs_torch_{form}": tm / m,
+                                 f"max_norm_rel_diff_vs_torch_{form}": diff[form][way]})
+                f_tc, f_hbm = 3 * flops[way] / 495e12 * 1e6, hbm[way] / 3.35e12 * 1e6
+                line.update({
+                    "l2": "flushed between iterations",
+                    "algorithmic_TFLOPs": flops[way] / (m * 1e-3) / 1e12, "algorithmic_GBps": hbm[way] / (m * 1e-3) / 1e9,
+                    "floor_3xtf32_us": f_tc, "floor_fp32_us": flops[way] / 67e12 * 1e6, "floor_hbm_us": f_hbm,
+                    "bound": "tensor" if f_tc >= f_hbm else "hbm", "floor_over_kernel": max(f_tc, f_hbm) / (m * 1e3),
+                    "note": "floors are data-sheet rates (H100 SXM, 700 W), not measured; torch: same layers, fp32, TF32 off"})
+                print(json.dumps(line), flush=True)
+            del out, sv, ps, ref
+    finally:
+        torch.backends.cuda.matmul.allow_tf32 = prev_tf32
+
+
 def flen_rows(iters, flush, rn, gen):
     """FLEN field-wise bi-interaction (ctr_embed_fwbi_fwd / ctr_fwbi_fwd / ctr_fwbi_bwd) at the config-5 tile shape F = 40,
     D = 32 with M = 3 and 8 groups, B = 4 096 and 65 536, over a 40 x 250 000-row table (1.28 GB, far above the 50 MB L2).
@@ -919,6 +1000,8 @@ def main():
         flen_rows(args.iters, flush, rn, gen)
     if "dcnv2" in only:  # DCN-V2 cross network, L = 3, at d = 480 (full rank, r = 120, 64) and d = 82; not in the default list
         dcnv2_rows(args.iters, flush, rn)
+    if "dcnmix" in only:  # DCN-Mix cross network, L = 3, d = 480 (K, r = 4, 32 and 8, 16) and d = 82; not in the default list
+        dcnmix_rows(args.iters, flush, rn)
 
 
 if __name__ == "__main__" and "--configs" not in sys.argv:
